@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — pair-HMM GCUPS of the B200 engine on BASELINE.json's (reads x haplotypes) workload.
+"""bench.py — pair-HMM GCUPS of the H100 engine on BASELINE.json's (reads x haplotypes) workload.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C3] [--reads R] [--haps H]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C3] [--reads R] [--haps H] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 A step = one pass of the hot path (HaplotypeLikelihoodArray::populate semantics, one mapping position per pair, naive
@@ -11,6 +11,10 @@ cells per alignment = 2*(L+band)*band (simd_pair_hmm.hpp:271). Prints ONE JSON l
   value  device-resident inputs → device-resident double matrix (+ gather to rank 0 when N > 1), max over ranks
   e2e    the same call through the C ABI with pinned HOST buffers: H2D of the batch and D2H of the matrix inside the timed region
   roofline / cpu_baseline / clocks: see DESIGN.md "Measurement"
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float64): every region's
+[H, R] likelihood matrix, or a fixed seeded sample of its read columns (DIR/<name>_reads.npy) where the whole would exceed the
+size budget. The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -30,7 +34,7 @@ import numpy as np  # noqa: E402
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="C3", help="BASELINE config name (octopus_b200.synth.CONFIGS)")
@@ -60,7 +64,36 @@ def parse_args():
     ap.add_argument("--gather", choices=["peer", "nccl"], default="peer",
                     help="several ranks: how the values reach rank 0 — peer (each rank's epilogue stores into rank 0's HBM through a CUDA IPC mapping) or nccl (gather collective)")
     ap.add_argument("--error-model", default=None, help="haplotype penalty arrays from the reference's error models (reset()), e.g. PCR-free.HiSeq-2500, instead of i.i.d. draws")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's likelihood matrices (rank 0) as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    return args
+
+
+DUMP_BUDGET = 48 << 20      # bytes of all dumped arrays together (<= 64 MB)
+
+
+def dump_sample(out, budget):
+    """A fixed seeded sample of the read columns of one [H, R] (or flat) float64 result that fits `budget` bytes, taken on the
+    device. Returns (values, column indices or None when every column is kept)."""
+    import torch
+    m = out if out.dim() == 2 else out.view(1, -1)
+    cols = m.shape[1]
+    keep = max(1, budget // (8 * m.shape[0]))
+    if keep >= cols:
+        return m.clone(), None
+    idx = np.sort(np.random.default_rng(12345).choice(cols, size=keep, replace=False))
+    return m.index_select(1, torch.as_tensor(idx, device=m.device)), idx
+
+
+def write_dump(directory, captured):
+    os.makedirs(directory, exist_ok=True)
+    for k, (vals, idx) in enumerate(captured):
+        name = "likelihoods_%03d" % k
+        np.save(os.path.join(directory, name + ".npy"), vals.cpu().numpy().astype(np.float64))
+        if idx is not None:
+            np.save(os.path.join(directory, name + "_reads.npy"), idx.astype(np.float64))
 
 
 METRIC = "pair-HMM GCUPS (DP cell-updates/s)"
@@ -72,28 +105,28 @@ def peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
-def issue_roofline(kernel_gcups, reads, band, clocks, alu_ops):
+def issue_roofline(kernel_gcups, reads, band, clocks, alu_ops, sm_count):
     """The binding roofline of the packed DP (DESIGN.md section 4): `alu_ops` half-rate ALU-pipe instructions per cell pair (5 when
     gap_open >= gap_extend everywhere — the OGE deletion update — else 6) at 64 thread-instructions/clk/SM; beside it the issue
     bound of the steady-state loop (9.6 warp instructions per cell pair, SASS). Both in the reference's cell count 2(L+B)B per
     alignment (the column sweep itself touches 2LB cells)."""
     lens = np.diff(np.asarray(reads.off))
     mean_ratio = float(((lens + band) / lens).mean())
-    mhz = (clocks or {}).get("sm_mhz") or 1965.0
-    peak = 148 * mhz * 1e6 * (64.0 * 2.0 / alu_ops) * mean_ratio / 1e9
-    issue_peak = 148 * mhz * 1e6 * (4 * 64.0 / 9.6) * mean_ratio / 1e9
+    mhz = (clocks or {}).get("sm_mhz") or 1980.0           # H100 SXM maximum SM clock where nvidia-smi gave no sample
+    peak = sm_count * mhz * 1e6 * (64.0 * 2.0 / alu_ops) * mean_ratio / 1e9
+    issue_peak = sm_count * mhz * 1e6 * (4 * 64.0 / 9.6) * mean_ratio / 1e9
     return {"bound": "alu-pipe (DPX packed-16)", "achieved": kernel_gcups, "peak": peak, "unit": "GCUPS", "frac": kernel_gcups / peak,
-            "alu_instr_per_cell_pair": alu_ops, "alu_thread_instr_per_clk_per_sm": 64, "sm_mhz": mhz,
+            "alu_instr_per_cell_pair": alu_ops, "alu_thread_instr_per_clk_per_sm": 64, "sm_mhz": mhz, "sms": sm_count,
             "issue_peak": issue_peak, "issue_frac": kernel_gcups / issue_peak, "warp_instr_per_cell_pair": 9.6}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons / power limit during the timed region (read-only queries)."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
-        "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+        "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, index=0):
         self.index, self.proc, self.lines = index, None, []
@@ -119,20 +152,24 @@ class ClockSampler:
             self.proc.wait(timeout=5)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, plim, reasons = [], [], [], set()
         for ln in self.lines:
             f = [x.strip() for x in ln.split(",")]
-            if len(f) < 9:
+            if len(f) < 10:
                 continue
             try:
                 sm.append(float(f[1])); mx.append(float(f[2]))
             except ValueError:
                 continue
+            try:
+                plim.append(float(f[9]))
+            except ValueError:
+                pass
             for name, val in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[5:9]):
                 if val.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "power_limit_w": max(plim) if plim else None, "reasons": sorted(reasons), "samples": len(sm)}
 
 
 def host_threads():
@@ -249,17 +286,6 @@ def parity_gate(eng, haps, reads, band, flank_state, shortcut, mapit, int_scores
     rel = np.abs(got[ok] - want[ok]) / np.maximum(np.abs(want[ok]), 1e-300)
     return {"pairs": int(ok.sum()), "mismatches": int((rel > 1e-4).sum() + (st[~ok] != wst[~ok]).sum()),
             "against": "oracle populate in the same mode (C restatement pinned to the compiled reference), 1e-4 relative"}
-
-
-def measured_traffic(config, R, H, band, mode_key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed ncu --set full captures
-    (profiles/traffic.json, written by tools/ncu_traffic.py from the .ncu-rep files); None when this workload was never captured."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            t = json.load(f)
-        return t.get("%s:%d:%d:%d:%s" % (config, R, H, band, mode_key))
-    except Exception:
-        return None
 
 
 def workload_name(config, R, lens, H, hap_len, band):
@@ -380,7 +406,14 @@ def main():
     recv = None
     if world > 1 and rank == 0 and not strong and peer_ring is None:
         recv = [[torch.empty_like(d_out[0]) for _ in range(world)] for _ in range(n_buf)]
-    state = {"k": 0, "gather_ms": [], "launches": 0}
+    state = {"k": 0, "gather_ms": [], "launches": 0, "capture": None}
+
+    def capture(out):
+        """--dump-outputs: a sample of one result of the last timed step. The next region re-uses the buffer, so the sample is
+        complete before the call returns."""
+        if state["capture"] is not None:
+            state["capture"].append(dump_sample(out, DUMP_BUDGET // (1 if args.batch_regions else len(regions))))
+            torch.cuda.current_stream().synchronize()
 
     def one_region(dh, dr):
         k = state["k"]
@@ -394,6 +427,7 @@ def main():
             else:
                 out = peer_ring.window(k, rank * max_region_bytes, dh.n, dr.n)
             eng.populate(model_cfg, dh, dr, flank_state=flank_state, out=out)
+            capture(out)
             dp = eng.last_dp_kernel_ms()
             state["launches"] += eng.launch_count()
             g0 = torch.cuda.Event(enable_timing=True)
@@ -405,6 +439,7 @@ def main():
             eng.wait_event(gather_done[b])
         out = d_out[b] if (dh.n, dr.n) == (H, R) else None
         out = eng.populate(model_cfg, dh, dr, flank_state=flank_state, out=out)
+        capture(out)
         dp = eng.last_dp_kernel_ms()
         state["launches"] += eng.launch_count()
         if world > 1:
@@ -430,6 +465,7 @@ def main():
         if batched is not None:
             eng.populate_regions(model_cfg, batched[0], batched[1], batched[2], batched[3],
                                  flank_states=[flank_state] * len(regions) if flank_state else None, out=flat_out)
+            capture(flat_out)
             state["launches"] += eng.launch_count()
             return eng.last_dp_kernel_ms()
         return sum(one_region(dh, dr) for dh, dr in d_regions)
@@ -452,7 +488,11 @@ def main():
     state["launches"] = 0
     sync_all()
     ev0.record()
-    for _ in range(args.steps):
+    for s in range(args.steps):
+        # with --dump-outputs the last timed step keeps a device-side sample of every result it returns; a region's buffer is
+        # re-used by the next region, so the sample is taken on the stream before that
+        if s == args.steps - 1 and args.dump_outputs and rank == 0:
+            state["capture"] = []
         dp_ms.append(step())
     ev1.record()
     launches = state["launches"]
@@ -463,6 +503,9 @@ def main():
     total_ms = float(ms.item())
     gather_ms = float(np.mean([a.elapsed_time(b) for a, b in state["gather_ms"]])) if state["gather_ms"] else 0.0
     clocks = sampler.stop() if rank == 0 else None
+    if state["capture"] is not None:
+        write_dump(args.dump_outputs, state["capture"])
+        state["capture"] = None
 
     # Did every rank's values land on rank 0? Each rank recomputes its last region locally; rank 0 compares an order-independent bit
     # digest (int64 sum of the float64 bit patterns) of every rank's window of the last slot with that rank's own digest.
@@ -533,8 +576,7 @@ def main():
         alg_bytes = sum(4 * h.n * r.n + 2 * int(r.off[-1]) + 16 * int(h.off[-1]) for h, r in regions)
         peak, peak_src = peaks()
         achieved = alg_bytes / (kernel_ms / 1e3) / 1e9
-        mode_key = "flank" if flank_state else ("ref" if (args.shortcut or args.map) else "dp")
-        traffic = measured_traffic(args.config, R, H, band, mode_key)
+        props = torch.cuda.get_device_properties(dev)
         role_warps = band in (32, 64) and H >= 17 and not os.environ.get("PHMM_NO_ROLE_WARPS")     # the engine's own rule (populate_impl)
         flank_fb = band <= 16 and not args.int_scores and not os.environ.get("PHMM_NO_FLANK_FB")          # the engine's own rule (populate_impl)
         kernel_name = ("k_flank_fwd<%d> + k_flank_bwd<%d> (+ score-only and labelled flank kernels of the tile)" % (band, band)) if flank_state and flank_fb else \
@@ -551,7 +593,7 @@ def main():
                        "regions_per_rank_and_step": len(regions), "regions_per_call": len(regions) if args.batch_regions else 1,
                        "alignments_per_step": haps.n * R_total if strong else sum(h.n * r.n for h, r in regions) * world,
                        "cells_per_step": cells_rank_total,
-                       "l2": "inputs+outputs (%.0f MB) larger than the 126 MB L2" % ((h2d + d2h + 4 * H * R) / 1e6),
+                       "l2": "inputs+outputs %.0f MB, L2 %.0f MB" % ((h2d + d2h + 4 * H * R) / 1e6, props.L2_cache_size / 1e6),
                        "parallelism": ("one batch, reads split over %d rank(s), [H, R_total] matrix assembled on rank 0 (%s)" % (world, how)) if strong else
                                       ("every rank its own region(s), haplotypes per region, the per-rank matrices collected on rank 0 (%d rank(s), %s)" % (world, how)),
                        "gather": (None if world == 1 else ("peer" if peer_ring is not None else "nccl")), "gather_note": gather_note,
@@ -562,17 +604,19 @@ def main():
                        "mode": {"flank_state": flank_state, "naive_shortcut": bool(args.shortcut), "kmer_mapper": bool(args.map), "use_int_scores": bool(args.int_scores)}},
             "e2e": {"value": e2e, "unit": "GCUPS", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "ms_per_step": e2e_ms / args.steps},
             "gpu_launches": launches,
+            "device": {"name": props.name, "sms": props.multi_processor_count, "power_limit_w": (clocks or {}).get("power_limit_w")},
             "clocks": clocks,
             "gather_ms_per_region": gather_ms,
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "peak_source": peak_src, "kernel": kernel_name, "kernel_ms": kernel_ms,
                          "algorithmic_bytes_per_launch": alg_bytes,
                          "note": "the path is integer-issue bound, not HBM bound (SURVEY.md F3); see DESIGN.md for the issue-rate roofline",
                          "kernel_gcups": cells_rank / (kernel_ms / 1e3) / 1e9},
             # The binding roofline (DESIGN.md §4): the packed cell costs 5 (6 for unordered penalties) ALU-pipe instructions per 2 cells
-            # and the ALU pipe issues 64 thread-instructions/clk/SM (profiles/r01_ubench_int.txt).
+            # and the ALU pipe is modelled at 64 thread-instructions/clk/SM (4 sub-partitions x 16 lanes; not measured on H100).
             "issue_roofline": issue_roofline(cells_rank / (kernel_ms / 1e3) / 1e9, reads, band, clocks,
-                                             5 if all(bool((np.asarray(h.gap_open) >= np.asarray(h.gap_extend)).all()) for h, _ in regions) else 6),
+                                             5 if all(bool((np.asarray(h.gap_open) >= np.asarray(h.gap_extend)).all()) for h, _ in regions) else 6,
+                                             props.multi_processor_count),
         }
         ref_scores, n_ref = None, 0
         if not args.no_cpu_baseline:

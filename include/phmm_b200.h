@@ -1,5 +1,5 @@
 /*
- * phmm_b200.h — C ABI of the B200-native pair-HMM haplotype-likelihood engine.
+ * phmm_b200.h — C ABI of the H100-native (sm_90a) pair-HMM haplotype-likelihood engine.
  *
  * Drop-in boundary for ONE path of luntergroup/octopus (v0.7.4): the banded pair-HMM that scores every
  * (read, haplotype) pair and fills HaplotypeLikelihoodArray. The reference has no FFI layer; the seams this
@@ -20,7 +20,7 @@
  * and never throw — the C++ adapter (octopus_b200/cpp/phmm_b200.hpp) re-throws the reference's exceptions.
  * An engine handle is not re-entrant (one per host thread, like the reference's per-thread model copies,
  * haplotype_likelihood_array.cpp:172).
- * There is no CPU fallback: every entry point that computes fails with PHMM_ERR_CUDA when no B200 is usable.
+ * There is no CPU fallback: every entry point that computes fails with PHMM_ERR_CUDA when no H100 is usable.
  */
 #ifndef PHMM_B200_H
 #define PHMM_B200_H
@@ -139,7 +139,7 @@ const char* phmm_last_error(const phmm_engine* e);   /* valid until the next cal
 int         phmm_wait_event(phmm_engine* e, void* cuda_event);
 void*       phmm_engine_stream(phmm_engine* e);
 /* The persistent DP kernels occupy every SM; a collective the caller runs BESIDE the next call (the gather of the previous result) then
- * waits for them. n_sms > 0 keeps the first n_sms SMs free of DP blocks (cost: n_sms / 148 of the DP throughput); 0 (default) = none. */
+ * waits for them. n_sms > 0 keeps the first n_sms SMs free of DP blocks (cost: n_sms / SM count of the DP throughput; 132 SMs on an H100 SXM); 0 (default) = none. */
 int         phmm_reserve_sms(phmm_engine* e, int n_sms);
 
 /* Page-locked host memory (cudaHostAlloc) for callers that do not link the CUDA runtime themselves: host-space calls on pinned
@@ -209,7 +209,7 @@ int phmm_populate(phmm_engine* e, const phmm_config* cfg,
 
 /* Many regions in one call. Octopus runs populate once per ACTIVE REGION (Caller::call_variants, core/callers/caller.cpp:445-531 →
  * compute_haplotype_likelihoods :1159-1196): a few to a few hundred haplotypes x some hundred to some thousand reads — far too small
- * to fill a B200 (one such call is launch-latency bound). Here region g owns the haplotypes [hap_first[g], hap_first[g+1]) and the
+ * to fill an H100 (one such call is launch-latency bound). Here region g owns the haplotypes [hap_first[g], hap_first[g+1]) and the
  * reads [read_first[g], read_first[g+1]) of the two blocks; every read is scored against the haplotypes of its own region only, all
  * regions in ONE kernel chain. The region arrays live in HOST memory whatever `space` says (they are tiny and the host sizes the
  * call from them). */

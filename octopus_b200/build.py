@@ -1,4 +1,4 @@
-"""Builds the CUDA extension in-tree: octopus_b200/libphmm_b200.so (sm_100a only, nvcc cross-compiles without a GPU)."""
+"""Builds the CUDA extension in-tree: octopus_b200/libphmm_b200.so (sm_90a only, nvcc cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB = os.path.join(_HERE, "libphmm_b200.so")
 SOURCES = ["phmm_engine.cu", "phmm_error_model.cpp"]
 DEPS = ["phmm_engine.cu", "phmm_kernels.cuh", "phmm_device.cuh", "phmm_error_model.cpp", "phmm_error_model_tables.inc", os.path.join("..", "..", "include", "phmm_b200.h")]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]
 
 
@@ -27,7 +27,7 @@ def _stale(target, deps):
 
 
 def build(force=False, verbose=False):
-    deps = [os.path.join(CSRC, d) for d in DEPS]
+    deps = [os.path.join(CSRC, d) for d in DEPS] + [__file__]    # a change of the flags here rebuilds too
     if not force and not _stale(LIB, deps):
         return LIB
     if not all(os.path.exists(os.path.join(CSRC, s)) for s in SOURCES):
@@ -44,9 +44,9 @@ def build_cpu_emulation(force=False):
     root = os.path.dirname(_HERE)
     src = os.path.join(root, "tests", "cpu_emul", "emul.cu")
     out = os.path.join(root, "tests", "cpu_emul", "libphmm_emul.so")
-    if not force and not _stale(out, [src, os.path.join(CSRC, "phmm_device.cuh")]):
+    if not force and not _stale(out, [src, os.path.join(CSRC, "phmm_device.cuh"), __file__]):
         return out
-    subprocess.run([_nvcc(), "-O2", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC",
+    subprocess.run([_nvcc(), "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
                     "-shared", "-o", out, src], check=True)
     return out
 

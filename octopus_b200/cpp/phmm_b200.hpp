@@ -151,7 +151,7 @@ public:
 
     explicit GpuPairHMM(Engine engine = Engine {}) : engine_ {std::move(engine)} {}
 
-    constexpr static const char* name() noexcept { return "B200"; }
+    constexpr static const char* name() noexcept { return "H100"; }
     constexpr static int band_size() noexcept { return BandSize; }
 
     // score only, no SNV model (simd_pair_hmm.hpp:438-452)
@@ -544,7 +544,7 @@ public:
         for (int b = 8; b <= 256; b <<= 1) if (min_band_size <= static_cast<unsigned>(b)) { band_ = b; return; }
         throw TooLargeBandSizeError {min_band_size};
     }
-    constexpr static const char* name() noexcept { return "B200"; }
+    constexpr static const char* name() noexcept { return "H100"; }
     int band_size() const noexcept { return band_; }
     template <typename GapExtend>
     int align(const char* truth, const char* target, const std::int8_t* qualities, int truth_len, int target_len,

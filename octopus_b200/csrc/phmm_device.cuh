@@ -1,7 +1,7 @@
-// Device-side building blocks of the B200 pair-HMM engine (sm_100a).
+// Device-side building blocks of the H100 pair-HMM engine (sm_90a).
 //
 // Recurrence: the integer min-plus banded DP of the reference kernel
-//   /root/reference/src/core/models/pairhmm/simd_pair_hmm.hpp:240-324 (align_helper)
+//   src/core/models/pairhmm/simd_pair_hmm.hpp:240-324 (align_helper)
 // restated in (x, y) prefix coordinates (x truth-window bases, y read bases consumed; band 0 <= x-y <= 2B-1):
 //   S          = min(m, i, d)                                    (:284, :308)
 //   m(x+1,y+1) = S + sub(x, y)                                   (:121-132 update_match_state)
@@ -14,7 +14,7 @@
 // The implementations that live here:
 //   * dp_pair<BAND>  — the fast path. One THREAD owns TWO alignments packed as s16x2 in every register and sweeps
 //     the band column by column (x outer, diagonal k = x-y unrolled in registers). No shuffles, no shared-memory
-//     DP state. The per-cell work is 10 integer instructions for 2 cells using Blackwell's DPX packed-16 ops
+//     DP state. The per-cell work is 10 integer instructions for 2 cells using the DPX packed-16 ops Hopper introduced
 //     (VIMNMX3.S16x2, VIADDMNMX.S16x2, VIMNMX.S16x2) and PRMT byte-table lookups for the emission.
 //   * dp_band / dp_band_roles — the same cell with the band's diagonals split over lanes or warps (bands 32 ... 256, 32-bit lanes).
 //   * dp_flank_fwd / dp_flank_bwd / fb_finish — the flank-aware path, packed: forward pass to the flank boundary, backward pass
@@ -55,7 +55,7 @@ constexpr int      kMaxScore16 = 0x7000 - 1024;  // a read whose sum of qualitie
 __host__ __device__ inline int base_code(char c) { return c == 'A' ? 0 : c == 'C' ? 1 : c == 'G' ? 2 : c == 'T' ? 3 : c == 'N' ? 4 : -1; }
 
 // The DP cores are __host__ __device__ so that tests/ can run the very same code on the CPU (with the few
-// sm_100a instructions emulated below) against the CPU checker without a GPU. The product library never calls the
+// sm_90a instructions emulated below) against the CPU checker without a GPU. The product library never calls the
 // host instantiations: every exported entry point launches kernels.
 #define PHMM_HD __host__ __device__ __forceinline__
 

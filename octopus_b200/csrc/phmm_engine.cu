@@ -1,4 +1,4 @@
-// C ABI of the B200 pair-HMM engine (include/phmm_b200.h): host-side orchestration only. All arithmetic of the
+// C ABI of the H100 pair-HMM engine (include/phmm_b200.h): host-side orchestration only. All arithmetic of the
 // hot path runs in the kernels of phmm_kernels.cuh; there is no CPU fallback — without a usable GPU every
 // computing entry point returns PHMM_ERR_CUDA.
 #include "../../include/phmm_b200.h"
@@ -49,7 +49,7 @@ int round_band(int requested)
 
 struct phmm_engine {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int reserved_sms = 0;       // phmm_reserve_sms
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -283,7 +283,7 @@ int blocks_per_sm_of(phmm_engine* e, F kernel, int threads, size_t smem, int* ou
 
 extern "C" {
 
-const char* phmm_version(void) { return "octopus_b200 phmm 0.1 (sm_100a)"; }
+const char* phmm_version(void) { return "octopus_b200 phmm 0.1 (sm_90a)"; }
 
 void phmm_default_config(phmm_config* c)
 {
@@ -316,8 +316,8 @@ int phmm_create(phmm_engine** out, int device)
     if (cudaSetDevice(device) != cudaSuccess) { g_create_error = "cudaSetDevice failed"; return PHMM_ERR_CUDA; }
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { g_create_error = "cudaGetDeviceProperties failed"; return PHMM_ERR_CUDA; }
-    if (prop.major < 10) {
-        g_create_error = "this library is built for sm_100a (B200) only; found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {   // sm_90a code loads on compute capability 9.0 only
+        g_create_error = "this library is built for sm_90a (H100) only; found compute capability " + std::to_string(prop.major) + "." + std::to_string(prop.minor);
         return PHMM_ERR_CUDA;
     }
     phmm_engine* e = new phmm_engine();

@@ -1,8 +1,8 @@
-// HaplotypeLikelihoodModel::reset for the B200 pair-HMM engine: the per-haplotype penalty arrays the kernels consume
+// HaplotypeLikelihoodModel::reset for the H100 pair-HMM engine: the per-haplotype penalty arrays the kernels consume
 // (SNV mask / prior per strand, gap_open[], gap_extend[]) from the haplotype sequence alone. Host C++, one haplotype per
 // task, bit-identical to the reference's error models so that the engine can be fed from sequences directly.
 //
-// Reference (paths under /root/reference/):
+// Reference (paths in the octopus source tree):
 //   src/core/models/haplotype_likelihood_model.cpp:60-78            reset: which model fills which array; the no-SNV-model default
 //   src/core/models/error/repeat_based_indel_error_model.cpp:67-83  per-base open / extend penalties from exact tandem repeats (period 1..5)
 //   src/core/models/error/basic_repeat_based_indel_error_model.cpp:51-103   penalty lookup by motif period and repeat count

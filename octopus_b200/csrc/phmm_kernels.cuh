@@ -1,4 +1,4 @@
-// Kernels of the B200 pair-HMM engine. See phmm_device.cuh for the DP cores and DESIGN.md for the data layout.
+// Kernels of the H100 pair-HMM engine. See phmm_device.cuh for the DP cores and DESIGN.md for the data layout.
 #pragma once
 
 #include "phmm_device.cuh"
@@ -459,7 +459,7 @@ __device__ __forceinline__ void split_index(const long long i, const int H, int*
 
 // Persistent DP kernels fill every SM's register file; a collective (NCCL gather of the previous result) launched beside them finds no
 // SM to run on until they finish. With reserved_sms > 0 the blocks that land on the first SMs exit at once (the work queue is dynamic:
-// the others take it all), which leaves those SMs to the collective at a cost of reserved / 148 of the DP throughput.
+// the others take it all), which leaves those SMs to the collective at a cost of reserved / (SM count: 132 on an H100 SXM) of the DP throughput.
 __device__ __forceinline__ bool on_reserved_sm(const PopParams& p)
 {
     if (p.reserved_sms <= 0) return false;
@@ -602,9 +602,9 @@ __global__ void k_build_kmer_table(const int H, const long long* __restrict__ of
 // CountT = uint8_t when no diagonal can collect more than 255 votes (one vote per query k-mer at most: reads of <= 260 bases),
 // else uint16_t. Haplotypes with more than MAXT k-mers are handled in tiles of MAXT diagonals, ascending, so the "first ten at the
 // maximum" order is kept (round 1 refused them).
-// Measured alternatives (profiles/README.md): round 1's haplotype-major bins (two dependent, uncoalesced L2 loads per k-mer) 6.4 ms per C2
-// step; a warp per pair with shared-memory vote tiles 13 ms (the per-pair latency chain is paid by every warp instead of being
-// spread over 32 pairs).
+// Rejected alternatives (both slower when measured; not re-measured on H100): round 1's haplotype-major bins (two dependent,
+// uncoalesced L2 loads per k-mer); a warp per pair with shared-memory vote tiles (the per-pair latency chain is paid by every warp
+// instead of being spread over 32 pairs).
 template <int MAXT, typename CountT>
 __global__ void k_kmer_map(const int* __restrict__ list, const int n_list_max, const SchedTotals* __restrict__ tot, const int base, const int kind,
                            const DevHaps hp, const DevReads rd,

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY — ctypes loaders for the two CPU oracles.
 
 * ``RefKernel``  — the UNMODIFIED reference SIMD kernel compiled into ``oracle/_ref/libref_phmm_<isa>.so``
-  (``oracle/ref_driver.cpp``, built by ``oracle/Makefile`` from /root/reference where it lies).
+  (``oracle/ref_driver.cpp``, built by ``oracle/Makefile`` from the reference checkout, see ``REFERENCE``).
 * ``RefHMM``     — the UNMODIFIED reference layer above the kernel (``hmm::evaluate`` / ``hmm::align`` / band choice) compiled
   into ``oracle/_ref/libref_hmm.so`` (``oracle/ref_hmm_driver.cpp``).
 * ``COracle``    — the plain-C restatement ``oracle/liboctopus_oracle.so`` (``oracle/phmm_oracle.c``).
@@ -17,6 +17,14 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 REF_DIR = os.path.join(_HERE, "_ref")
+# A source checkout of luntergroup/octopus: OCTOPUS_REFERENCE, else the build environment's standard location of it. Only where
+# one exists are the reference oracles compiled into oracle/_ref/; elsewhere the tests use what oracle/_ref/ already holds and the
+# fixtures under tests/golden/.
+REFERENCE = os.environ.get("OCTOPUS_REFERENCE") or "/root/reference"
+
+
+def have_reference():
+    return bool(REFERENCE) and os.path.isdir(os.path.join(REFERENCE, "src", "core", "models", "pairhmm"))
 
 _i8p = C.POINTER(C.c_int8)
 _i32p = C.POINTER(C.c_int32)
@@ -47,9 +55,10 @@ def available_ref_isas():
     return [i for i in out if os.path.exists(os.path.join(REF_DIR, "libref_phmm_%s.so" % i))]
 
 
-def build(ref=True, quiet=True):
-    """(Re)build the oracle libraries. The reference build only happens where /root/reference exists."""
-    target = ["all"] if ref else ["liboctopus_oracle.so"]
+def build(ref=None, quiet=True):
+    """(Re)build the oracle libraries. The reference build only happens where the reference checkout exists."""
+    ref = have_reference() if ref is None else ref and have_reference()
+    target = ["all", "REF=" + REFERENCE] if ref else ["liboctopus_oracle.so"]
     subprocess.run(["make", "-C", _HERE] + target, check=True,
                    stdout=subprocess.DEVNULL if quiet else None)
 
@@ -119,7 +128,7 @@ class RefKernel:
         isas = available_ref_isas()
         if isa is None:
             if not isas:
-                raise RuntimeError("no oracle/_ref library usable on this host (build with `make -C oracle` where /root/reference exists)")
+                raise RuntimeError("no oracle/_ref library usable on this host (build with `make -C oracle REF=<octopus checkout>`)")
             isa = isas[0]
         elif isa not in isas:
             raise RuntimeError("reference ISA build %r not available on this host (have %s)" % (isa, isas))

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — never linked into or called from the product path.
 //
 // extern "C" driver around the UNMODIFIED reference SIMD pair-HMM kernel. The reference sources are
-// compiled from where they lie under /root/reference (nothing is copied into this repo):
+// compiled from the octopus checkout named by REF (nothing is copied into this repo):
 //   src/core/models/pairhmm/simd_pair_hmm_factory.hpp  (selector, :55-130)
 //   src/core/models/pairhmm/simd_pair_hmm.hpp          (align_helper :240-324, flank replay :352-430)
 //   src/core/models/pairhmm/{sse2,avx2,avx512}_pair_hmm_impl.hpp, rolling_initializer.hpp

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY — the slice of the reference's basics/cigar_string.hpp that pair_hmm.hpp touches
 // (make_cigar, pair_hmm.hpp:152-188, 335): an operation is (length, SAM flag), a CIGAR is a vector of them.
-// The real header needs Boost; this one exists so that pair_hmm.hpp itself compiles unmodified from /root/reference.
+// The real header needs Boost; this one exists so that pair_hmm.hpp itself compiles unmodified from the reference checkout.
 #ifndef REF_SHIM_CIGAR_STRING_HPP
 #define REF_SHIM_CIGAR_STRING_HPP
 #include <cstdint>

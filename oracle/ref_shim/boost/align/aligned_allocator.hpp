@@ -1,5 +1,5 @@
 // Test-infrastructure stand-in for <boost/align/aligned_allocator.hpp> (Boost is not installed in
-// this image). Only what /root/reference/src/core/models/pairhmm/simd_pair_hmm.hpp:32 needs:
+// this image). Only what src/core/models/pairhmm/simd_pair_hmm.hpp:32 needs:
 // an allocator template usable with std::vector that returns storage aligned for SIMD vectors.
 #pragma once
 #include <cstddef>

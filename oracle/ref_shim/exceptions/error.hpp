@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY — a minimal octopus::Error family so that the UNMODIFIED reference headers pair_hmm.hpp (HMMOverflow
-// derives from ProgramError, :47-65) and simd_pair_hmm_wrapper.hpp (includes user_error.hpp) compile from /root/reference.
+// derives from ProgramError, :47-65) and simd_pair_hmm_wrapper.hpp (includes user_error.hpp) compile from the reference checkout.
 // The real exceptions/*.hpp pull in Octopus's config and Boost. All three classes live here; program_error.hpp and
 // user_error.hpp only forward to this file.
 #ifndef REF_SHIM_ERROR_HPP

@@ -9,13 +9,13 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with `pytest -m gpu` on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with `pytest -m gpu` on a GPU machine)")
 
 
 @pytest.fixture(scope="session")
 def coracle():
     from oracle.oracle import COracle, build
-    build(ref=os.path.isdir("/root/reference"))
+    build()
     return COracle()
 
 

@@ -1,9 +1,9 @@
 // The per-call seam, literally: the reference's OWN hmm::evaluate / hmm::align templates (src/core/models/pairhmm/pair_hmm.hpp:827-874,
-// compiled from /root/reference where it lies, Boost-free through oracle/ref_shim/) instantiated over octopus_b200::GpuPairHMM<Band>
+// compiled from the reference checkout, Boost-free through oracle/ref_shim/) instantiated over octopus_b200::GpuPairHMM<Band>
 // and over the reference's SIMD kernel, on the same seeded inputs. Every value must be identical: the GPU type is a drop-in
 // for the duck-typed PairHMM concept (band_size, name, 4 x align, calculate_flank_score).
 //
-// Built only where /root/reference exists (tests/test_gpu_cpp.py); the binary travels to the GPU box with the snapshot.
+// Built only where the reference checkout is given (tests/test_gpu_cpp.py), into oracle/_ref/ beside the other reference builds.
 #include <cstdint>
 #include <cstdio>
 #include <string>

@@ -1,5 +1,5 @@
 // TEST HELPER (not part of the product library): runs the engine's __host__ __device__ DP cores on the CPU, with the
-// sm_100a packed-16 instructions emulated (octopus_b200/csrc/phmm_device.cuh), so that `pytest -m "not gpu"` can check
+// sm_90a packed-16 (DPX) instructions emulated (octopus_b200/csrc/phmm_device.cuh), so that `pytest -m "not gpu"` can check
 // the very code the kernels execute against the oracle without a GPU.
 #include <cstdint>
 #include <vector>

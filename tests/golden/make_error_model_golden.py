@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generates tests/golden/error_model_golden.json from the UNMODIFIED reference error models + lib/tandem compiled here
-(oracle/_ref/libref_errmodel.so). Run in the container that has /root/reference; the JSON is committed."""
+(oracle/_ref/libref_errmodel.so). Run with OCTOPUS_REFERENCE set; the JSON is committed."""
 import json
 import os
 import sys
@@ -35,7 +35,7 @@ def main():
         cases.append(c)
     out = os.path.join(ROOT, "tests", "golden", "error_model_golden.json")
     with open(out, "w") as f:
-        json.dump({"source": "oracle/_ref/libref_errmodel.so (reference error models + lib/tandem, compiled from /root/reference)", "cases": cases}, f)
+        json.dump({"source": "oracle/_ref/libref_errmodel.so (reference error models + lib/tandem, compiled from the reference checkout)", "cases": cases}, f)
     print("wrote", out, len(cases), "cases")
 
 

@@ -2,20 +2,21 @@
 """Extract the reference's own known-answer tests for the raw pair-HMM kernel into a JSON fixture.
 
 Source (read at generation time only, never at test time):
-    /root/reference/test/unit/core/models/pair_hmm_tests.cpp
+    test/unit/core/models/pair_hmm_tests.cpp of the octopus tree
       TestCase  {target(=truth window), query(=read), base_qualities, gap_open[], gap_extend, nuc_prior}  (:22-28)
       Alignment {score, begin(=first_pos), target(=aligned truth), query(=aligned read)}                   (:30-35)
       sse2_band_size_{8,16,32}_check_alignments, avx2_check_alignments (band 16, short)                    (:203-712)
       band8_speed_test / band16_speed_test + expected alignments                                           (:104-199)
 
-Run (in the build container, where /root/reference exists):
+Run with OCTOPUS_REFERENCE naming an octopus checkout:
     python tests/golden/make_pair_hmm_kats.py > tests/golden/pair_hmm_kats.json
 """
 import json
+import os
 import re
 import sys
 
-SRC = "/root/reference/test/unit/core/models/pair_hmm_tests.cpp"
+SRC = os.path.join(os.environ.get("OCTOPUS_REFERENCE", "."), "test", "unit", "core", "models", "pair_hmm_tests.cpp")
 
 
 def _ints(body):

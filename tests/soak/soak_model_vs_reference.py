@@ -1,5 +1,5 @@
 """Long-running CPU soak (test infrastructure, not collected by pytest): oracle_model_evaluate against the reference's own HaplotypeLikelihoodModel (compiled from
-/root/reference, oracle/_ref/libref_hmm.so) on adversarial inputs: low-complexity and N-rich haplotypes, zero penalties,
+the reference checkout, oracle/_ref/libref_hmm.so) on adversarial inputs: low-complexity and N-rich haplotypes, zero penalties,
 qualities 0..93, reads with N, out-of-range positions, short haplotypes.
 
 usage: python tests/soak/soak_model_vs_reference.py [seed] [cases]

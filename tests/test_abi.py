@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a without a GPU, loads, exports every symbol include/phmm_b200.h declares, and
+"""The C-ABI library builds for sm_90a without a GPU, loads, exports every symbol include/phmm_b200.h declares, and
 refuses to compute without a GPU (no CPU fallback)."""
 import ctypes as C
 import os
@@ -21,9 +21,9 @@ def test_library_builds_and_exports_header_symbols():
     for name in declared:
         assert hasattr(lib, name), name
     assert lib.phmm_version().decode().startswith("octopus_b200")
-    # the library contains sm_100a code only
+    # the library contains sm_90a code only
     sass = subprocess.run(["cuobjdump", "-lelf", path], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass and "sm_90" not in sass and "sm_80" not in sass
+    assert "sm_90a" in sass and "sm_100" not in sass and "sm_80" not in sass
 
 
 def test_struct_layouts_match_header():

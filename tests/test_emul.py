@@ -1,5 +1,5 @@
 """The engine's __host__ __device__ DP cores (octopus_b200/csrc/phmm_device.cuh) executed on the CPU with the
-sm_100a packed-16 instructions emulated, checked against the oracle. This is the same source the kernels compile."""
+sm_90a packed-16 (DPX) instructions emulated, checked against the oracle. This is the same source the kernels compile."""
 import ctypes as C
 import os
 

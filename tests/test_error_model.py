@@ -1,5 +1,5 @@
 """HaplotypeLikelihoodModel::reset (SURVEY.md a11 / N2): the engine's own error models (octopus_b200/csrc/phmm_error_model.cpp, host C++
-inside libphmm_b200.so) against the UNMODIFIED reference models + lib/tandem compiled from /root/reference (oracle/_ref/libref_errmodel.so),
+inside libphmm_b200.so) against the UNMODIFIED reference models + lib/tandem compiled from the reference checkout (oracle/_ref/libref_errmodel.so),
 array for array — and against committed golden fixtures where the reference build is absent."""
 import json
 import os
@@ -32,10 +32,9 @@ def repeat_rich_sequence(rng, max_len=400):
 @pytest.fixture(scope="module")
 def ref():
     from oracle.oracle import RefErrorModel, build
-    if os.path.isdir("/root/reference"):
-        build(ref=True)
+    build()
     if not RefErrorModel.available():
-        pytest.skip("oracle/_ref/libref_errmodel.so not built (needs /root/reference)")
+        pytest.skip("oracle/_ref/libref_errmodel.so not built (needs the reference checkout, oracle.REFERENCE)")
     return RefErrorModel()
 
 
@@ -123,7 +122,7 @@ def test_custom_model_text_equals_the_reference(ref):
 
 def test_golden_fixture():
     """Committed vectors generated from the compiled reference (tests/golden/make_error_model_golden.py): this is what pins the
-    models where /root/reference is absent (the GPU box)."""
+    models where the reference build is absent."""
     from octopus_b200 import ErrorModel
     with open(GOLDEN) as f:
         cases = json.load(f)["cases"]

@@ -348,7 +348,7 @@ def test_multi_sample_array_is_one_batch_with_per_sample_views(engine, coracle):
 
 def test_populate_matches_the_compiled_reference_populate(engine, refhmm):
     """The CUDA engine against the reference's OWN HaplotypeLikelihoodArray::populate (haplotype_likelihood_array.cpp compiled from
-    /root/reference in the authoring container, oracle/_ref/libref_hmm.so) — no restatement in between: same haplotypes, reads,
+    the reference checkout, oracle/_ref/libref_hmm.so) — no restatement in between: same haplotypes, reads,
     flank state and configuration in, the same [H][R] ln-likelihoods out (integer penalties identical; the double epilogue to 1e-4
     relative, in practice a few ulp)."""
     if refhmm is None:

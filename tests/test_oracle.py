@@ -165,7 +165,7 @@ def test_model_evaluate_mapping_quality_floor(coracle):
 
 # ---------------------------------------------------------------------------------------------------------------------
 # The layer above the kernel, pinned to the reference's own code (pair_hmm.hpp, simd_pair_hmm_wrapper.hpp compiled from
-# /root/reference behind oracle/ref_hmm_driver.cpp). The reference has no unit tests for this layer.
+# the reference checkout behind oracle/ref_hmm_driver.cpp). The reference has no unit tests for this layer.
 # ---------------------------------------------------------------------------------------------------------------------
 def _hmm_case(rng, hap_len, L, exact_rate=0.25):
     hap = ACGT[rng.integers(0, 4, hap_len)].copy()
@@ -246,7 +246,7 @@ def test_c_restatement_align_matches_reference_hmm_align(coracle, refhmm):
 
 
 def test_c_restatement_kmer_mapper_matches_reference_mapper(coracle, refhmm):
-    """oracle_kmer_map against utils/kmer_mapper.hpp itself (compiled from /root/reference), called the way
+    """oracle_kmer_map against utils/kmer_mapper.hpp itself (compiled from the reference checkout), called the way
     HaplotypeLikelihoodArray::populate calls it: repeats (many tied diagonals), non-ACGT bases, reads longer than the
     haplotype, sequences shorter than a k-mer, more than ten maximal diagonals."""
     if refhmm is None:
@@ -305,7 +305,7 @@ def _model_case(rng):
 
 def test_c_restatement_model_evaluate_matches_reference_model(coracle, refhmm):
     """oracle_model_evaluate against the reference's own HaplotypeLikelihoodModel::reset + evaluate
-    (haplotype_likelihood_model.cpp compiled from /root/reference): in-range rule, max over mapping positions U original position,
+    (haplotype_likelihood_model.cpp compiled from the reference checkout): in-range rule, max over mapping positions U original position,
     shifted fallback, ShortHaplotypeError with its required extension, strand-specific SNV arrays, mapping-quality mixing with cap
     trigger, clamp; candidate positions either explicit or mapped by the reference's k-mer mapper as populate() does."""
     if refhmm is None:
@@ -394,7 +394,7 @@ def test_model_layer_agrees_on_hostile_inputs_within_the_quality_domain(coracle,
 
 def test_c_restatement_populate_matches_reference_array_populate(coracle, refhmm):
     """oracle_populate — the checker every GPU populate test compares against — equals the reference's own
-    HaplotypeLikelihoodArray::populate (haplotype_likelihood_array.cpp compiled from /root/reference: H x S x R loop, inline k-mer
+    HaplotypeLikelihoodArray::populate (haplotype_likelihood_array.cpp compiled from the reference checkout: H x S x R loop, inline k-mer
     mapping, model reset / evaluate per haplotype), for several samples (= column ranges of one concatenated batch), with and
     without a flank state, and for the TemplateMap overload (sum over a template's reads)."""
     if refhmm is None:

@@ -1,7 +1,7 @@
-// Integer-issue roofline microbenchmark for sm_100a: per-SM throughput of the instructions the packed pair-HMM cell is
+// Integer-issue roofline microbenchmark for sm_90a: per-SM throughput of the instructions the packed pair-HMM cell is
 // made of (VIMNMX.S16x2, VIMNMX3.S16x2, VIADDMNMX.S16x2, PRMT, IMAD.IADD / IADD3, LDS broadcast), each as 8 independent
 // dependency chains per thread so that latency is hidden, and of the exact 10-instruction cell mix.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o ubench_int ubench_int.cu && ./ubench_int
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o ubench_int ubench_int.cu && ./ubench_int
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
