@@ -1620,22 +1620,32 @@ PHMM_HD int discount_flank(const int score, int flank, const int read_len, const
     return flank <= score ? score - flank : score + flank;   // :760-764
 }
 
-// haplotype_likelihood_model.cpp:285-303: mapping-quality mixing and the > -1e-15 clamp, from the integer penalty.
-__host__ __device__ inline double finish_likelihood(const int best, const bool use_mapq, int mapq, const int mapq_cap, const int mapq_trigger)
+// haplotype_likelihood_model.cpp:285-303: mapping-quality mixing and the > -1e-15 clamp, from the integer penalty. The read's share
+// (mapq_terms) depends on its mapping quality alone, so a caller can tabulate it over the 256 values and finish with finish_mixed.
+struct MapqTerms { double ln_mapped, ln_miss; };
+__host__ __device__ inline MapqTerms mapq_terms(int mapq, const int mapq_cap, const int mapq_trigger)
 {
     const double c = 0.230258509299404568401799145468436420760110148862877297603;   // utils/maths.hpp:41
+    // a trigger at or above the cap is dropped when the model is configured (haplotype_likelihood_model.cpp:49-51, 117-119)
+    if (mapq_trigger >= 0 && mapq_trigger < mapq_cap && mapq >= mapq_trigger) mapq = mapq_cap;
+    const double ln_miss = -c * (double)mapq;
+    return MapqTerms {log(1.0 - exp(ln_miss)), ln_miss};
+}
+__host__ __device__ inline double finish_mixed(const int best, const bool use_mapq, const MapqTerms t)
+{
+    const double c = 0.230258509299404568401799145468436420760110148862877297603;
     const double ln_given_mapped = best == kBestInf ? -1.7976931348623157e308 : -c * (double)best;
     if (use_mapq) {
-        // a trigger at or above the cap is dropped when the model is configured (haplotype_likelihood_model.cpp:49-51, 117-119)
-        if (mapq_trigger >= 0 && mapq_trigger < mapq_cap && mapq >= mapq_trigger) mapq = mapq_cap;
-        const double ln_miss = -c * (double)mapq;
-        const double ln_mapped = log(1.0 - exp(ln_miss));
-        const double a = ln_mapped + ln_given_mapped, b = ln_miss;
+        const double a = t.ln_mapped + ln_given_mapped, b = t.ln_miss;
         const double lo = b < a ? b : a, hi = b < a ? a : b;          // std::minmax (utils/maths.hpp:294-298)
         const double r = hi + log1p(exp(lo - hi));
         return r > -1e-15 ? 0.0 : r;
     }
     return ln_given_mapped > -1e-15 ? 0.0 : ln_given_mapped;
+}
+__host__ __device__ inline double finish_likelihood(const int best, const bool use_mapq, int mapq, const int mapq_cap, const int mapq_trigger)
+{
+    return finish_mixed(best, use_mapq, use_mapq ? mapq_terms(mapq, mapq_cap, mapq_trigger) : MapqTerms {0.0, 0.0});
 }
 
 } // namespace phmm

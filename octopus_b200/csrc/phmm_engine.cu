@@ -63,7 +63,7 @@ struct phmm_engine {
     DBuf c_off, c_pos;
     // derived / scratch
     DBuf tab_f, tab_r, rowhalf, info, flags, best, status, out, slow, counters, pairs, generic_reads, wide_reads, bp, regs, rregion, rpbase, rpstride;
-    DBuf tasks_lane, tasks_generic, works, scores;
+    DBuf tasks_lane, tasks_generic, works, scores, mapq_tab;
     DBuf rhash, kbins, kitems, kpos, kcnt, ftasks, fcnt, gtasks, atasks, gcnt, sched, sorted, fb_scratch, fb_pairs, npre_f, npre_r;
     std::vector<cudaEvent_t> tile_events;
     std::vector<int2> info_host;
@@ -341,7 +341,7 @@ void phmm_destroy(phmm_engine* e)
     DBuf* all[] = {&e->h_off, &e->h_seq, &e->h_mf, &e->h_pf, &e->h_mr, &e->h_pr, &e->h_go, &e->h_ge, &e->h_begin,
                    &e->r_off, &e->r_bases, &e->r_quals, &e->r_mapq, &e->r_rev, &e->r_begin, &e->c_off, &e->c_pos,
                    &e->tab_f, &e->tab_r, &e->rowhalf, &e->info, &e->flags, &e->best, &e->status, &e->out, &e->slow,
-                   &e->counters, &e->pairs, &e->generic_reads, &e->wide_reads, &e->bp, &e->regs, &e->rregion, &e->rpbase, &e->rpstride, &e->tasks_lane, &e->tasks_generic, &e->works, &e->scores,
+                   &e->counters, &e->pairs, &e->generic_reads, &e->wide_reads, &e->bp, &e->regs, &e->rregion, &e->rpbase, &e->rpstride, &e->tasks_lane, &e->tasks_generic, &e->works, &e->scores, &e->mapq_tab,
                    &e->rhash, &e->kbins, &e->kitems, &e->kpos, &e->kcnt, &e->ftasks, &e->fcnt, &e->gtasks, &e->atasks, &e->gcnt, &e->sched, &e->sorted, &e->fb_scratch, &e->fb_pairs, &e->npre_f, &e->npre_r};
     for (DBuf* b : all) b->release();
     for (cudaEvent_t ev : e->tile_events) cudaEventDestroy(ev);
@@ -885,6 +885,15 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
     }
     const bool use_mapper = !(positions && positions->off && positions->pos) && cfg->map_positions;
     p.single_candidate = max_dp_per_pair == 1 ? 1 : 0;
+    // bands 32 / 64 with enough tasks per read to fill a warp: one WARP per chunk of the band (k_populate_roles) instead of one lane
+    static const bool no_role_warps = std::getenv("PHMM_NO_ROLE_WARPS") != nullptr;       // measurement hook: the lane-per-chunk kernel for every band
+    const bool role_band = (band == 32 || band == 64) && H >= 17 && !no_role_warps;
+    // Direct mode (PopParams::direct): every pair has one candidate position and a plain DP for it, so the pair list needs neither
+    // the classify pass nor the epilogue. Reads with 'N' go to the wide list, which keeps both. k_populate_roles keeps the classify
+    // path: the task derivation and the FP64 finish would more than double its register spills.
+    static const bool no_direct = std::getenv("PHMM_NO_DIRECT") != nullptr;              // measurement hook: the classify path for every list
+    const bool direct = !no_direct && !p.pos_off && !use_mapper && !p.shortcut && !multi->any_flank && !cfg->use_int_scores && !role_band;
+    p.direct = direct ? 1 : 0;
     p.reserved_sms = e->reserved_sms;
     int mapper_maxt = 0;
     if (use_mapper) {
@@ -917,7 +926,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
     mode.packed_ok = task_word_ok ? 1 : 0;
     mode.wide_ok = (task_word_ok && wide_warps >= 1) ? 1 : 0;
     mode.force_wide = cfg->use_int_scores ? 1 : 0;
-    mode.n_to_wide = band > 32 ? 1 : 0;
+    mode.n_to_wide = (band > 32 || direct) ? 1 : 0;
     mode.wide_max_len = kWideMaxReadLen;
     const bool fast_ok = mode.packed_ok && !mode.force_wide;
     // lane groups per warp of the packed kernel: with few haplotypes a read has few DP tasks, so several read pairs share a warp
@@ -962,11 +971,25 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
     CU(e->status.ensure((size_t)HR * sizeof(int)));
     CU(e->counters.ensure(256));
     CU(cudaMemsetAsync(e->counters.p, 0, 256, e->stream));
-    CU(cudaMemsetAsync(e->status.p, 0, (size_t)HR * sizeof(int), e->stream));
-    k_fill_int<<<(unsigned)((HR + 255) / 256), 256, 0, e->stream>>>(e->best.as<int>(), HR, kBestInf);
-    LAUNCHED();
+    if (!direct) {           // direct mode: k_list_slots sets up the wide / generic tiles' slots, the pair list needs none
+        CU(cudaMemsetAsync(e->status.p, 0, (size_t)HR * sizeof(int), e->stream));
+        k_fill_int<<<(unsigned)((HR + 255) / 256), 256, 0, e->stream>>>(e->best.as<int>(), HR, kBestInf);
+        LAUNCHED();
+    }
     p.best = e->best.as<int>();
     p.status = e->status.as<int>();
+    CU(e->out.ensure((size_t)HR * sizeof(double)));
+    double* d_out = (space == PHMM_SPACE_DEVICE && !template_off) ? out : e->out.as<double>();
+    p.out = d_out;
+    p.out_row_extra = d_out == out && space == PHMM_SPACE_DEVICE && out_pitch > R ? out_pitch - R : 0LL;
+    p.out_status = status ? p.status : nullptr;
+    p.use_mapq = cfg->use_mapping_quality; p.mapq_cap = cfg->mapping_quality_cap; p.mapq_trigger = cfg->mapping_quality_cap_trigger;
+    if (direct && p.use_mapq) {
+        CU(e->mapq_tab.ensure(256 * sizeof(MapqTerms)));
+        k_mapq_terms<<<1, 256, 0, e->stream>>>(p.mapq_cap, p.mapq_trigger, e->mapq_tab.as<MapqTerms>());
+        LAUNCHED();
+        p.mapq_tab = e->mapq_tab.as<MapqTerms>();
+    }
     p.flags = e->flags.as<int>();
     int* counters = e->counters.as<int>();
     p.pair_cursor = counters + 0;
@@ -1052,9 +1075,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
         PHMM_FAST_DISPATCH(PHMM_FAST_SETUP)
         if (blocks_per_sm < 1) { e->err = "fast kernel does not fit on an SM (read too long?)"; return PHMM_ERR_INVALID; }
     }
-    // bands 32 / 64 with enough tasks per read to fill a warp: one WARP per chunk of the band (k_populate_roles) instead of one lane
-    static const bool no_role_warps = std::getenv("PHMM_NO_ROLE_WARPS") != nullptr;       // measurement hook: the lane-per-chunk kernel for every band
-    bool role_warps = n_pairs && (band == 32 || band == 64) && groups == 1 && !no_role_warps;
+    bool role_warps = n_pairs && role_band;
     const int role_groups = kFastWarpsPerBlock / std::max(1, NL);
     const size_t role_smem = role_warps ? (size_t)role_groups * fast_row_stride * sizeof(RowEntry) + (size_t)role_groups * kRoleWordsPerGroup(NL) * sizeof(uint32_t) : 0;
     int role_blocks_per_sm = 0;
@@ -1177,10 +1198,11 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
                 p.kpos = e->kpos.as<int32_t>(); p.kcnt = e->kcnt.as<uint8_t>();
             }
             CU(cudaMemsetAsync(counters, 0, 8 * sizeof(int), e->stream));                       // cursors, any-tasks flags (the traceback queue is empty between tiles)
-            CU(cudaMemsetAsync(p.fcnt, 0, (size_t)2 * np * sizeof(int), e->stream));
-            CU(cudaMemsetAsync(p.gcnt, 0, (size_t)2 * np * sizeof(int), e->stream));
-            CU(cudaMemsetAsync(p.acnt, 0, (size_t)2 * np * sizeof(int), e->stream));
-            {   // classify pass: shortcut values → best[], near-flank candidates → slow queue, DP candidates → task lists
+            if (!direct) {
+                CU(cudaMemsetAsync(p.fcnt, 0, (size_t)2 * np * sizeof(int), e->stream));
+                CU(cudaMemsetAsync(p.gcnt, 0, (size_t)2 * np * sizeof(int), e->stream));
+                CU(cudaMemsetAsync(p.acnt, 0, (size_t)2 * np * sizeof(int), e->stream));
+                // classify pass: shortcut values → best[], near-flank candidates → slow queue, DP candidates → task lists
                 const long long threads = 2LL * np * H;
                 k_populate_generic<64, true><<<(unsigned)((threads + 127) / 128), 128, 0, e->stream>>>(p);
                 LAUNCHED();
@@ -1202,7 +1224,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
             // with a flank state the tile's DP work is split between the score-only kernel and the flank-aware kernels: time them together
             if (!p.use_flanks) CU(cudaEventRecord(e->tile_events[2 * n_timed + 1], e->stream));
             lap(" dp queued");
-            if ((rc = launch_flank(2 * np, fast_row_stride))) return rc;
+            if (!direct && (rc = launch_flank(2 * np, fast_row_stride))) return rc;
             if (p.use_flanks) CU(cudaEventRecord(e->tile_events[2 * n_timed + 1], e->stream));
             ++n_timed; timed = true;
             p0 += np;
@@ -1222,6 +1244,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
             CU(cudaMemsetAsync(p.fcnt, 0, (size_t)nw * sizeof(int), e->stream));
             CU(cudaMemsetAsync(p.gcnt, 0, (size_t)nw * sizeof(int), e->stream));
             CU(cudaMemsetAsync(p.acnt, 0, (size_t)nw * sizeof(int), e->stream));
+            if (direct) { k_list_slots<<<cgrid, 128, 0, e->stream>>>(p, true); LAUNCHED(); }
             k_populate_generic<64, true><<<cgrid, 128, 0, e->stream>>>(p);          // classify pass over the wide list
             LAUNCHED();
             const unsigned wgrid = (unsigned)std::max(1, std::min((nw + wide_warps - 1) / wide_warps, e->sm_count * wide_blocks_per_sm));
@@ -1236,6 +1259,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
             if (wide_row_stride <= fast_row_stride + 8 || (size_t)kFastWarpsPerBlock * wide_row_stride * sizeof(RowEntry) <= (200u << 10)) {
                 if ((rc = launch_flank(nw, wide_row_stride))) return rc;
             }
+            if (direct) { k_list_slots<<<cgrid, 128, 0, e->stream>>>(p, false); LAUNCHED(); }
             w0 += nw;
         } else {
             const int ng = (int)std::min<long long>(reads_per_tile, n_generic - g0);
@@ -1250,12 +1274,14 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
                 p.kpos = e->kpos.as<int32_t>(); p.kcnt = e->kcnt.as<uint8_t>();
             }
             const bool time_generic = n_pairs == 0 && n_wide == 0 && n_timed == 0;
+            if (direct) { k_list_slots<<<ggrid, 64, 0, e->stream>>>(p, true); LAUNCHED(); }
             CU(chunk_order.wait_for_previous());
             if (time_generic) CU(cudaEventRecord(e->ev0, e->stream));
             if (band <= 32) k_populate_generic<64, false><<<ggrid, 64, 0, e->stream>>>(p);
             else k_populate_generic<kGenericMaxDiag, false><<<ggrid, 64, 0, e->stream>>>(p);
             LAUNCHED();
             if (time_generic) { CU(cudaEventRecord(e->ev1, e->stream)); timed = true; }
+            if (direct) { k_list_slots<<<ggrid, 64, 0, e->stream>>>(p, false); LAUNCHED(); }
             g0 += ng;
         }
         if (p.use_flanks) {
@@ -1269,15 +1295,12 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
 
     chunk_order.publish(true);
     lap("tiles enqueued");
-    CU(e->out.ensure((size_t)HR * sizeof(double)));
-    double* d_out = (space == PHMM_SPACE_DEVICE && !template_off) ? out : e->out.as<double>();
-    {
+    if (!direct) {
         const long long threads = (long long)H * R;
         k_epilogue<<<(unsigned)((threads + 255) / 256), 256, 0, e->stream>>>(p.best, p.status, s.rd, e->regs.as<RegionInfo>(), H, cfg->use_mapping_quality,
-                                                                             cfg->mapping_quality_cap, cfg->mapping_quality_cap_trigger, d_out,
-                                                                             d_out == out && space == PHMM_SPACE_DEVICE && out_pitch > R ? out_pitch - R : 0LL);
+                                                                             cfg->mapping_quality_cap, cfg->mapping_quality_cap_trigger, d_out, p.out_row_extra);
+        LAUNCHED();
     }
-    LAUNCHED();
     CU(cudaGetLastError());
     if (template_off && G > 1) { e->err = "templates are not supported with several regions"; return PHMM_ERR_INVALID; }
     if (template_off) {

@@ -137,6 +137,7 @@ __global__ void k_read_info(const int n_reads, const long long* __restrict__ off
     const long long b = off[r];
     const int L = (int)(off[r + 1] - b);
     int flags = 0, qsum = 0;
+#pragma unroll 4      // the loads of several iterations in flight: a warp's read is only a handful of iterations long
     for (int y = lane; y < L; y += 32) {
         const int c = base_code(bases[b + y]);
         const int q = quals[b + y];
@@ -179,6 +180,20 @@ __global__ void k_read_regions(const int n_reads, const int n_regions, const Reg
 constexpr int kLenBins = kFastMaxReadLen + 1;
 struct SchedTotals { int n_pairs, n_generic, lmax_fast, lmax_all, n_eligible, bad; long long cells; int n_with_n, n_wide; };
 
+// Append one task to list slot li with a warp-aggregated counter update: the lanes of a warp that append to the same list
+// (normally all of them: consecutive threads are consecutive haplotypes of one read) share a single atomicAdd. The scheduler
+// uses it for its length bins, which the reads of a batch of one read length all hit.
+__device__ __forceinline__ int list_append_slot(int* counts, const int li)
+{
+    const unsigned active = __activemask();
+    const unsigned peers = __match_any_sync(active, li);
+    const int leader = __ffs(peers) - 1, lane = threadIdx.x & 31;
+    int base = 0;
+    if (lane == leader) base = atomicAdd(counts + li, __popc(peers));
+    base = __shfl_sync(peers, base, leader);
+    return base + __popc(peers & ((1u << lane) - 1u));
+}
+
 // misc counters: [0] generic reads, [1] longest read, [2] bad, [3] packed reads holding 'N', [4] wide reads
 __global__ void k_sched_hist(const int R, const int2* __restrict__ info, const SchedMode mode, int* __restrict__ hist,
                              int* __restrict__ generic, int* __restrict__ wide, int* __restrict__ misc,
@@ -187,15 +202,16 @@ __global__ void k_sched_hist(const int R, const int2* __restrict__ info, const S
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     // banded cells of the read against every haplotype of its region (the GCUPS numerator), one atomic per warp
     unsigned long long mine = r < R ? (unsigned long long)(2LL * (info[r].x + band) * band) * (unsigned long long)regs[region[r]].nH : 0ull;
+    int lmax = r < R ? info[r].x : 0;
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
+    for (int o = 16; o > 0; o >>= 1) { mine += __shfl_xor_sync(0xffffffffu, mine, o); lmax = max(lmax, __shfl_xor_sync(0xffffffffu, lmax, o)); }
     if ((threadIdx.x & 31) == 0 && mine) atomicAdd(cells, mine);
+    if ((threadIdx.x & 31) == 0) atomicMax(misc + 1, lmax);
     if (r >= R) return;
     const int2 inf = info[r];
     if (inf.x < 1) atomicExch(misc + 2, 1);
-    atomicMax(misc + 1, inf.x);
     const int route = read_route(inf, mode);
-    if (route == 0) { atomicAdd(&hist[inf.x], 1); if (inf.y & kReadHasN) atomicAdd(misc + 3, 1); }
+    if (route == 0) { list_append_slot(hist, inf.x); if (inf.y & kReadHasN) atomicAdd(misc + 3, 1); }
     else if (route == 1) wide[atomicAdd(misc + 4, 1)] = r;
     else generic[atomicAdd(misc + 0, 1)] = r;
 }
@@ -249,7 +265,7 @@ __global__ void k_sched_scatter(const int R, const int2* __restrict__ info, cons
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= R) return;
     const int2 inf = info[r];
-    if (read_route(inf, mode) == 0) sorted[read_start[inf.x] + atomicAdd(&cursors[inf.x], 1)] = r;
+    if (read_route(inf, mode) == 0) sorted[read_start[inf.x] + list_append_slot(cursors, inf.x)] = r;
 }
 
 // pair slot j → (read, read | -1) or (-1, -1) padding
@@ -448,6 +464,15 @@ struct PopParams {
     // kind 0 = the pair list (two entries per pair, -1 = padding), 1 = wide reads, 2 = generic reads.
     const int* list;
     int list_kind, n_list, list_base;   // n_list: upper bound on the tile's entries; list_base: index of the tile's first entry
+    // Direct mode (one candidate position per pair and a plain DP for it: no listed / mapped positions, shortcut off, no flank state,
+    // 16-bit scores): the pair list has no classify pass and no epilogue. Task k of a read is its region's haplotype slot k, its window
+    // comes from direct_window, and the lane that owns a result writes the ln-likelihood (and the status word) itself.
+    int direct;
+    double* out;                // result matrix: slot pair_slot(h, r) + hl * out_row_extra (as k_epilogue)
+    long long out_row_extra;
+    int* out_status;            // status words of direct-mode pairs, or null when the caller did not ask for them
+    int use_mapq, mapq_cap, mapq_trigger;
+    const MapqTerms* mapq_tab;  // mapq_terms of every mapping quality 0..255 (k_mapq_terms), read when use_mapq
 };
 
 // flat index → (list slot, haplotype); 64-bit division is an expensive software routine, the index nearly always fits 32 bits
@@ -484,19 +509,6 @@ __device__ __forceinline__ ReadView read_view(const DevReads& rd, const int r)
     return ReadView {rd.bases + o, rd.quals + o, (int)(rd.off[r + 1] - o)};
 }
 
-// Append one task to list slot li with a warp-aggregated counter update: the lanes of a warp that append to the same list
-// (normally all of them: consecutive threads are consecutive haplotypes of one read) share a single atomicAdd.
-__device__ __forceinline__ int list_append_slot(int* counts, const int li)
-{
-    const unsigned active = __activemask();
-    const unsigned peers = __match_any_sync(active, li);
-    const int leader = __ffs(peers) - 1, lane = threadIdx.x & 31;
-    int base = 0;
-    if (lane == leader) base = atomicAdd(counts + li, __popc(peers));
-    base = __shfl_sync(peers, base, leader);
-    return base + __popc(peers & ((1u << lane) - 1u));
-}
-
 // as list_append_slot, for lanes that may append to different lists (route) of the same slot
 __device__ __forceinline__ int list_append_slot2(int* counts, const int li, const int route)
 {
@@ -514,6 +526,59 @@ __device__ __forceinline__ void push_slow(const PopParams& p, const int r, const
     const int idx = atomicAdd(p.slow_count, 1);
     if (idx < p.slow_cap) p.slow[idx] = make_int4(r, h, a, 0);
     else atomicOr(p.flags, 4);
+}
+
+// Direct mode: the classify pass's candidate walk for pair (h, read of length L) with no listed positions, shortcut and flank state
+// off (candidate_slot / classify_candidate with npos = 0: the original position, then the shifted fallback). Returns the column-table
+// index of the DP window, or -1 when the pair runs no DP; *status gets the pair's status word (0, 1, or 2 | extension << 16).
+__device__ __forceinline__ long long direct_window(const PopParams& p, const int h, const int L, const long long read_begin, int* status)
+{
+    const long long o = p.hp.off[h];
+    const HapView hv {nullptr, nullptr, nullptr, nullptr, nullptr, (int)(p.hp.off[h + 1] - o)};
+    const ReadView rv {nullptr, nullptr, L};
+    const long long orig = read_begin - (p.hp.begin ? p.hp.begin[h] : 0);
+    EnumState st {false, false};
+    *status = 1;
+    for (int c = 0; c < 2; ++c) {
+        int pos;
+        const int k = candidate_slot(c, 0, nullptr, orig, L, hv.len, p.band, st, &pos);
+        if (k < 0) { *status = 2 | (min(pos, 0x7FFF) << 16); return -1; }
+        if (k == 0) continue;
+        int a;
+        if (classify_candidate(hv, rv, p.band, pos, false, false, 0, 0, &a) == CAND_DP) { *status = 0; return o + a; }
+    }
+    return -1;
+}
+
+// Direct mode: what k_epilogue does for one pair, from the DP's score (kBestInf: no DP) and the pair's status word.
+__device__ __forceinline__ void direct_store(const PopParams& p, const int r, const int h, const int hl, const int score, const int status)
+{
+    const long long i = pair_slot(p.rd, h, r);
+    const MapqTerms t = p.use_mapq ? p.mapq_tab[p.rd.mapq[r]] : MapqTerms {0.0, 0.0};
+    p.out[i + hl * p.out_row_extra] = finish_mixed(status == 0 ? score : kBestInf, p.use_mapq != 0, t);
+    if (p.out_status) p.out_status[i] = status;
+    if ((status & 3) == 2) atomicOr(p.flags, 2);
+}
+
+// Direct mode: the column windows of one lane's two halves (task slot k of reads r0 / r1, haplotype bases hb0 / hb1, -1 = no task).
+// A half without a window replays the other half's, a lane with none replays the first lane's that has one (results discarded).
+// Returns false when no lane of the warp has a window: the warp skips the DP of this round.
+__device__ __forceinline__ bool direct_columns(const PopParams& p, const ColEntry* tab0, const ColEntry* tab1, const int r0, const int r1,
+                                               const int hb0, const int hb1, const int k, const int L, int* st0, int* st1,
+                                               const ColEntry** c0, const ColEntry** c1)
+{
+    const long long i0 = hb0 >= 0 ? direct_window(p, hb0 + k, L, p.rd.begin ? p.rd.begin[r0] : 0, st0) : -1;
+    const long long i1 = hb1 >= 0 ? direct_window(p, hb1 + k, L, p.rd.begin ? p.rd.begin[r1] : 0, st1) : -1;
+    const ColEntry* a = i0 >= 0 ? tab0 + i0 : (i1 >= 0 ? tab1 + i1 : nullptr);
+    const ColEntry* b = i1 >= 0 ? tab1 + i1 : a;
+    const unsigned anyone = __ballot_sync(0xffffffffu, a != nullptr);
+    if (anyone == 0u) return false;
+    const int src = __ffs(anyone) - 1;
+    const ColEntry* sa = (const ColEntry*)__shfl_sync(0xffffffffu, (unsigned long long)a, src);
+    const ColEntry* sb = (const ColEntry*)__shfl_sync(0xffffffffu, (unsigned long long)b, src);
+    *c0 = a ? a : sa;
+    *c1 = a ? b : sb;
+    return true;
 }
 
 constexpr int kRoundsPerUnit = 8;   // dp_pair rounds per work unit of the fast kernel (bounds the tail imbalance of long task lists)
@@ -722,7 +787,14 @@ k_populate_fast(const PopParams p)
         const int j = jb + grp;
         const int r0 = j < n_pairs ? p.pair_reads[2 * j] : -1;
         const int r1 = r0 >= 0 ? p.pair_reads[2 * j + 1] : -1;
-        const int n0 = r0 >= 0 ? p.fcnt[2 * j] : 0, n1 = r1 >= 0 ? p.fcnt[2 * j + 1] : 0;
+        // direct mode: a read's tasks are its region's haplotype slots (hb: the region's first haplotype)
+        int n0 = 0, n1 = 0, hb0 = 0, hb1 = 0;
+        if (p.direct) {
+            if (r0 >= 0) { const RegionInfo g = p.regs[p.rd.region[r0]]; n0 = g.nH; hb0 = g.h0; }
+            if (r1 >= 0) { const RegionInfo g = p.regs[p.rd.region[r1]]; n1 = g.nH; hb1 = g.h0; }
+        } else {
+            n0 = r0 >= 0 ? p.fcnt[2 * j] : 0; n1 = r1 >= 0 ? p.fcnt[2 * j + 1] : 0;
+        }
         int nmax = max(n0, n1), L = r0 >= 0 ? p.rd.info[r0].x : 0;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) { nmax = max(nmax, __shfl_xor_sync(0xffffffffu, nmax, o)); L = max(L, __shfl_xor_sync(0xffffffffu, L, o)); }
@@ -743,25 +815,37 @@ k_populate_fast(const PopParams p)
         const uint32_t* q1 = q0 + p.fcap;
         for (int c = c_begin; c < c_end; c += TPR) {
             const bool v0 = c + slot < n0, v1 = c + slot < n1;
-            // idle half-lanes replay a valid task (result discarded): of their own group if it has one, else of any lane
-            const bool have = (n0 > 0) || (n1 > 0);
-            uint32_t t0 = 0, t1 = 0;
-            const ColEntry *b0 = tab0, *b1 = tab1;
-            if (have) {
-                t0 = n0 > 0 ? q0[v0 ? c + slot : 0] : q1[0];
-                t1 = n1 > 0 ? q1[v1 ? c + slot : 0] : t0;
-                if (n0 == 0) b0 = tab1;
-                if (n1 == 0) b1 = tab0;
+            const ColEntry *c0, *c1;
+            bool run = true;
+            int st0 = 0, st1 = 0, h0 = 0, h1 = 0;
+            if (p.direct) {
+                h0 = hb0 + c + slot; h1 = hb1 + c + slot;
+                run = direct_columns(p, tab0, tab1, r0, r1, v0 ? hb0 : -1, v1 ? hb1 : -1, c + slot, L, &st0, &st1, &c0, &c1);
+            } else {
+                // idle half-lanes replay a valid task (result discarded): of their own group if it has one, else of any lane
+                const bool have = (n0 > 0) || (n1 > 0);
+                uint32_t t0 = 0, t1 = 0;
+                const ColEntry *b0 = tab0, *b1 = tab1;
+                if (have) {
+                    t0 = n0 > 0 ? q0[v0 ? c + slot : 0] : q1[0];
+                    t1 = n1 > 0 ? q1[v1 ? c + slot : 0] : t0;
+                    if (n0 == 0) b0 = tab1;
+                    if (n1 == 0) b1 = tab0;
+                }
+                const unsigned anyone = __ballot_sync(0xffffffffu, have);
+                const int src = __ffs(anyone) - 1;
+                const uint32_t s0 = __shfl_sync(0xffffffffu, t0, src), s1 = __shfl_sync(0xffffffffu, t1, src);
+                const unsigned long long sb0 = __shfl_sync(0xffffffffu, (unsigned long long)b0, src), sb1 = __shfl_sync(0xffffffffu, (unsigned long long)b1, src);
+                if (!have) { t0 = s0; t1 = s1; b0 = (const ColEntry*)sb0; b1 = (const ColEntry*)sb1; }
+                h0 = (int)(t0 & 0xFFFFu); h1 = (int)(t1 & 0xFFFFu);
+                c0 = b0 + p.hp.off[h0] + (int)(t0 >> 16); c1 = b1 + p.hp.off[h1] + (int)(t1 >> 16);
             }
-            const unsigned anyone = __ballot_sync(0xffffffffu, have);
-            const int src = __ffs(anyone) - 1;
-            const uint32_t s0 = __shfl_sync(0xffffffffu, t0, src), s1 = __shfl_sync(0xffffffffu, t1, src);
-            const unsigned long long sb0 = __shfl_sync(0xffffffffu, (unsigned long long)b0, src), sb1 = __shfl_sync(0xffffffffu, (unsigned long long)b1, src);
-            if (!have) { t0 = s0; t1 = s1; b0 = (const ColEntry*)sb0; b1 = (const ColEntry*)sb1; }
-            const int h0 = (int)(t0 & 0xFFFFu), a0 = (int)(t0 >> 16), h1 = (int)(t1 & 0xFFFFu), a1 = (int)(t1 >> 16);
-            const ColEntry *c0 = b0 + p.hp.off[h0] + a0, *c1 = b1 + p.hp.off[h1] + a1;
-            const uint32_t res = oge ? packed_dp<BAND, true>(rows, L, c0, c1, nucp, jl, (uint32_t)p.one) : packed_dp<BAND, false>(rows, L, c0, c1, nucp, jl, (uint32_t)p.one);
-            if (jl == 0) {
+            uint32_t res = 0u;
+            if (run) res = oge ? packed_dp<BAND, true>(rows, L, c0, c1, nucp, jl, (uint32_t)p.one) : packed_dp<BAND, false>(rows, L, c0, c1, nucp, jl, (uint32_t)p.one);
+            if (jl == 0 && p.direct) {
+                if (v0) direct_store(p, r0, h0, c + slot, (int)(res & 0xFFFFu), st0);
+                if (v1) direct_store(p, r1, h1, c + slot, (int)(res >> 16), st1);
+            } else if (jl == 0) {
                 // at most one candidate per pair (single_candidate): its value IS the pair's minimum — a plain store, no read of best[]
                 if (v0) { int* dst = p.best + pair_slot(p.rd, h0, r0); const int v = (int)(res & 0xFFFFu); if (p.single_candidate) *dst = v; else atomicMin(dst, v); }
                 if (v1) { int* dst = p.best + pair_slot(p.rd, h1, r1); const int v = (int)(res >> 16); if (p.single_candidate) *dst = v; else atomicMin(dst, v); }
@@ -1580,6 +1664,33 @@ __global__ void k_epilogue(const int* __restrict__ best, int* __restrict__ statu
     if (b == kBestInf && status[i] == 0) status[i] = 1;
     // `out` may be another GPU's memory (a peer mapping, phmm_ipc_open): plain coalesced stores, nothing is read back
     out[i + hl * out_row_extra] = finish_likelihood(b, use_mapq != 0, rd.mapq[r], mapq_cap, mapq_trigger);
+}
+
+// Direct mode: the read-dependent half of finish_likelihood for every mapping quality, once per call (one block of 256 threads), so
+// that the DP kernel's lanes only finish their own pair.
+__global__ void k_mapq_terms(const int mapq_cap, const int mapq_trigger, MapqTerms* __restrict__ tab)
+{
+    tab[threadIdx.x] = mapq_terms((int)threadIdx.x, mapq_cap, mapq_trigger);
+}
+
+// Direct mode: best[] / status[] of the current wide or generic tile's pairs only. init: what k_fill_int and the status memset do
+// for the whole matrix; !init: k_epilogue's work. The pair list's results never touch best[] (the DP kernel stores them itself).
+__global__ void k_list_slots(const PopParams p, const bool init)
+{
+    const int n_list = tile_list(p);
+    const long long total = (long long)n_list * p.Hmax, step = (long long)gridDim.x * blockDim.x;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += step) {
+        int li, hl;
+        split_index(t, p.Hmax, &li, &hl);
+        const int r = p.list[li];
+        const RegionInfo g = p.regs[p.rd.region[r]];
+        if (hl >= g.nH) continue;
+        const long long i = pair_slot(p.rd, g.h0 + hl, r);
+        if (init) { p.best[i] = kBestInf; p.status[i] = 0; continue; }
+        const int b = p.best[i];
+        if (b == kBestInf && p.status[i] == 0) p.status[i] = 1;
+        p.out[i + hl * p.out_row_extra] = finish_likelihood(b, p.use_mapq != 0, p.rd.mapq[r], p.mapq_cap, p.mapq_trigger);
+    }
 }
 
 } // namespace phmm
