@@ -154,6 +154,14 @@ __device__ __forceinline__ uint32_t fma_add(uint32_t a, uint32_t b, uint32_t one
 inline uint32_t fma_add(uint32_t a, uint32_t b, uint32_t one) { return a * one + b; }
 #endif
 
+// An empty asm statement whose text differs per tag: branches that go through one of these to a common target each keep a block of
+// their own, which is where ptxas then places the register copies that branch needs
+#ifdef __CUDA_ARCH__
+#define PHMM_DISTINCT_PATH(tag) asm volatile("// path " tag);
+#else
+#define PHMM_DISTINCT_PATH(tag)
+#endif
+
 // ---------------------------------------------------------------------------------------------------------
 // Fast path: two alignments per thread, s16x2 lanes, band state in registers
 // ---------------------------------------------------------------------------------------------------------
@@ -170,11 +178,17 @@ inline uint32_t fma_add(uint32_t a, uint32_t b, uint32_t one) { return a * one +
 //
 // Four column bodies, all fully unrolled over k with M / D in registers:
 //   steady    2B <= x <= L      every cell exists
-//   prologue  x < 2B, x <= L    cell (x, 0) is the free start; cells k < x follow — entered through a jump table
+//   prologue  x < 2B, x <= L    cell (x, 0) is the free start; cells k < x follow — an indexed branch to an entry copy of cell
+//                               x-1, which continues in the unrolled sequence at x-2
 //   epilogue  x > L, x >= 2B    cells k >= x - L; leaves the unrolled sequence after the row-L cell
 //   general   x < 2B, x > L     (reads shorter than the band) both limits, per-cell predicates
 #define PHMM_REP8(F, b)  F(b + 7) F(b + 6) F(b + 5) F(b + 4) F(b + 3) F(b + 2) F(b + 1) F(b + 0)
 #define PHMM_REP64(F)    PHMM_REP8(F, 56) PHMM_REP8(F, 48) PHMM_REP8(F, 40) PHMM_REP8(F, 32) PHMM_REP8(F, 24) PHMM_REP8(F, 16) PHMM_REP8(F, 8) PHMM_REP8(F, 0)
+// 63 .. 0 as single tokens (for labels built with ##)
+#define PHMM_DESC64(F)   F(63) F(62) F(61) F(60) F(59) F(58) F(57) F(56) F(55) F(54) F(53) F(52) F(51) F(50) F(49) F(48) \
+                         F(47) F(46) F(45) F(44) F(43) F(42) F(41) F(40) F(39) F(38) F(37) F(36) F(35) F(34) F(33) F(32) \
+                         F(31) F(30) F(29) F(28) F(27) F(26) F(25) F(24) F(23) F(22) F(21) F(20) F(19) F(18) F(17) F(16) \
+                         F(15) F(14) F(13) F(12) F(11) F(10) F(9) F(8) F(7) F(6) F(5) F(4) F(3) F(2) F(1) F(0)
 
 // OGE ("open >= extend"): the caller knows gap_open[x] >= gap_extend[x] for every column of both windows (true of every penalty
 // array the reference's short-read error models produce — the PacBio tables break it inside long homopolymers, custom models may;
@@ -208,8 +222,12 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
         if ((k) + 1 < K) D[((k) + 1) < K ? (k) + 1 : 0] = vaddmin(d, ge, fma_add(OGE ? s : vmin2(m, i_run), go, one)); \
         i_run = vaddmin(i_run, gep, fma_add(m, gop, one));                                  \
     }
-#define PHMM_CASE_PROLOGUE(k) case (k) + 1: if ((k) < K) PHMM_CELL(k)
-#define PHMM_CASE_ROW0(k)     case (k): if ((k) < K) M[(k) < K ? (k) : 0] = sub0; break;
+    // prologue: the entry cell k = x-1 of column x reads the row-0 value of column x-1 from M[2B-1] instead of M[x-1], then jumps
+    // into the shared chain at k = x-2: one dispatch per column and no indexed store of the row-0 value
+#define PHMM_PRO_ENTRY(k)     case (k) + 1: if ((k) + 1 < K) { M[(k) < K ? (k) : 0] = M[K - 1]; PHMM_CELL(k) goto pro_##k; } goto pro_0;
+#define PHMM_PRO_CHAIN(k)     pro_##k: if ((k) >= 1 && (k) <= K) PHMM_CELL((k) >= 1 && (k) <= K ? (k) - 1 : 0)
+    // epilogue: cell k, then, if it was the row-L cell, a jump to the column end through a block of its own (PHMM_DISTINCT_PATH)
+#define PHMM_EPI_CELL(k)      if ((k) >= 1 && (k) < K) { PHMM_CELL((k) < K ? (k) : 0) if ((k) == klo) { PHMM_DISTINCT_PATH(#k) goto column_end; } }
 
     for (int x = 0; x <= W; ++x) {
         const int xn = (x + 1 < W) ? x + 1 : W - 1;
@@ -227,32 +245,32 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
 #pragma unroll
                 for (int k = K - 1; k >= 0; --k) PHMM_CELL(k)
             } else {
-                // epilogue: rows beyond L do not exist; stop after the row-L cell so that M[x-L] keeps S(x, L)
+                // epilogue: rows beyond L do not exist; stop after the row-L cell (k = x - L >= 1) so that M[x-L] keeps S(x, L).
+                // Every exit leaves through a block of its own: when they all branch straight to the column end, ptxas puts the
+                // register copies each exit needs on the path that falls through to the next cell, where they run for every cell.
                 const int klo = x - L;
-#pragma unroll
-                for (int k = K - 1; k >= 0; --k) {
-                    PHMM_CELL(k)
-                    if (k == klo) break;
-                }
+                PHMM_DESC64(PHMM_EPI_CELL)
             }
-        } else {
-            // cell (x, 0): S = 0, so m(x+1, 1) = sub(x, 0), and i(x, 1) = gap_open[x-1] + nuc for odd x, +inf for even x
-            const uint32_t sub0 = vmin2(w0.y, prmt(caps0, caps1, w0.x));
+        } else if (x <= L) {
+            // prologue: cell (x, 0) has S = 0, so m(x+1, 1) = sub(x, 0), and i(x, 1) = gap_open[x-1] + nuc for odd x, +inf for even x;
+            // cells k = x-1 .. 0 all exist. No cell reads M[2B-1] before column 2B, so it carries m(x+1, 1) to the next column's
+            // entry cell, and after column 2B-1 it holds what the first steady column reads.
             i_run = (x & 1) ? gop : kInf16x2;
-            if (x <= L) {
-                // prologue: cells k = x-1 .. 0 all exist — jump into the unrolled sequence at k = x-1
-                switch (x) { PHMM_REP64(PHMM_CASE_PROLOGUE) default: break; }
-                switch (x) { PHMM_REP64(PHMM_CASE_ROW0) default: break; }
-            } else {
-                // reads shorter than the band: both limits apply
-                const int klo = x - L;
+            switch (x) { PHMM_DESC64(PHMM_PRO_ENTRY) default: goto pro_0; }
+            PHMM_DESC64(PHMM_PRO_CHAIN)
+            M[K - 1] = vmin2(w0.y, prmt(caps0, caps1, w0.x));
+        } else {
+            // reads shorter than the band, L < x < 2B: both limits apply; the row-0 value travels in M[2B-1] as in the prologue
+            i_run = (x & 1) ? gop : kInf16x2;
+            const int klo = x - L;
 #pragma unroll
-                for (int k = K - 1; k >= 0; --k) {
-                    if (k < x && k >= klo) PHMM_CELL(k)
-                }
-                switch (x) { PHMM_REP64(PHMM_CASE_ROW0) default: break; }
+            for (int k = K - 2; k >= 0; --k) {
+                if (k == x - 1) M[k] = M[K - 1];
+                if (k < x && k >= klo) PHMM_CELL(k)
             }
+            M[K - 1] = vmin2(w0.y, prmt(caps0, caps1, w0.x));
         }
+    column_end:
         go_prev = go; ge_prev = ge;
         // The next column's entries were loaded at the top of this column and must not be waited for before its end.
         // Left to itself ptxas copies them into e0 / e1 right after issuing the loads (a full L2 round trip per column,
@@ -262,8 +280,9 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
         e0.x = n0.x + z; e0.y = n0.y + z; e1.x = n1.x + z; e1.y = n1.y + z;
     }
 #undef PHMM_CELL
-#undef PHMM_CASE_PROLOGUE
-#undef PHMM_CASE_ROW0
+#undef PHMM_PRO_ENTRY
+#undef PHMM_PRO_CHAIN
+#undef PHMM_EPI_CELL
     uint32_t best = M[0];
 #pragma unroll
     for (int k = 1; k < K; ++k) best = vmin2(best, M[k]);
