@@ -1358,7 +1358,8 @@ PHMM_HD void traceback_walk(const uint32_t* __restrict__ bp, const size_t bps, c
             --y;
             const int k = x - y;
             if (k < 0 || k >= K) { ok = false; break; }
-            ns = (int)((bp[((size_t)x * K + k) * bps] >> 22) & 3u);
+            // the insertion into row 1 comes from row 0, whose cells the forward pass does not store: it opens a run
+            ns = y > 0 ? (int)((bp[((size_t)x * K + k) * bps] >> 22) & 3u) : LM;
             if (align1) { align1[n] = '-'; align2[n] = target[y]; }
             if (x < lhs_flank || x >= rhs_begin) { fs += (ns == LI ? (int)gm.gap_extend[x - 1] : (int)gm.gap_open[x - 1]) + gm.nuc_prior; ++ms; }
         } else {

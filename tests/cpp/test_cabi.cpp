@@ -41,6 +41,13 @@ int main()
         HaplotypeLikelihoodArray arr {cfg};
         arr.populate(reads, haps);
         for (std::size_t h = 0; h < 2; ++h) { const auto row = arr[h]; std::printf("ROW %zu %.17g %.17g\n", h, row[0], row[1]); }
+        {   // the same without mapping quality: -ln10/10 times the integer penalty, to be matched bit for bit
+            auto exact_cfg = cfg;
+            exact_cfg.use_mapping_quality = 0;
+            HaplotypeLikelihoodArray exact {exact_cfg};
+            exact.populate(reads, haps);
+            for (std::size_t h = 0; h < 2; ++h) { const auto row = exact[h]; std::printf("EXACT %zu %.17g %.17g\n", h, row[0], row[1]); }
+        }
         {   // multi-sample container semantics (haplotype_likelihood_array.cpp:200-409): samples are column ranges of one batch
             ReadBlock r0, r1;
             r0.add(h0.substr(30, 40), std::vector<std::uint8_t>(40, 30), 60, false, 30);

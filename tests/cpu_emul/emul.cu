@@ -74,6 +74,24 @@ int emul_generic(int band, int tb, int L, const char* read, const int8_t* q,
     return generic_align<false, kGenericMaxDiag>(band, gm, read, q, L, nullptr, 1, 0, 0, nullptr, nullptr, nullptr);
 }
 
+// The FP64 finish of every populate path, host-compiled from the same source: mapq_terms (the read's share, tabulated by
+// k_mapq_terms), finish_mixed (the pair's share) and finish_likelihood (both in one, as k_epilogue and k_align_reads call it).
+// best == INT_MIN stands for kBestInf (lowest()).
+static int best_of(int s) { return s == INT32_MIN ? kBestInf : s; }
+void emul_mapq_terms(int mapq, int cap, int trigger, double* ln_mapped, double* ln_miss)
+{
+    const MapqTerms t = mapq_terms(mapq, cap, trigger);
+    *ln_mapped = t.ln_mapped; *ln_miss = t.ln_miss;
+}
+void emul_finish_mixed(int n, const int* s, const int* mapq, int use_mapq, int cap, int trigger, double* out)
+{
+    for (int i = 0; i < n; ++i) out[i] = finish_mixed(best_of(s[i]), use_mapq != 0, mapq_terms(mapq[i], cap, trigger));
+}
+void emul_finish_likelihood(int n, const int* s, const int* mapq, int use_mapq, int cap, int trigger, double* out)
+{
+    for (int i = 0; i < n; ++i) out[i] = finish_likelihood(best_of(s[i]), use_mapq != 0, mapq[i], cap, trigger);
+}
+
 } // extern "C"
 
 // The whole per-(haplotype, read) evaluation exactly as the populate kernels perform it, on the CPU:
@@ -283,7 +301,9 @@ extern "C" int emul_traceback(int band, int L, const char* read, const uint8_t* 
     rows[L] = 0;
     std::vector<ColEntry> t(W);
     for (int x = 0; x < W; ++x) t[x] = make_col_entry(truth[x], mask[x], prior[x], go[x], ge[x]);
-    std::vector<uint32_t> bp((size_t)(W + 1) * 2 * band, 0u);
+    // the kernel's back-pointer scratch is reused across calls and never cleared: fill it with words whose every label reads as an
+    // insertion, so a walk that reads a cell the forward pass did not write gives a wrong flank score here too
+    std::vector<uint32_t> bp((size_t)(W + 1) * 2 * band, 0x55555555u);
     int x_end = -1, state = 0;
     const TbModel gm {truth, mask, prior, go, ge, nuc_prior};
     switch (band) {

@@ -5,6 +5,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from exact import assert_mix_within_bound, assert_same_penalties, penalties
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cpp", "test_cabi.cpp")
 EXE = os.path.join(ROOT, "tests", "cpp", "test_cabi")
@@ -24,11 +26,11 @@ def test_cpp_adapter_compiles_against_the_abi():
 
 
 @pytest.mark.gpu
-def test_cpp_client_matches_oracle(coracle):
+def test_cpp_client_matches_oracle_exactly(coracle):
     _build()
     out = subprocess.run([EXE], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stdout + out.stderr
-    lines = dict((l.split()[0] + (l.split()[1] if l.startswith("ROW") else ""), l.split()) for l in out.stdout.strip().splitlines())
+    lines = dict((l.split()[0] + (l.split()[1] if l.startswith(("ROW", "EXACT")) else ""), l.split()) for l in out.stdout.strip().splitlines())
     assert lines["KAT"][1:] == ["84", "84", "0", "CCCCACGTATATATATATATATGGGGACGT", "CCCCACGT---------------GGGACGT"]
     h0 = "ACGTTGCAAGCTTAGGCTAACGTTAGCATCGATCGGATCTAGCTAGGATCGATACGATCGATCGTAGCTAGCTAGTCGATCGATTTAGCGCGATATCGCGAT"
     h1 = list(h0); h1[50] = "C" if h1[50] == "A" else "A"; h1 = "".join(h1)
@@ -37,9 +39,11 @@ def test_cpp_client_matches_oracle(coracle):
     for hi, h in enumerate((h0, h1)):
         for ri, (r, q, p) in enumerate(reads):
             st, want, _ = coracle.model_evaluate(16, h, r, np.full(40, q, np.uint8), np.full(n, 40, np.int8), np.full(n, 3, np.int8), h.encode(),
-                                                 np.full(n, 50, np.int8), [], p, mapping_quality=60)
-            got = float(lines["ROW%d" % hi][2 + ri])
-            assert st == 0 and abs(got - want) <= 1e-4 * max(abs(want), 1e-300)
+                                                 np.full(n, 50, np.int8), [], p, use_mapping_quality=False)
+            assert st == 0
+            exact = np.array([float(lines["EXACT%d" % hi][2 + ri])])
+            assert_same_penalties(exact, np.array([want]), None, np.zeros(1), (hi, ri))       # %.17g round-trips a double
+            assert_mix_within_bound([float(lines["ROW%d" % hi][2 + ri])], penalties([want]), [60], (hi, ri))
     assert lines["SHORT"][1].startswith("hap=0")
     e2e = dict(kv.split("=") for kv in lines["E2E"][1:])
     assert e2e["same"] == "1" and float(e2e["pinned_ms"]) > 0 and float(e2e["pageable_ms"]) > 0

@@ -8,6 +8,7 @@ import sys
 import numpy as np
 import pytest
 
+from exact import assert_same_penalties
 from helpers import random_region
 
 pytestmark = pytest.mark.gpu
@@ -100,29 +101,24 @@ def test_direct_mode_equals_classify_path(both):
 
 
 def test_direct_mode_matches_oracle(both, coracle):
+    """Mapping quality off: bit-equal to the oracle. On (cap 60, trigger 40): within the bound of the exact mix of those penalties."""
+    from test_gpu_parity import mixed_within_bound
     direct, _ = both
     for name, band_req, haps, reads in _single_cases():
-        for use_mq in (True, False):
-            rc, want, wst = coracle.populate(_band(band_req), haps, reads, None, None, use_mapping_quality=use_mq, mapq_cap=60,
-                                             mapq_cap_trigger=40, dp_only=True, map_positions=False)
-            got, st = direct["%s_mq%d_val" % (name, use_mq)], direct["%s_mq%d_st" % (name, use_mq)]
-            ok = wst == 0
-            assert np.array_equal(st & 0xFFFF == 2, wst & 0xFFFF == 2) and np.array_equal(st[~ok], wst[~ok]), name
-            if use_mq:      # mapping-quality mixing: the oracle's libm against CUDA's
-                assert np.allclose(got[ok], want[ok], rtol=1e-4, atol=0), name
-            else:
-                assert np.array_equal(got[ok], want[ok]), name
+        rc, want, wst = coracle.populate(_band(band_req), haps, reads, None, None, use_mapping_quality=False, dp_only=True, map_positions=False)
+        assert_same_penalties(direct["%s_mq0_val" % name], want, direct["%s_mq0_st" % name], wst, name)
+        got, st = direct["%s_mq1_val" % name], direct["%s_mq1_st" % name]
+        assert np.array_equal(st, direct["%s_mq0_st" % name]), name
+        mixed_within_bound(got, want, wst, reads.mapq[None, :], 60, 40, name)
     regions, (_, _, hf, rf) = _region_case()
     off = 0
     for haps, reads in regions:
-        rc, want, wst = coracle.populate(_band(16), haps, reads, None, None, use_mapping_quality=True, mapq_cap=60, mapq_cap_trigger=40,
-                                         dp_only=True, map_positions=False)
+        rc, want, wst = coracle.populate(_band(16), haps, reads, None, None, use_mapping_quality=False, dp_only=True, map_positions=False)
         n = haps.n * reads.n
         st = direct["regions_st"][off:off + n].reshape(haps.n, reads.n)
         got = direct["regions_val"][off:off + n].reshape(haps.n, reads.n)
-        ok = wst == 0
-        assert np.array_equal(st & 0xFFFF == 2, wst & 0xFFFF == 2) and np.array_equal(st[~ok], wst[~ok])
-        assert np.allclose(got[ok], want[ok], rtol=1e-4, atol=0)
+        assert np.array_equal(st != 0, (wst != 0) | (want == -1.7976931348623157e308)) and np.array_equal(st[wst != 0], wst[wst != 0])
+        mixed_within_bound(got, want, wst, reads.mapq[None, :], 60, 40, "regions")
         off += n
 
 

@@ -1,14 +1,15 @@
 """GPU parity tests: the CUDA engine (through the C ABI) against the oracle on the same seeded inputs.
-Integer scores must be bit-exact; final ln-likelihoods must agree to 1e-4 relative (BASELINE.json's bar) — in fact the
-only floating-point work is the double-precision epilogue, so the observed difference is a few ulp."""
+Integer scores must be bit-exact. Every populate-level check runs twice: with mapping quality off, where a value is
+-ln10/10 times its integer penalty and must equal the oracle's bit for bit, and with it on, where the value must lie within
+4 eps (1 + c|s| + c mapq) of the exact mixed value of that penalty (tests/exact.py), the forward-error bound of the reference's
+own double formula."""
 import numpy as np
 import pytest
 
+from exact import (LOWEST, assert_mix_within_bound, assert_same_penalties, assert_sums_within_bound, effective_mapq, penalties)
 from helpers import random_positions, random_region
 
 pytestmark = pytest.mark.gpu
-
-REL_TOL = 1e-4
 
 
 def _tasks_for(rng, haps, reads, band, n):
@@ -81,11 +82,32 @@ def test_align_scores_match_reference_kernel(engine, refkernels):
         assert np.array_equal(got[sel], want)
 
 
-def _close(got, want):
-    got, want = np.asarray(got), np.asarray(want)
-    denom = np.maximum(np.abs(want), 1e-300)
-    bad = np.abs(got - want) > REL_TOL * denom
-    return not bad.any(), float(np.max(np.abs(got - want) / denom))
+def mixed_within_bound(got, want_exact, wst, mapq, cap=120, trig=None, what=""):
+    """The mixed leg: got [H, R] (mapping quality on) against the exact mix of the penalties the exact leg showed equal to the
+    oracle's (want_exact, mapping quality off), at each read's effective mapping quality. Returns the largest error in bound units."""
+    ok = np.asarray(wst) == 0
+    s = penalties(np.where(ok, want_exact, 0.0))
+    mq = np.broadcast_to(effective_mapq(mapq, cap, trig), s.shape)
+    return assert_mix_within_bound(np.asarray(got)[ok], s[ok], mq[ok], what)
+
+
+def populate_legs(engine, coracle, band, haps, reads, positions=None, flanks=None, what="", cap=120, trig=None, dp_only=False,
+                  map_positions=False, **cfg):
+    """One populate scenario in both legs: mapping quality off, bit-exact against the oracle; on, within the bound of the exact mix.
+    cfg: further HaplotypeLikelihoodModel.Config fields (max_indel_error, use_int_scores). Returns (rc, exact values, statuses, largest mixed error in bound units)."""
+    from octopus_b200 import HaplotypeLikelihoodModel
+    rc, want, wst = coracle.populate(band, haps, reads, positions, flanks, use_mapping_quality=False, dp_only=dp_only,
+                                     map_positions=map_positions)
+    for use_mq in (False, True):
+        c = HaplotypeLikelihoodModel.Config(use_mapping_quality=use_mq, mapping_quality_cap=cap, mapping_quality_cap_trigger=trig,
+                                            disable_naive_shortcut=dp_only, map_positions=map_positions, **cfg)
+        got, st = engine.populate(c, haps, reads, positions, flanks, want_status=True)
+        if not use_mq:
+            assert_same_penalties(got, want, st, wst, what)
+        else:
+            assert np.array_equal(st != 0, (wst != 0) | (want == LOWEST)) and np.array_equal(st[wst != 0], wst[wst != 0]), what
+            worst = mixed_within_bound(got, want, wst, reads.mapq[None, :], cap, trig, what)
+    return rc, want, wst, worst
 
 
 @pytest.mark.parametrize("band_req", [8, 12, 16, 32, 40])
@@ -100,23 +122,11 @@ def test_populate_matches_oracle(engine, coracle, band_req):
         positions = random_positions(rng, haps, reads) if trial % 3 else None
         flanks = (int(rng.integers(0, 90)), int(rng.integers(0, 90))) if trial % 2 else None
         for dp_only in (False, True):
-            for use_mq in (True, False):
-                mapit = (trial % 3 == 0) and (trial % 2 == 0 or dp_only)      # positions=None: k-mer mapped on the device, or original only
-                # trial 5: a trigger at or above the cap is ignored (haplotype_likelihood_model.cpp:49-51); trial 3: a low cap that bites
-                trig, cap = {1: (40, 120), 3: (40, 50), 5: (200, 50)}.get(trial, (None, 120))
-                cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band_req, use_mapping_quality=use_mq, mapping_quality_cap=cap,
-                                                      mapping_quality_cap_trigger=trig, disable_naive_shortcut=dp_only,
-                                                      map_positions=mapit)
-                rc, want, wst = coracle.populate(band, haps, reads, positions, flanks, use_mapping_quality=use_mq, mapq_cap=cap,
-                                                 mapq_cap_trigger=-1 if trig is None else trig, dp_only=dp_only, map_positions=mapit)
-                got, st = engine.populate(cfg, haps, reads, positions, flanks, want_status=True)
-                ok_pairs = wst == 0
-                assert np.array_equal((st & 0xFFFF) == 2, (wst & 0xFFFF) == 2)
-                assert np.array_equal(st[~ok_pairs], wst[~ok_pairs])
-                if not use_mq:
-                    assert np.array_equal(got[ok_pairs], want[ok_pairs]), (band_req, trial, dp_only)   # -ln10/10 * integer: exact
-                ok, worst = _close(got[ok_pairs], want[ok_pairs])
-                assert ok, (band_req, trial, dp_only, use_mq, worst)
+            mapit = (trial % 3 == 0) and (trial % 2 == 0 or dp_only)      # positions=None: k-mer mapped on the device, or original only
+            # trial 5: a trigger at or above the cap is ignored (haplotype_likelihood_model.cpp:49-51); trial 3: a low cap that bites
+            trig, cap = {1: (40, 120), 3: (40, 50), 5: (200, 50)}.get(trial, (None, 120))
+            populate_legs(engine, coracle, band, haps, reads, positions, flanks, (band_req, trial, dp_only), cap=cap, trig=trig,
+                          dp_only=dp_only, map_positions=mapit, max_indel_error=band_req)
 
 
 def test_populate_raises_short_haplotype_error(engine):
@@ -175,12 +185,8 @@ def test_populate_with_device_kmer_mapper_matches_reference_loop(engine, coracle
     from octopus_b200 import HaplotypeLikelihoodModel, synth
     haps, reads, band = synth.make_batch("C2", n_reads=700, n_haps=24)
     for flanks in (None, (40, 30)):
-        cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band)
-        got = engine.populate(cfg, haps, reads, flank_state=flanks)
-        rc, want, _ = coracle.populate(band, haps, reads, None, flanks, map_positions=True)
-        assert rc == 0
-        ok, worst = _close(got, want)
-        assert ok, worst
+        rc = populate_legs(engine, coracle, band, haps, reads, None, flanks, flanks, map_positions=True, max_indel_error=band)
+        assert rc[0] == 0
     # repetitive haplotypes: many equally good mapping positions (exercises the <= 10 cap and the tie order)
     rng = np.random.default_rng(4)
     unit = np.frombuffer(b"ACGTTGCAAG", dtype=np.uint8)
@@ -199,10 +205,8 @@ def test_populate_with_device_kmer_mapper_matches_reference_loop(engine, coracle
         if r % 2: b[rng.integers(0, L)] = ord("A")
         rb.append(b); rq.append(rng.integers(10, 41, L).astype(np.uint8)); rbeg.append(p)
     reads2 = pack_reads(rb, rq, begin=np.asarray(rbeg))
-    got = engine.populate(HaplotypeLikelihoodModel.Config(max_indel_error=16), haps2, reads2)
-    rc, want, _ = coracle.populate(16, haps2, reads2, None, None, map_positions=True)
-    ok, worst = _close(got, want)
-    assert rc == 0 and ok, worst
+    rc = populate_legs(engine, coracle, 16, haps2, reads2, None, None, "repetitive", map_positions=True, max_indel_error=16)
+    assert rc[0] == 0
 
 
 def test_align_reads_matches_reference_align(engine, coracle):
@@ -222,20 +226,38 @@ def test_align_reads_matches_reference_align(engine, coracle):
             lists.extend(ps); off.append(len(lists))
         positions = (np.asarray(off, np.int64), np.asarray(lists if lists else [0], np.int32))
         flanks = (int(rng.integers(0, 80)), int(rng.integers(0, 80))) if trial % 2 else None
-        cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band_req, mapping_quality_cap_trigger=40 if trial == 3 else None)
-        mp, lk, cig, st = engine.align_reads(cfg, haps, reads, pairs, positions, flanks)
-        for j, (r, h) in enumerate(pairs):
-            hp = haps.hap(int(h)); b, q = reads.read(int(r)); rev = bool(reads.reverse[r])
-            wst, wmp, wlk, wcig, wext = coracle.model_align(band, hp["seq"].tobytes(), b.tobytes(), q, hp["gap_open"], hp["gap_extend"],
-                                                            hp["snv_mask_rev" if rev else "snv_mask_fwd"].tobytes(), hp["snv_prior_rev" if rev else "snv_prior_fwd"],
-                                                            positions[1][off[j]:off[j + 1]], int(reads.begin[r]), mapping_quality=int(reads.mapq[r]),
-                                                            flanks=flanks, mapq_cap_trigger=40 if trial == 3 else -1)
+        align_reads_legs(engine, coracle, band, band_req, haps, reads, pairs, positions, off, flanks, trig=40 if trial == 3 else None,
+                         what=trial)
+
+
+def align_reads_legs(engine, coracle, band, band_req, haps, reads, pairs, positions, off, flanks, trig=None, what=""):
+    """phmm_align_reads in both legs against HaplotypeLikelihoodModel::align (oracle): mapping position and CIGAR equal, the likelihood
+    bit-equal with mapping quality off and within the bound of the exact mix of that penalty with it on."""
+    from octopus_b200 import HaplotypeLikelihoodModel
+    res = {}
+    for use_mq in (False, True):
+        cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band_req, use_mapping_quality=use_mq, mapping_quality_cap_trigger=trig)
+        res[use_mq] = engine.align_reads(cfg, haps, reads, pairs, positions, flanks)
+    lk_exact, lk_mixed, mq_eff = [], [], []
+    for j, (r, h) in enumerate(pairs):
+        hp = haps.hap(int(h)); b, q = reads.read(int(r)); rev = bool(reads.reverse[r])
+        wst, wmp, wlk, wcig, wext = coracle.model_align(band, hp["seq"].tobytes(), b.tobytes(), q, hp["gap_open"], hp["gap_extend"],
+                                                        hp["snv_mask_rev" if rev else "snv_mask_fwd"].tobytes(), hp["snv_prior_rev" if rev else "snv_prior_fwd"],
+                                                        positions[1][off[j]:off[j + 1]], int(reads.begin[r]), mapping_quality=int(reads.mapq[r]),
+                                                        flanks=flanks, use_mapping_quality=False)
+        for use_mq in (False, True):
+            mp, lk, cig, st = res[use_mq]
             if wst == 1:
-                assert (st[j] & 0xFFFF) == 2 and (st[j] >> 16) == wext
+                assert (st[j] & 0xFFFF) == 2 and (st[j] >> 16) == wext, (what, j)
                 continue
-            assert wst == 0 and st[j] == 0, (trial, j, wst, st[j])
-            assert mp[j] == wmp and cig[j] == wcig, (trial, j, mp[j], wmp, cig[j], wcig)
-            assert abs(lk[j] - wlk) <= REL_TOL * max(abs(wlk), 1e-300)
+            assert wst == 0 and st[j] == 0, (what, j, wst, st[j])
+            assert mp[j] == wmp and cig[j] == wcig, (what, j, use_mq, mp[j], wmp, cig[j], wcig)
+        if wst == 0:
+            lk_exact.append((res[False][1][j], wlk)); lk_mixed.append(res[True][1][j])
+            mq_eff.append(int(effective_mapq([reads.mapq[r]], 120, trig)[0]))
+    got, want = np.array(lk_exact).T
+    assert_same_penalties(got, want, None, np.zeros(len(got), np.int32), what)
+    assert_mix_within_bound(np.array(lk_mixed), penalties(want), np.array(mq_eff), what)
 
 
 def test_genotype_likelihood_reduction_on_the_resident_matrix(engine, coracle):
@@ -288,15 +310,16 @@ def test_populate_edge_cases(engine, coracle):
     ]
     for rk, ck in cases:
         haps, reads = region(**rk)
-        cfg = HaplotypeLikelihoodModel.Config(map_positions=False, **ck)
-        band = HaplotypeLikelihoodModel(cfg).pad_requirement()
+        band = HaplotypeLikelihoodModel(HaplotypeLikelihoodModel.Config(**ck)).pad_requirement()
         for flanks in (None, (30, 25)):
-            rc, want, wst = coracle.populate(band, haps, reads, None, flanks)
-            got, st = engine.populate(cfg, haps, reads, flank_state=flanks, want_status=True)
-            ok = wst == 0
-            assert np.array_equal((st & 0xFFFF) == 2, (wst & 0xFFFF) == 2), (rk, ck)
-            good, worst = _close(got[ok], want[ok])
-            assert good, (rk, ck, flanks, worst)
+            populate_legs(engine, coracle, band, haps, reads, None, flanks, (rk, ck, flanks), **ck)
+        if rk["qmax"] > 127:
+            # qualities above 127 can make a penalty negative, which the finish clamps to 0.0: check the integers themselves
+            tasks = np.array([(r, h, int(reads.begin[r]) - band, int(reads.reverse[r])) for r in range(reads.n) for h in range(haps.n)
+                              if 0 <= int(reads.begin[r]) - band and int(reads.begin[r]) + reads.length(r) + band - 1 <= haps.length(h)], np.int32)
+            assert len(tasks)
+            got = engine.align_scores(band, haps, reads, tasks, nuc_prior=2, precision_bits=32)
+            assert np.array_equal(got, _oracle_scores(coracle, haps, reads, band, tasks, 2)), (rk, ck)
     with pytest.raises(Exception) as ei:
         engine.populate(HaplotypeLikelihoodModel.Config(max_indel_error=300), *region(hap_len=120, read_lens=[40], n_haps=1, qmax=41))
     assert "256" in str(ei.value)
@@ -311,15 +334,17 @@ def test_populate_templates_sums_the_reads_of_each_template(engine, coracle):
     while sum(sizes) < reads.n:
         sizes.append(min(int(rng.choice([1, 2, 2, 2, 3])), reads.n - sum(sizes)))
     toff = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-    cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band)
-    got = engine.populate_templates(cfg, haps, reads, toff, flank_state=(50, 40))
-    rc, per_read, _ = coracle.populate(band, haps, reads, None, (50, 40), map_positions=True)
+    rc, per_read, wst = coracle.populate(band, haps, reads, None, (50, 40), use_mapping_quality=False, map_positions=True)
+    assert rc == 0 and (wst == 0).all()
     want = np.zeros((haps.n, len(sizes)))
     for t in range(len(sizes)):
         for r in range(toff[t], toff[t + 1]):
             want[:, t] = want[:, t] + per_read[:, r]
-    ok, worst = _close(got, want)
-    assert rc == 0 and ok, worst
+    exact = engine.populate_templates(HaplotypeLikelihoodModel.Config(max_indel_error=band, use_mapping_quality=False), haps, reads, toff,
+                                      flank_state=(50, 40))
+    assert np.array_equal(exact, want)           # both sides add the reads' -ln10/10 * s in read order
+    got = engine.populate_templates(HaplotypeLikelihoodModel.Config(max_indel_error=band), haps, reads, toff, flank_state=(50, 40))
+    assert_sums_within_bound(got, penalties(per_read), reads.mapq[None, :], toff, "templates")
 
 
 def test_multi_sample_array_is_one_batch_with_per_sample_views(engine, coracle):
@@ -333,15 +358,19 @@ def test_multi_sample_array_is_one_batch_with_per_sample_views(engine, coracle):
     before = engine.launch_count(total=True)
     arr = HaplotypeLikelihoodArray(model, engine).populate(parts, haps, flank_state=(40, 40))
     one_call = engine.launch_count(total=True) - before
-    rc, want, _ = coracle.populate(band, haps, reads, None, (40, 40), map_positions=True)
+    exact = HaplotypeLikelihoodArray(HaplotypeLikelihoodModel(HaplotypeLikelihoodModel.Config(max_indel_error=band, use_mapping_quality=False)),
+                                     engine).populate(parts, haps, flank_state=(40, 40))
+    rc, want, wst = coracle.populate(band, haps, reads, None, (40, 40), use_mapping_quality=False, map_positions=True)
     assert rc == 0 and arr.samples() == ["NA1", "NA2", "NA3"]
     lo = 0
     for name, block in parts.items():
-        ok, worst = _close(arr.extract_sample(name), want[:, lo:lo + block.n])
-        assert ok, (name, worst)
+        sl = slice(lo, lo + block.n)
+        assert_same_penalties(exact.extract_sample(name), want[:, sl], None, wst[:, sl], name)
+        mixed_within_bound(arr.extract_sample(name), want[:, sl], wst[:, sl], reads.mapq[None, sl], what=name)
         lo += block.n
     merged = arr.merge_samples()
-    assert merged.is_primed() and merged.num_likelihoods() == reads.n and _close(np.stack([merged[h] for h in range(haps.n)]), want)[0]
+    assert merged.is_primed() and merged.num_likelihoods() == reads.n
+    mixed_within_bound(np.stack([merged[h] for h in range(haps.n)]), want, wst, reads.mapq[None, :], what="merged")
     engine.populate(model.config, haps, reads, flank_state=(40, 40))
     assert one_call == engine.launch_count()          # the three samples cost exactly one populate call's launches
 
@@ -349,8 +378,8 @@ def test_multi_sample_array_is_one_batch_with_per_sample_views(engine, coracle):
 def test_populate_matches_the_compiled_reference_populate(engine, refhmm):
     """The CUDA engine against the reference's OWN HaplotypeLikelihoodArray::populate (haplotype_likelihood_array.cpp compiled from
     the reference checkout, oracle/_ref/libref_hmm.so) — no restatement in between: same haplotypes, reads,
-    flank state and configuration in, the same [H][R] ln-likelihoods out (integer penalties identical; the double epilogue to 1e-4
-    relative, in practice a few ulp)."""
+    flank state and configuration in, the same [H][R] ln-likelihoods out (integer penalties identical: with mapping quality off the values are
+    bit-equal; with it on they lie within the bound of the exact mix)."""
     if refhmm is None:
         pytest.skip("oracle/_ref/libref_hmm.so not built")
     from octopus_b200 import HaplotypeLikelihoodModel, synth
@@ -366,15 +395,19 @@ def test_populate_matches_the_compiled_reference_populate(engine, refhmm):
         flanks = (int(rng.integers(0, 80)), int(rng.integers(0, 80))) if trial % 2 else None
         trig, cap = {1: (40, 120), 3: (40, 50), 5: (200, 50)}.get(trial, (None, 120))
         cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band_req, mapping_quality_cap=cap, mapping_quality_cap_trigger=trig)
-        st, want, _ = refhmm.array_populate(band_req, haps, reads, flanks=flanks, mapq_cap=cap, mapq_cap_trigger=-1 if trig is None else trig)
+        st, want, _ = refhmm.array_populate(band_req, haps, reads, flanks=flanks, use_mapping_quality=False)
         if st == 1:
             from octopus_b200.api import ShortHaplotypeError
             with pytest.raises(ShortHaplotypeError):
                 engine.populate(cfg, haps, reads, None, flanks)
             continue
+        cfg.use_mapping_quality = False
+        exact = engine.populate(cfg, haps, reads, None, flanks)
+        z = np.zeros(want.shape, np.int32)
+        assert_same_penalties(exact, want, None, z, trial)
+        cfg.use_mapping_quality = True
         got = engine.populate(cfg, haps, reads, None, flanks)
-        ok, worst = _close(got, want)
-        assert ok and np.array_equal(got == 0.0, want == 0.0), (trial, worst)
+        mixed_within_bound(got, want, z, reads.mapq[None, :], cap, trig, trial)
 
 
 def test_flank_discount_with_n_columns_matchable_below_two(engine, coracle, refhmm):

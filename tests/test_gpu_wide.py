@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 
 from helpers import ACGT, random_positions, random_region
-from test_gpu_parity import _close, _oracle_scores, _tasks_for
+from exact import assert_same_penalties
+from test_gpu_parity import _oracle_scores, _tasks_for, align_reads_legs, mixed_within_bound, populate_legs
 
 pytestmark = pytest.mark.gpu
 
@@ -66,14 +67,8 @@ def test_populate_wide_bands_match_oracle(engine, coracle, band_req):
         flanks = (int(rng.integers(0, 90)), int(rng.integers(0, 90))) if trial == 3 else None
         for dp_only in (False, True):
             for int_scores in (False, True):
-                cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band_req, disable_naive_shortcut=dp_only, map_positions=False,
-                                                      use_int_scores=int_scores)
-                rc, want, wst = coracle.populate(band, haps, reads, positions, flanks, dp_only=dp_only, map_positions=False)
-                got, st = engine.populate(cfg, haps, reads, positions, flanks, want_status=True)
-                ok_pairs = wst == 0
-                assert np.array_equal(st[~ok_pairs], wst[~ok_pairs])
-                ok, worst = _close(got[ok_pairs], want[ok_pairs])
-                assert ok, (band_req, trial, dp_only, int_scores, worst)
+                populate_legs(engine, coracle, band, haps, reads, positions, flanks, (band_req, trial, dp_only, int_scores), dp_only=dp_only,
+                              max_indel_error=band_req, use_int_scores=int_scores)
 
 
 def test_populate_int_scores_and_unsafe_reads_equal_the_default(engine, coracle):
@@ -86,14 +81,9 @@ def test_populate_int_scores_and_unsafe_reads_equal_the_default(engine, coracle)
         reads.quals[:] = np.where(rng.random(len(reads.quals)) < 0.9, 41, reads.quals)      # long reads: quality sum ~ 30 000 > 16-bit budget
         for flanks in (None, (120, 150)):
             for mapit in (False, True):
-                rc, want, wst = coracle.populate(band, haps, reads, None, flanks, map_positions=mapit)
                 for int_scores in (False, True):
-                    cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band, use_int_scores=int_scores, map_positions=mapit)
-                    got, st = engine.populate(cfg, haps, reads, None, flanks, want_status=True)
-                    ok_pairs = wst == 0
-                    assert np.array_equal(st[~ok_pairs], wst[~ok_pairs])
-                    ok, worst = _close(got[ok_pairs], want[ok_pairs])
-                    assert ok, (band, flanks, mapit, int_scores, worst)
+                    populate_legs(engine, coracle, band, haps, reads, None, flanks, (band, flanks, mapit, int_scores), map_positions=mapit,
+                                  max_indel_error=band, use_int_scores=int_scores)
 
 
 def test_populate_long_candidate_lists(engine, coracle):
@@ -108,12 +98,8 @@ def test_populate_long_candidate_lists(engine, coracle):
     positions = pack_positions(lists, haps.n, reads.n)
     for flanks in (None, (50, 60)):
         for dp_only in (True, False):
-            cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band, disable_naive_shortcut=dp_only)
-            rc, want, wst = coracle.populate(band, haps, reads, positions, flanks, dp_only=dp_only)
-            got, st = engine.populate(cfg, haps, reads, positions, flanks, want_status=True)
-            ok_pairs = wst == 0
-            ok, worst = _close(got[ok_pairs], want[ok_pairs])
-            assert ok, (flanks, dp_only, worst)
+            populate_legs(engine, coracle, band, haps, reads, positions, flanks, (flanks, dp_only), dp_only=dp_only, map_positions=True,
+                          max_indel_error=band)
 
 
 def test_populate_h1024_shape(engine, coracle):
@@ -121,12 +107,7 @@ def test_populate_h1024_shape(engine, coracle):
     from octopus_b200 import HaplotypeLikelihoodModel, synth
     haps, reads, band = synth.make_batch("C5", n_reads=48)
     assert haps.n == 1024
-    cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band, disable_naive_shortcut=True, map_positions=False)
-    got = engine.populate(cfg, haps, reads)
-    rc, want, _ = coracle.populate(band, haps, reads, dp_only=True, map_positions=False)
-    assert rc == 0
-    ok, worst = _close(got, want)
-    assert ok, worst
+    assert populate_legs(engine, coracle, band, haps, reads, what="H1024", dp_only=True, max_indel_error=band)[0] == 0
 
 
 def test_populate_c4_shape_vs_oracle(engine, coracle):
@@ -135,11 +116,7 @@ def test_populate_c4_shape_vs_oracle(engine, coracle):
     haps, reads, band = synth.make_batch("C4", n_reads=300, n_haps=40)
     assert band == 32
     for dp_only in (True, False):
-        cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band, disable_naive_shortcut=dp_only, map_positions=False)
-        got = engine.populate(cfg, haps, reads)
-        rc, want, _ = coracle.populate(band, haps, reads, dp_only=dp_only, map_positions=False)
-        ok, worst = _close(got, want)
-        assert ok, (dp_only, worst)
+        populate_legs(engine, coracle, band, haps, reads, what=("C4", dp_only), dp_only=dp_only, max_indel_error=band)
 
 
 def test_populate_with_error_model_penalties(engine, coracle):
@@ -174,13 +151,7 @@ def test_populate_with_error_model_penalties(engine, coracle):
     reads = pack_reads(bases, quals, reverse=(rng.random(120) < 0.5).astype(np.uint8), begin=np.asarray(begin, np.int64))
     for flanks in (None, (40, 60)):
         for mapit in (False, True):
-            cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band, map_positions=mapit)
-            got, st = engine.populate(cfg, haps, reads, None, flanks, want_status=True)
-            rc, want, wst = coracle.populate(band, haps, reads, None, flanks, map_positions=mapit)
-            ok_pairs = wst == 0
-            assert np.array_equal(st[~ok_pairs], wst[~ok_pairs])
-            ok, worst = _close(got[ok_pairs], want[ok_pairs])
-            assert ok, (flanks, mapit, worst)
+            populate_legs(engine, coracle, band, haps, reads, None, flanks, (flanks, mapit), map_positions=mapit, max_indel_error=band)
 
 
 def test_device_mapper_takes_long_haplotypes(engine, coracle):
@@ -212,13 +183,7 @@ def test_device_mapper_takes_long_haplotypes(engine, coracle):
             bases.append(b); quals.append(rng.integers(10, 42, L).astype(np.uint8)); begin.append(p)
         reads = pack_reads(bases, quals, begin=np.asarray(begin, np.int64))
         for flanks in (None, (500, 700)):
-            cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band, map_positions=True)
-            got, st = engine.populate(cfg, haps, reads, None, flanks, want_status=True)
-            rc, want, wst = coracle.populate(band, haps, reads, None, flanks, map_positions=True)
-            ok_pairs = wst == 0
-            assert np.array_equal(st[~ok_pairs], wst[~ok_pairs])
-            ok, worst = _close(got[ok_pairs], want[ok_pairs])
-            assert ok, (hap_len, flanks, worst)
+            populate_legs(engine, coracle, band, haps, reads, None, flanks, (hap_len, flanks), map_positions=True, max_indel_error=band)
 
 
 def test_lean_flank_kernel_geometries(engine, coracle):
@@ -236,13 +201,8 @@ def test_lean_flank_kernel_geometries(engine, coracle):
                 reads.quals[rng.random(len(reads.quals)) < 0.1] = 0
             for flanks in ((0, 0), (30, 40), (int(hap_len * 0.45), int(hap_len * 0.45)), (hap_len // 2, hap_len // 2 + 5), (hap_len - 10, 0), (0, hap_len - 20)):
                 for mapit in (False, True):
-                    cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band, map_positions=mapit)
-                    got, st = engine.populate(cfg, haps, reads, None, flanks, want_status=True)
-                    rc, want, wst = coracle.populate(band, haps, reads, None, flanks, map_positions=mapit)
-                    ok_pairs = wst == 0
-                    assert np.array_equal(st[~ok_pairs], wst[~ok_pairs])
-                    ok, worst = _close(got[ok_pairs], want[ok_pairs])
-                    assert ok, (band, trial, flanks, mapit, worst)
+                    populate_legs(engine, coracle, band, haps, reads, None, flanks, (band, trial, flanks, mapit), map_positions=mapit,
+                                  max_indel_error=band)
 
 
 def test_reserved_sms_leave_results_unchanged(coracle):
@@ -259,9 +219,12 @@ def test_reserved_sms_leave_results_unchanged(coracle):
         for n in (8, 100, 147, 10**6):
             eng.reserve_sms(n)
             assert np.array_equal(eng.populate(cfg, haps, reads, None, flanks), base), (band, n)
-        rc, want, wst = coracle.populate(band, haps, reads, None, flanks, dp_only=not mapit, map_positions=mapit)
-        ok, worst = _close(base[wst == 0], want[wst == 0])
-        assert ok, (band, worst)
+        eng.reserve_sms(0)
+        cfg.use_mapping_quality = False
+        rc, want, wst = coracle.populate(band, haps, reads, None, flanks, use_mapping_quality=False, dp_only=not mapit, map_positions=mapit)
+        exact, st = eng.populate(cfg, haps, reads, None, flanks, want_status=True)
+        assert_same_penalties(exact, want, st, wst, band)
+        mixed_within_bound(base, want, wst, reads.mapq[None, :], what=band)
     eng.close()
 
 
@@ -301,12 +264,15 @@ def test_populate_regions_equals_one_call_per_region(engine, coracle):
         flat, off, st = engine.populate_regions(cfg, haps, reads, hf, rf, flank_states=flanks, want_status=True)
         mats = engine.split_regions(flat, off, hf, rf)
         sts = engine.split_regions(st, off, hf, rf)
+        cfg_exact = HaplotypeLikelihoodModel.Config(max_indel_error=band, use_mapping_quality=False, disable_naive_shortcut=dp_only, map_positions=mapit)
+        flat_x, off_x, st_x = engine.populate_regions(cfg_exact, haps, reads, hf, rf, flank_states=flanks, want_status=True)
+        mats_x, sts_x = engine.split_regions(flat_x, off_x, hf, rf), engine.split_regions(st_x, off_x, hf, rf)
         for g, (h, r) in enumerate(zip(hap_blocks, read_blocks)):
-            rc, want, wst = coracle.populate(band, h, r, None, flanks[g], dp_only=dp_only, map_positions=mapit)
+            rc, want, wst = coracle.populate(band, h, r, None, flanks[g], use_mapping_quality=False, dp_only=dp_only, map_positions=mapit)
             ok_pairs = wst == 0
-            assert np.array_equal(sts[g][~ok_pairs], wst[~ok_pairs]), (band, g)
-            ok, worst = _close(mats[g][ok_pairs], want[ok_pairs])
-            assert ok, (band, mapit, g, worst)
+            assert_same_penalties(mats_x[g], want, sts_x[g], wst, (band, g))
+            assert np.array_equal(sts[g], sts_x[g]), (band, g)
+            mixed_within_bound(mats[g], want, wst, r.mapq[None, :], what=(band, mapit, g))
             one, _ = engine.populate(cfg, h, r, None, flanks[g], want_status=True)
             assert np.array_equal(one[ok_pairs], mats[g][ok_pairs]), (band, g)
 
@@ -315,7 +281,6 @@ def test_align_reads_register_traceback_and_fallbacks(engine, coracle):
     """phmm_align_reads with the register traceback kernel (bands <= 32) and the generic kernel side by side: long reads beyond the
     register kernel's shared-memory budget, reads with 'N', wide bands — each pair against HaplotypeLikelihoodModel::align (oracle)."""
     from octopus_b200 import HaplotypeLikelihoodModel
-    from test_gpu_parity import REL_TOL
     rng = np.random.default_rng(97)
     for band_req, lens, hap_len in ((8, [30, 76], 300), (16, [76, 150, 900], 1200), (32, [100, 250], 600), (64, [100, 150], 500)):
         band = HaplotypeLikelihoodModel(HaplotypeLikelihoodModel.Config(max_indel_error=band_req)).pad_requirement()
@@ -328,19 +293,7 @@ def test_align_reads_register_traceback_and_fallbacks(engine, coracle):
             lists.extend(ps); off.append(len(lists))
         positions = (np.asarray(off, np.int64), np.asarray(lists if lists else [0], np.int32))
         flanks = (int(rng.integers(0, 80)), int(rng.integers(0, 80))) if band_req != 16 else None
-        cfg = HaplotypeLikelihoodModel.Config(max_indel_error=band_req)
-        mp, lk, cig, st = engine.align_reads(cfg, haps, reads, pairs, positions, flanks)
-        for j, (r, h) in enumerate(pairs):
-            hp = haps.hap(int(h)); b, q = reads.read(int(r)); rev = bool(reads.reverse[r])
-            wst, wmp, wlk, wcig, wext = coracle.model_align(band, hp["seq"].tobytes(), b.tobytes(), q, hp["gap_open"], hp["gap_extend"],
-                                                            hp["snv_mask_rev" if rev else "snv_mask_fwd"].tobytes(), hp["snv_prior_rev" if rev else "snv_prior_fwd"],
-                                                            positions[1][off[j]:off[j + 1]], int(reads.begin[r]), mapping_quality=int(reads.mapq[r]), flanks=flanks)
-            if wst == 1:
-                assert (st[j] & 0xFFFF) == 2 and (st[j] >> 16) == wext
-                continue
-            assert wst == 0 and st[j] == 0, (band_req, j, wst, st[j])
-            assert mp[j] == wmp and cig[j] == wcig, (band_req, j, mp[j], wmp, cig[j], wcig)
-            assert abs(lk[j] - wlk) <= REL_TOL * max(abs(wlk), 1e-300)
+        align_reads_legs(engine, coracle, band, band_req, haps, reads, pairs, positions, off, flanks, what=band_req)
 
 
 def test_align_pairs_equals_the_mutation_model_hmm(engine, refhmm):
