@@ -1117,6 +1117,12 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
     // the 32-bit flank kernel over the current list (near-flank candidates, and every candidate of pair-list reads holding 'N')
     static const bool no_flank_fb = std::getenv("PHMM_NO_FLANK_FB") != nullptr;           // measurement hook: the labelled one-alignment-per-thread flank kernels only
     const bool flank_fb_ok = !no_flank_fb && band <= kFlankFbMaxBand;
+    // Whether a tile's flank kernels run: bands above 32 have none, and on the wide list the labelled kernel needs a warp's row
+    // entries of the call's longest read in shared memory (reads of 6 400+ bases do not fit). The classify pass reads this decision:
+    // near-flank candidates of a tile whose flank kernels do not run take the traceback queue (k_slow_flank) instead.
+    const bool pair_flank_kernels = band <= 32;
+    const bool wide_flank_kernels = band <= 32 && (wide_row_stride <= fast_row_stride + 8 ||
+                                                   (size_t)kFastWarpsPerBlock * wide_row_stride * sizeof(RowEntry) <= (200u << 10));
     auto launch_flank = [&](int n_entries, int row_stride) -> int {
         if (band > 32) return PHMM_OK;              // wide bands: near-flank candidates take the traceback queue
         if (p.atasks && p.fb_route) {
@@ -1192,6 +1198,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
             p.list = p.pair_reads; p.list_kind = 0; p.n_list = 2 * np; p.list_base = (int)(2 * p0);
             p.row_stride = fast_row_stride;
             p.fb_route = (p.atasks && flank_fb_ok) ? 1 : 0;
+            p.flank_kernels = pair_flank_kernels ? 1 : 0;
             if (use_mapper) {
                 launch_mapper(p.list, p.n_list, p.list_base, 0);
                 LAUNCHED();
@@ -1233,6 +1240,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
             p.list = e->wide_reads.as<int>() + w0; p.list_kind = 1; p.n_list = nw; p.list_base = (int)w0;
             p.row_stride = wide_row_stride;
             p.fb_route = 0;
+            p.flank_kernels = wide_flank_kernels ? 1 : 0;
             const long long threads = (long long)nw * H;
             const unsigned cgrid = (unsigned)std::max<long long>(1, std::min<long long>((threads + 127) / 128, (long long)e->sm_count * 64));
             if (use_mapper) {
@@ -1256,15 +1264,14 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
             PHMM_WIDE_DISPATCH(PHMM_WIDE_LAUNCH)
             LAUNCHED();
             if (time_wide) { CU(cudaEventRecord(e->tile_events[2 * n_timed + 1], e->stream)); ++n_timed; timed = true; }
-            if (wide_row_stride <= fast_row_stride + 8 || (size_t)kFastWarpsPerBlock * wide_row_stride * sizeof(RowEntry) <= (200u << 10)) {
-                if ((rc = launch_flank(nw, wide_row_stride))) return rc;
-            }
+            if (p.flank_kernels && (rc = launch_flank(nw, wide_row_stride))) return rc;
             if (direct) { k_list_slots<<<cgrid, 128, 0, e->stream>>>(p, false); LAUNCHED(); }
             w0 += nw;
         } else {
             const int ng = (int)std::min<long long>(reads_per_tile, n_generic - g0);
             p.list = e->generic_reads.as<int>() + g0; p.list_kind = 2; p.n_list = ng; p.list_base = (int)g0;
             p.fb_route = 0;
+            p.flank_kernels = 0;
             // ng is an upper bound (normally there are no generic reads at all): grid-stride kernels on a bounded grid
             const long long threads = (long long)ng * H;
             const unsigned ggrid = (unsigned)std::max<long long>(1, std::min<long long>((threads + 63) / 64, (long long)e->sm_count * 32));

@@ -430,6 +430,7 @@ struct PopParams {
     int* acc_cursor;
     int* any_acc_tasks;
     int fb_route;               // the atasks lists of this tile go to k_flank_fwd / k_flank_bwd (pair list, bands <= 16): any flank geometry, reads of >= 2*band bases
+    int flank_kernels;          // this tile's gtasks / atasks lists are consumed (launch_flank runs); 0: near-flank candidates take the traceback queue
     int* fb_cursor;             // work counter of k_flank_bwd (k_flank_fwd uses acc_cursor)
     int* fb_rounds;             // rounds of forward scratch handed out so far (this tile)
     int* fb_round_base;         // per list slot: first round of the read's forward scratch, -1 = none left
@@ -1274,7 +1275,7 @@ __device__ __forceinline__ void populate_one_pair(const PopParams& p, const int 
                     best = min(best, generic_align<false, MAXK>(p.band, gm, rv.bases, (const int8_t*)rv.quals, rv.len, nullptr, 1, 0, 0, nullptr, nullptr, nullptr));
                 }
             } else {
-                if (FASTQ && p.band <= 32 && !(p.rd.info[r].y & kReadUnsafeFlank32)) {
+                if (FASTQ && p.flank_kernels && !(p.rd.info[r].y & kReadUnsafeFlank32)) {
                     // which flank-aware kernel: window-coordinate flanks of this candidate (pair_hmm.hpp:573-588)
                     int route = 0;                                   // 0: crossing-cell kernel, 1: lean kernel, 2: plain score-only DP
                     if ((pend_flank >> i2) & 1u) {
