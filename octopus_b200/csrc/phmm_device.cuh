@@ -168,7 +168,8 @@ inline uint32_t fma_add(uint32_t a, uint32_t b, uint32_t one) { return a * one +
 //
 // rows : shared-memory row entries of this lane's read pair, rows[0..L-1] real, rows[L] = pad_row_entry()
 // t0/t1: column tables of the two haplotype windows (already offset to the window start); W = L + 2*BAND - 1
-//        entries are read at indices 0..W-1 only
+//        entries are read at indices 0..W-1 only, column x at t[x * CS]. The kernels use CS = 1 (the haplotype-major tables);
+//        tools/ubench_colgather.cu runs CS = 32 over haplotype-interleaved tiles, a layout measured and rejected (DESIGN.md §4)
 // Returns best0 | best1 << 16 (each the integer phred score of reference hmm.align()).
 //
 // Column x holds the cells k = x - y, k in [max(0, x-L), min(2B-1, x)], processed in DESCENDING k so that the
@@ -196,7 +197,7 @@ inline uint32_t fma_add(uint32_t a, uint32_t b, uint32_t one) { return a * one +
 //   min(d + ge, min(m, i) + go) == min(d + ge, min(m, i, d) + go)        (d + go >= d + ge)
 // and the deletion update re-uses S = min(m, i, d), which the match update needs anyway: 5 ALU-pipe instructions per cell pair
 // instead of 6 (the ALU pipe is what binds this kernel, DESIGN.md section 4).
-template <int BAND, bool OGE = false>
+template <int BAND, bool OGE = false, int CS = 1>
 PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
                          const ColEntry* __restrict__ t0, const ColEntry* __restrict__ t1,
                          const uint32_t nucp /* nuc_prior in both halves */,
@@ -212,15 +213,19 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
     uint32_t go_prev = 0u, ge_prev = 0u;
     const RowEntry w0 = rows[0];
 
+    // Every use of the old m (the insertion's m + gop, the deletion's operands) comes before M[k] is written, so the old value is dead
+    // when the new one lands and ptxas updates M[k] in place. With m + gop taken after the write it kept m alive in a copy: 15 moves
+    // per steady column and up to 24 in an epilogue cell (DESIGN.md §4).
 #define PHMM_CELL(k)                                                                        \
     {                                                                                       \
         const RowEntry w   = rp[-(k)];                                                      \
         const uint32_t sub = vmin2(w.y, prmt(caps0, caps1, w.x));                           \
         const uint32_t m = M[(k) < K ? (k) : 0], d = D[(k) < K ? (k) : 0];                  \
         const uint32_t s = vmin3(m, i_run, d);                                              \
-        M[(k) < K ? (k) : 0] = fma_add(s, sub, one);                                        \
+        const uint32_t mg = fma_add(m, gop, one);                                           \
         if ((k) + 1 < K) D[((k) + 1) < K ? (k) + 1 : 0] = vaddmin(d, ge, fma_add(OGE ? s : vmin2(m, i_run), go, one)); \
-        i_run = vaddmin(i_run, gep, fma_add(m, gop, one));                                  \
+        M[(k) < K ? (k) : 0] = fma_add(s, sub, one);                                        \
+        i_run = vaddmin(i_run, gep, mg);                                                    \
     }
     // prologue: the entry cell k = x-1 of column x reads the row-0 value of column x-1 from M[2B-1] instead of M[x-1], then jumps
     // into the shared chain at k = x-2: one dispatch per column and no indexed store of the row-0 value
@@ -231,7 +236,7 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
 
     for (int x = 0; x <= W; ++x) {
         const int xn = (x + 1 < W) ? x + 1 : W - 1;
-        const ColEntry n0 = ldg(t0 + xn), n1 = ldg(t1 + xn);
+        const ColEntry n0 = ldg(t0 + xn * CS), n1 = ldg(t1 + xn * CS);
         const uint32_t caps0 = e0.x, caps1 = e1.x;
         const uint32_t go = prmt(e0.y, e1.y, 0x3430u);   // gap_open[x]   of both halves (byte 3 of .y is the zero source)
         const uint32_t ge = prmt(e0.y, e1.y, 0x3531u);   // gap_extend[x]
