@@ -19,7 +19,7 @@
  * synchronous (results complete on return) unless stated; functions return PHMM_OK or a negative error code
  * and never throw — the C++ adapter (octopus_b200/cpp/phmm_b200.hpp) re-throws the reference's exceptions.
  * An engine handle is not re-entrant (one per host thread, like the reference's per-thread model copies,
- * haplotype_likelihood_array.cpp:172).
+ * haplotype_likelihood_array.cpp:172); threads that want to share one engine use a phmm_batcher.
  * There is no CPU fallback: every entry point that computes fails with PHMM_ERR_CUDA when no H100 is usable.
  */
 #ifndef PHMM_B200_H
@@ -256,6 +256,56 @@ int phmm_populate_templates(phmm_engine* e, const phmm_config* cfg,
                             const int64_t* template_off, int32_t n_templates,
                             const phmm_positions* positions, const phmm_flank_state* flank,
                             double* out, int32_t* status, int space);
+
+/* ---------------------------------------------------------------------------------------------------------------------
+ * Shared engine for many host threads. Octopus runs one populate per active region, one region after the other per region
+ * task, and many region tasks on a thread pool (core/octopus.cpp:867-895): many small synchronous requests from many threads at
+ * once. A batcher owns one engine; the requests that concurrent threads have in flight are merged into one
+ * phmm_populate_regions call (one kernel chain for all of them).
+ *
+ * Policy: the first request to join an empty batch leads it. The leader waits until `clients` requests wait in the batcher
+ * (every open batch and every request that runs alone counts), until max_wait_us have passed since it joined, or until the batch
+ * is full (65535 haplotypes, or an internal pair / staging budget); and until the engine has finished the previous call. It then
+ * seals the batch and makes the call; the other members copy their own slices of the result out. Each thread copies its own
+ * request into the batch's page-locked staging, so packing runs in parallel; two or more staging sets alternate, so the next
+ * batch fills while one is on the GPU. Only requests with identical phmm_config share a batch. The library starts no thread.
+ * Requests with explicit positions, requests phmm_populate would pipeline (>= twice its chunk size in pairs) and requests with
+ * more than 65535 haplotypes or a haplotype longer than 65535 bp run alone on the batcher's engine, in turn with the batches.
+ *
+ * Contract: a request's return code, status and its out at every pair whose status is PHMM_STATUS_OK are bit for bit what
+ * phmm_populate / phmm_populate_templates return for it alone on its own engine. Every request is checked on its own thread,
+ * with phmm_populate's checks and messages, before it joins a batch (the [0,127] penalty check included, on the host); a
+ * failing request returns at once and never changes another request's result. When a request fails with another code than
+ * PHMM_ERR_SHORT_HAPLOTYPE, its out and status are unspecified. Errors of the whole call (CUDA, NOMEM) go to every member.
+ * ------------------------------------------------------------------------------------------------------------------- */
+typedef struct phmm_batcher phmm_batcher;
+typedef struct {
+    int32_t clients;       /* threads expected to submit; a batch is sent once this many requests wait (0 = deadline only) */
+    int32_t max_wait_us;   /* longest time the first request of a batch waits for company */
+} phmm_batcher_options;
+typedef struct {
+    int64_t requests;              /* requests that reached the GPU (batched or alone) */
+    int64_t gpu_calls;             /* engine calls: batches + requests run alone */
+    int64_t merged_calls;          /* calls that carried more than one request */
+    int64_t max_regions_per_call;  /* most requests in one call */
+    int64_t dp_cells;              /* phmm_last_dp_cells summed over the calls */
+} phmm_batcher_stats;
+
+/* device < 0: current CUDA device. opt NULL = defaults (clients 0, max_wait_us 500). PHMM_ERR_CUDA without a usable H100. */
+int  phmm_batcher_create(phmm_batcher** out, int device, const phmm_batcher_options* opt);
+/* Waits until no request is in flight, then frees the engine and the staging. */
+void phmm_batcher_destroy(phmm_batcher* b);
+/* Thread-local: the message of this thread's last failing batcher call. */
+const char* phmm_batcher_last_error(void);
+/* Thread-safe and blocking; host memory only. Arguments, return code, out and status as phmm_populate (space = host). */
+int  phmm_batcher_populate(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                           const phmm_positions* positions, const phmm_flank_state* flank, double* out, int32_t* status);
+/* As phmm_populate_templates without position lists: the request runs as a read request, its thread then sums its rows into
+ * [H][n_templates] left to right from 0.0 (the order of the device's template sum). status (optional) stays per read. */
+int  phmm_batcher_populate_templates(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                                     const int64_t* template_off, int32_t n_templates, const phmm_flank_state* flank,
+                                     double* out, int32_t* status);
+int  phmm_batcher_stats_get(const phmm_batcher* b, phmm_batcher_stats* out);
 
 /* Consumer of the matrix ("next" row N1): ConstantMixtureGenotypeLikelihoodModel::evaluate for G genotypes of one ploidy
  * (core/models/genotype/constant_mixture_genotype_likelihood_model.cpp:30-140) over a [H][R] matrix in `space`:

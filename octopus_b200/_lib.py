@@ -12,7 +12,9 @@ EXPORTS = ["phmm_version", "phmm_default_config", "phmm_create", "phmm_destroy",
            "phmm_last_dp_kernel_ms", "phmm_last_dp_cells", "phmm_align_scores", "phmm_align_traceback", "phmm_align_reads", "phmm_align_pairs", "phmm_genotype_likelihoods", "phmm_populate", "phmm_populate_templates", "phmm_populate_regions",
            "phmm_error_model_create", "phmm_error_model_create_custom", "phmm_error_model_destroy", "phmm_error_model_last_error",
            "phmm_reset_haplotypes", "phmm_tandem_repeats", "phmm_wait_event", "phmm_engine_stream", "phmm_reserve_sms", "phmm_host_alloc", "phmm_host_free",
-           "phmm_populate_ld", "phmm_device_alloc", "phmm_device_free", "phmm_ipc_export", "phmm_ipc_open", "phmm_ipc_close"]
+           "phmm_populate_ld", "phmm_device_alloc", "phmm_device_free", "phmm_ipc_export", "phmm_ipc_open", "phmm_ipc_close",
+           "phmm_batcher_create", "phmm_batcher_destroy", "phmm_batcher_last_error", "phmm_batcher_populate",
+           "phmm_batcher_populate_templates", "phmm_batcher_stats_get"]
 
 
 class Config(C.Structure):
@@ -43,6 +45,15 @@ class FlankState(C.Structure):
 
 class Regions(C.Structure):
     _fields_ = [("n", C.c_int32), ("hap_first", C.c_void_p), ("read_first", C.c_void_p), ("flank", C.c_void_p)]
+
+
+class BatcherOptions(C.Structure):
+    _fields_ = [("clients", C.c_int32), ("max_wait_us", C.c_int32)]
+
+
+class BatcherStats(C.Structure):
+    _fields_ = [("requests", C.c_int64), ("gpu_calls", C.c_int64), ("merged_calls", C.c_int64), ("max_regions_per_call", C.c_int64),
+                ("dp_cells", C.c_int64)]
 
 
 _lib = None
@@ -97,6 +108,19 @@ def load():
     lib.phmm_populate_templates.restype = C.c_int
     lib.phmm_populate_templates.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p, C.c_int32,
                                             C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_int]
+    lib.phmm_batcher_create.restype = C.c_int
+    lib.phmm_batcher_create.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(BatcherOptions)]
+    lib.phmm_batcher_destroy.argtypes = [C.c_void_p]
+    lib.phmm_batcher_last_error.restype = C.c_char_p
+    lib.phmm_batcher_last_error.argtypes = []
+    lib.phmm_batcher_populate.restype = C.c_int
+    lib.phmm_batcher_populate.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads),
+                                          C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_void_p]
+    lib.phmm_batcher_populate_templates.restype = C.c_int
+    lib.phmm_batcher_populate_templates.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p,
+                                                    C.c_int32, C.POINTER(FlankState), C.c_void_p, C.c_void_p]
+    lib.phmm_batcher_stats_get.restype = C.c_int
+    lib.phmm_batcher_stats_get.argtypes = [C.c_void_p, C.POINTER(BatcherStats)]
     lib.phmm_populate_ld.restype = C.c_int
     lib.phmm_populate_ld.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads),
                                      C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_int64, C.c_void_p]

@@ -346,6 +346,96 @@ class PairHMMEngine:
         return (out, status) if want_status else out
 
 
+class PopulateBatcher:
+    """One engine shared by many host threads (phmm_batcher_*): the populate requests that concurrent threads have in flight run
+    as one multi-region kernel chain. Calls are thread-safe and block; ctypes releases the GIL during them, so Python threads
+    really do wait together. Each result equals what ``PairHMMEngine.populate`` returns for the request alone. Host blocks only."""
+
+    def __init__(self, device=-1, clients=0, max_wait_us=None):
+        self._lib = _lib.load()
+        h = C.c_void_p()
+        opt = None
+        if clients or max_wait_us is not None:
+            opt = _lib.BatcherOptions(int(clients), 500 if max_wait_us is None else int(max_wait_us))
+        rc = self._lib.phmm_batcher_create(C.byref(h), int(device), C.byref(opt) if opt is not None else None)
+        if rc != _lib.PHMM_OK:
+            raise PhmmError(rc, self._lib.phmm_batcher_last_error().decode())
+        self._h = h
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.phmm_batcher_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def _raise(self, rc):
+        msg = self._lib.phmm_batcher_last_error().decode()      # this thread's last failing request
+        if rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE:
+            raise ShortHaplotypeError(rc, msg)
+        if rc == _lib.PHMM_ERR_BAND:
+            raise TooLargeBandSizeError(rc, msg)
+        raise PhmmError(rc, msg)
+
+    def stats(self):
+        """Counters since creation: requests, gpu_calls, merged_calls, max_regions_per_call, dp_cells."""
+        s = _lib.BatcherStats()
+        rc = self._lib.phmm_batcher_stats_get(self._h, C.byref(s))
+        if rc != _lib.PHMM_OK:
+            raise PhmmError(rc, "stats")
+        return {f: int(getattr(s, f)) for f, _ in _lib.BatcherStats._fields_}
+
+    def populate(self, config, haps: HaplotypeBlock, reads: ReadBlock, positions=None, flank_state=None, want_status=False):
+        """As PairHMMEngine.populate for host blocks: the (H, R) matrix (and the status matrix with want_status)."""
+        assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
+        H, R = haps.n, reads.n
+        hs, rs = haps.c_struct(), reads.c_struct()
+        cfg = config.c_struct() if hasattr(config, "c_struct") else config
+        pstruct, keep = None, []
+        if positions is not None:
+            off = np.ascontiguousarray(positions[0], dtype=np.int64)
+            pos = np.ascontiguousarray(positions[1], dtype=np.int32)
+            pstruct = _lib.Positions(off.ctypes.data, pos.ctypes.data)
+            keep += [off, pos]
+        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
+        out = np.empty((H, R), dtype=np.float64)
+        status = np.empty((H, R), dtype=np.int32) if want_status else None
+        rc = self._lib.phmm_batcher_populate(self._h, C.byref(cfg), C.byref(hs), C.byref(rs),
+                                             C.byref(pstruct) if pstruct is not None else None,
+                                             C.byref(fstruct) if fstruct is not None else None,
+                                             out.ctypes.data, status.ctypes.data if want_status else None)
+        if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
+            self._raise(rc)
+        return (out, status) if want_status else out
+
+    def populate_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, flank_state=None, want_status=False):
+        """As PairHMMEngine.populate_templates: the (H, T) matrix (and the per-read (H, R) status matrix with want_status)."""
+        assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
+        toff = np.ascontiguousarray(template_off, dtype=np.int64)
+        T = len(toff) - 1
+        hs, rs = haps.c_struct(), reads.c_struct()
+        cfg = config.c_struct() if hasattr(config, "c_struct") else config
+        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
+        out = np.empty((haps.n, T), dtype=np.float64)
+        status = np.empty((haps.n, reads.n), dtype=np.int32) if want_status else None
+        rc = self._lib.phmm_batcher_populate_templates(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), toff.ctypes.data, T,
+                                                       C.byref(fstruct) if fstruct is not None else None, out.ctypes.data,
+                                                       status.ctypes.data if want_status else None)
+        if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
+            self._raise(rc)
+        return (out, status) if want_status else out
+
+
 class ErrorModel:
     """The reference's sequencing-error models behind HaplotypeLikelihoodModel::reset (haplotype_likelihood_model.cpp:60-78):
     make_error_model(label) / make_error_model(file) (core/models/error/error_model_factory.cpp:531-589). ``reset`` turns

@@ -72,6 +72,7 @@ public:
         if (rc != PHMM_OK) throw Error {rc, phmm_last_error(nullptr)};
         handle_.reset(e, [] (phmm_engine* p) { phmm_destroy(p); });
     }
+    explicit Engine(std::nullptr_t) noexcept {}   // no engine (an array that runs on a SharedEngine)
     phmm_engine* get() const noexcept { return handle_.get(); }
     void check(int rc) const
     {
@@ -80,6 +81,38 @@ public:
     }
 private:
     std::shared_ptr<phmm_engine> handle_;
+};
+
+// One engine for a whole process's threads (phmm_batcher): the populate calls that concurrent threads have in flight run as one
+// multi-region kernel chain, each with the result it would get on an Engine of its own. Copies share the batcher; every thread
+// may call it at once. clients: the number of threads that submit (Octopus's --threads); a batch is sent once that many wait,
+// or max_wait_us after its first request arrived.
+class SharedEngine
+{
+public:
+    explicit SharedEngine(int device = -1, int clients = 0, int max_wait_us = 500)
+    {
+        phmm_batcher* b = nullptr;
+        const phmm_batcher_options opt {clients, max_wait_us};
+        const int rc = phmm_batcher_create(&b, device, &opt);
+        if (rc != PHMM_OK) throw Error {rc, phmm_batcher_last_error()};
+        handle_.reset(b, [] (phmm_batcher* p) { phmm_batcher_destroy(p); });
+    }
+    explicit SharedEngine(std::nullptr_t) noexcept {}
+    phmm_batcher* get() const noexcept { return handle_.get(); }
+    void check(int rc) const
+    {
+        if (rc == PHMM_OK) return;
+        throw Error {rc, phmm_batcher_last_error()};   // the calling thread's own last error
+    }
+    phmm_batcher_stats stats() const
+    {
+        phmm_batcher_stats s {};
+        check(phmm_batcher_stats_get(handle_.get(), &s));
+        return s;
+    }
+private:
+    std::shared_ptr<phmm_batcher> handle_;
 };
 
 // Page-locked storage for the batch blocks: a std::allocator over phmm_host_alloc (cudaHostAlloc) that falls back to malloc where
@@ -376,6 +409,11 @@ public:
     {
         if (config.max_indel_error > 256) throw TooLargeBandSizeError {static_cast<unsigned>(config.max_indel_error)};
     }
+    // populate() goes through a process-wide SharedEngine: any number of threads, each with its own array, share one GPU engine
+    HaplotypeLikelihoodArray(phmm_config config, SharedEngine shared) : engine_ {nullptr}, shared_ {std::move(shared)}, config_ {config}
+    {
+        if (config.max_indel_error > 256) throw TooLargeBandSizeError {static_cast<unsigned>(config.max_indel_error)};
+    }
     static phmm_config default_config() noexcept { phmm_config c; phmm_default_config(&c); return c; }
 
     // populate(const ReadMap&, haplotypes, flank_state) — haplotype_likelihood_array.cpp:51-103.
@@ -452,7 +490,7 @@ public:
     {
         SampleName name;
         if (new_sample) name = *new_sample; else for (const auto& s : samples) name += s;
-        HaplotypeLikelihoodArray result {config_, engine_};
+        HaplotypeLikelihoodArray result = shared_.get() ? HaplotypeLikelihoodArray {config_, shared_} : HaplotypeLikelihoodArray {config_, engine_};
         std::vector<std::size_t> idx;
         std::size_t total = 0;
         for (const auto& s : samples) { idx.push_back(sample_index(s)); total += width(idx.back()); }
@@ -473,6 +511,7 @@ public:
 
 private:
     Engine engine_;
+    SharedEngine shared_ {nullptr};   // set: populate() goes through the batcher instead of engine_
     phmm_config config_;
     pinned_vector<double> likelihoods_;
     pinned_vector<std::int32_t> status_;
@@ -511,16 +550,24 @@ private:
         pinned_vector<std::int32_t>& status = status_;               // page-locked scratch kept across calls: allocating pinned memory costs milliseconds
         status.resize(num_haplotypes_ * reads.size());
         phmm_flank_state fs {flank_state ? 1 : 0, flank_state ? flank_state->lhs_flank : 0, flank_state ? flank_state->rhs_flank : 0};
-        const int rc = template_off
-            ? phmm_populate_templates(engine_.get(), &config_, &hv, &rv, template_off->data(), static_cast<std::int32_t>(template_off->size() - 1),
-                                      positions, &fs, likelihoods_.data(), status.data(), PHMM_SPACE_HOST)
-            : phmm_populate(engine_.get(), &config_, &hv, &rv, positions, &fs, likelihoods_.data(), status.data(), PHMM_SPACE_HOST);
+        const auto n_templates = template_off ? static_cast<std::int32_t>(template_off->size() - 1) : 0;
+        int rc;
+        if (shared_.get()) {
+            rc = template_off
+                ? phmm_batcher_populate_templates(shared_.get(), &config_, &hv, &rv, template_off->data(), n_templates, &fs, likelihoods_.data(), status.data())
+                : phmm_batcher_populate(shared_.get(), &config_, &hv, &rv, positions, &fs, likelihoods_.data(), status.data());
+        } else {
+            rc = template_off
+                ? phmm_populate_templates(engine_.get(), &config_, &hv, &rv, template_off->data(), n_templates, positions, &fs, likelihoods_.data(),
+                                          status.data(), PHMM_SPACE_HOST)
+                : phmm_populate(engine_.get(), &config_, &hv, &rv, positions, &fs, likelihoods_.data(), status.data(), PHMM_SPACE_HOST);
+        }
         if (rc == PHMM_ERR_SHORT_HAPLOTYPE) {
             for (std::size_t i = 0; i < status.size(); ++i) {
                 if ((status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) throw ShortHaplotypeError {i / reads.size(), static_cast<unsigned>(static_cast<std::uint32_t>(status[i]) >> 16)};
             }
         }
-        engine_.check(rc);
+        if (shared_.get()) shared_.check(rc); else engine_.check(rc);
     }
 };
 

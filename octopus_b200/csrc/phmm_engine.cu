@@ -2,6 +2,7 @@
 // hot path runs in the kernels of phmm_kernels.cuh; there is no CPU fallback — without a usable GPU every
 // computing entry point returns PHMM_ERR_CUDA.
 #include "../../include/phmm_b200.h"
+#include "phmm_checks.h"
 #include "phmm_kernels.cuh"
 
 #include <algorithm>
@@ -163,22 +164,14 @@ int fetch_offsets(phmm_engine* e, const int64_t* off, int n, int space, std::vec
 int stage_batch(phmm_engine* e, const phmm_haplotypes* haps, const phmm_reads* reads, int space, Staged& s, bool need_info_host = true,
                 bool defer_flag_check = false)
 {
-    if (!haps || !reads || haps->n <= 0 || reads->n <= 0 || !haps->off || !reads->off) {
-        e->err = "empty or null haplotype / read block";
-        return PHMM_ERR_INVALID;
-    }
-    if (!haps->seq || !haps->snv_mask_fwd || !haps->snv_prior_fwd || !haps->snv_mask_rev || !haps->snv_prior_rev ||
-        !haps->gap_open || !haps->gap_extend || !reads->bases || !reads->quals) {
-        e->err = "null per-base array";
-        return PHMM_ERR_INVALID;
-    }
     int rc;
+    if ((rc = phmm_checks::blocks(haps, reads, e->err)) != PHMM_OK) return rc;
     if ((rc = fetch_offsets(e, haps->off, haps->n, space, s.hap_off_host)) != PHMM_OK) return rc;
     OffsetSummary rs {};
     if (space == PHMM_SPACE_HOST) {
         const int64_t* off = reads->off;
-        long long lo = 1LL << 62, hi = 0;
-        for (int r = 0; r < reads->n; ++r) { const long long len = off[r + 1] - off[r]; lo = std::min(lo, len); hi = std::max(hi, len); }
+        long long lo, hi;
+        phmm_checks::read_length_range(reads, &lo, &hi);
         rs.first = off[0]; rs.last = off[reads->n]; rs.len_max = hi; rs.inv_len_min = kOffsetBig - lo;
     } else {
         // device-resident offsets: reduce them where they are instead of copying the array back
@@ -194,12 +187,7 @@ int stage_batch(phmm_engine* e, const phmm_haplotypes* haps, const phmm_reads* r
     s.read_bases = rs.last;
     s.read_len_min = kOffsetBig - rs.inv_len_min;
     s.read_len_max = rs.len_max;
-    if (s.hap_off_host[0] != 0 || rs.first != 0 || s.hap_bases <= 0 || s.read_bases <= 0) {
-        e->err = "offset arrays must start at 0 and be increasing";
-        return PHMM_ERR_INVALID;
-    }
-    if (s.read_len_min < 1) { e->err = "empty read (offsets must be strictly increasing)"; return PHMM_ERR_INVALID; }
-    if (s.read_len_max > (1LL << 30)) { e->err = "read too long"; return PHMM_ERR_INVALID; }
+    if ((rc = phmm_checks::offsets(s.hap_off_host[0], s.hap_bases, rs.first, s.read_bases, s.read_len_min, s.read_len_max, e->err)) != PHMM_OK) return rc;
     DevHaps& hp = s.hp;
     DevReads& rd = s.rd;
     hp.n = haps->n; rd.n = reads->n;
@@ -797,13 +785,11 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
     };
     e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
     if (cudaSetDevice(e->device) != cudaSuccess) { e->err = "cudaSetDevice failed"; return PHMM_ERR_CUDA; }
-    if (!cfg || !out) { e->err = "null config / output"; return PHMM_ERR_INVALID; }
-    if (cfg->max_indel_error > 256) { e->err = "max_indel_error > 256"; return PHMM_ERR_BAND; }
+    int rc = phmm_checks::config_and_output(cfg, out, reads, e->err);
+    if (rc != PHMM_OK) return rc;
     const int band = round_band(std::max(1, cfg->max_indel_error));
-    if (cfg->nuc_prior < 0 || cfg->nuc_prior > 127) { e->err = "nuc_prior outside [0,127]"; return PHMM_ERR_INVALID; }
-    if (!reads || !reads->mapq || !reads->reverse) { e->err = "reads->mapq / reads->reverse required"; return PHMM_ERR_INVALID; }
     Staged s;
-    int rc = stage_batch(e, haps, reads, space, s, false, true);
+    rc = stage_batch(e, haps, reads, space, s, false, true);
     if (rc != PHMM_OK) return rc;
     const int H_total = s.hp.n, R = s.rd.n;
     RegionSetup single;
@@ -900,8 +886,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
         long long max_hap = 0;
         for (int h = 0; h < H_total; ++h) max_hap = std::max(max_hap, s.hap_off_host[h + 1] - s.hap_off_host[h]);
         mapper_maxt = max_hap - 5 <= 512 ? 512 : 2048;       // vote-array capacity per thread (longer haplotypes: tiles of 2048 diagonals)
-        if (max_hap > 65535) { e->err = "haplotype longer than 65535 bp: the device k-mer mapper indexes k-mer positions with 16 bits (pass explicit positions)"; return PHMM_ERR_INVALID; }
-        if (s.hap_bases > 65535LL * 65535LL) { e->err = "haplotype block too large"; return PHMM_ERR_INVALID; }
+        if ((rc = phmm_checks::mapper_haplotypes(max_hap, s.hap_bases, e->err)) != PHMM_OK) return rc;
         CU(e->rhash.ensure((size_t)s.read_bases * sizeof(uint16_t)));
         CU(e->kbins.ensure((size_t)H_total * (kKmerBins + 1) * sizeof(int)));
         CU(e->kitems.ensure((size_t)s.hap_bases * sizeof(uint16_t)));
@@ -1360,6 +1345,21 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
     return PHMM_OK;
 }
 
+} // extern "C"
+
+long long phmm_checks::populate_chunk_pairs(long long all_pairs)
+{
+    static const long long kForcedChunkPairs = [] {
+        const char* v = std::getenv("PHMM_CHUNK_PAIRS");          // test hook: force the pipelined path on small batches
+        const long long n = v ? std::atoll(v) : 0;
+        return n > 0 ? n : 0LL;
+    }();
+    // chunk size: an eighth of the batch, between 2M pairs (below that the per-chunk launch chain shows) and 8M pairs
+    return kForcedChunkPairs ? kForcedChunkPairs : std::max<long long>(2LL << 20, std::min<long long>(8LL << 20, all_pairs / 8));
+}
+
+extern "C" {
+
 int phmm_populate_regions(phmm_engine* e, const phmm_config* cfg,
                           const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_regions* regions,
                           double* out, int32_t* status, int space)
@@ -1448,11 +1448,8 @@ int phmm_populate_templates(phmm_engine* e, const phmm_config* cfg,
                             double* out, int32_t* status, int space)
 {
     if (!e) return PHMM_ERR_INVALID;
-    if (!template_off || n_templates <= 0 || !reads) { e->err = "null / empty template offsets"; return PHMM_ERR_INVALID; }
-    if (space == PHMM_SPACE_HOST) {
-        if (template_off[0] != 0 || template_off[n_templates] != reads->n) { e->err = "template offsets must cover the reads exactly"; return PHMM_ERR_INVALID; }
-        for (int t = 0; t < n_templates; ++t) if (template_off[t + 1] < template_off[t]) { e->err = "template offsets must be non-decreasing"; return PHMM_ERR_INVALID; }
-    }
+    const int rc = phmm_checks::template_offsets(template_off, n_templates, reads, space == PHMM_SPACE_HOST, e->err);
+    if (rc != PHMM_OK) return rc;
     return populate_impl(e, cfg, haps, reads, positions, flank, out, status, space, 0, template_off, n_templates);
 }
 
@@ -1464,14 +1461,8 @@ int phmm_populate(phmm_engine* e, const phmm_config* cfg,
     if (!e) return PHMM_ERR_INVALID;
     // Pipelined path: host-resident batch, no caller-supplied position lists (a [H][R] CSR cannot be sliced by columns
     // without a pass over it), enough pairs to amortise the per-chunk overheads.
-    static const long long kForcedChunkPairs = [] {
-        const char* v = std::getenv("PHMM_CHUNK_PAIRS");          // test hook: force the pipelined path on small batches
-        const long long n = v ? std::atoll(v) : 0;
-        return n > 0 ? n : 0LL;
-    }();
-    // chunk size: an eighth of the batch, between 2M pairs (below that the per-chunk launch chain shows) and 8M pairs
     const long long all_pairs = (haps && reads) ? (long long)haps->n * reads->n : 0;
-    const long long kChunkPairs = kForcedChunkPairs ? kForcedChunkPairs : std::max<long long>(2LL << 20, std::min<long long>(8LL << 20, all_pairs / 8));
+    const long long kChunkPairs = phmm_checks::populate_chunk_pairs(all_pairs);
     const bool can_chunk = !e->is_sub && space == PHMM_SPACE_HOST && haps && reads && cfg && out && haps->n > 0 && reads->n > 1 &&
                            reads->off && reads->mapq && reads->reverse && !(positions && positions->off && positions->pos) &&
                            all_pairs >= 2 * kChunkPairs;
