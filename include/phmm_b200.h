@@ -185,6 +185,23 @@ int phmm_align_reads(phmm_engine* e, const phmm_config* cfg,
                      const phmm_positions* positions, const phmm_flank_state* flank,
                      int64_t* mapping_position, double* likelihood, char* cigar, int32_t cigar_stride, int32_t* status, int space);
 
+/* map_query_to_target(read, haplotype) UNCAPPED, K = 6, for explicit pairs: the vector overload ReadRealigner uses
+ * (utils/kmer_mapper.cpp:14-22 → kmer_mapper.hpp:120-159 with max_mapping_positions = SIZE_MAX), i.e. every mapping begin whose
+ * k-mer vote count equals the pair's maximum, ascending. Sequences shorter than 6 map to nothing; haplotypes longer than 65535 bp
+ * (and reads longer than 65540 bp) are refused with PHMM_ERR_INVALID. Unlike the mapper inside phmm_populate, no cap of 10 applies.
+ * off[n_pairs+1] (pair j owns pos[off[j], off[j+1])) is always written; pos only when pos != NULL and pos_cap >= off[n_pairs].
+ * pos == NULL: a size query. Pair indices out of range: PHMM_ERR_INVALID. */
+int phmm_map_pairs(phmm_engine* e, const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_pair* pairs, int64_t n_pairs,
+                   int64_t* off, int32_t* pos, int64_t pos_cap, int space);
+
+/* ReadRealigner::realign (core/tools/read_realigner.cpp:105-144): pair j = model.align(read, map_query_to_target(read, haplotype)),
+ * the mapper above on the device and the traceback of phmm_align_reads fed its positions, in one kernel chain (one synchronisation
+ * in mid-call brings the number of positions back). cfg->map_positions = 0: the original position only (= phmm_align_reads with
+ * positions == NULL). Outputs, statuses and return codes as phmm_align_reads; SHORT_HAP statuses carry each pair's required extension. */
+int phmm_realign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                       const phmm_pair* pairs, int64_t n_pairs, const phmm_flank_state* flank,
+                       int64_t* mapping_position, double* likelihood, char* cigar, int32_t cigar_stride, int32_t* status, int space);
+
 /* hmm::align itself, batched (pair_hmm.hpp:858-874 → try_naive_align :321-340, simd_align :784-823): pair j aligns target
  * `pairs[j].read` of the `targets` block against truth `pairs[j].hap` of the `truths` block at target offset target_offsets[j] — no
  * candidate enumeration, no in-range rule. This is the call DeNovoModel makes per (haplotype, haplotype) pair

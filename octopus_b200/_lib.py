@@ -9,7 +9,7 @@ PHMM_OK, PHMM_ERR_INVALID, PHMM_ERR_CUDA, PHMM_ERR_BAND, PHMM_ERR_SHORT_HAPLOTYP
 SPACE_HOST, SPACE_DEVICE = 0, 1
 
 EXPORTS = ["phmm_version", "phmm_default_config", "phmm_create", "phmm_destroy", "phmm_last_error", "phmm_launch_count",
-           "phmm_last_dp_kernel_ms", "phmm_last_dp_cells", "phmm_align_scores", "phmm_align_traceback", "phmm_align_reads", "phmm_align_pairs", "phmm_genotype_likelihoods", "phmm_populate", "phmm_populate_templates", "phmm_populate_regions",
+           "phmm_last_dp_kernel_ms", "phmm_last_dp_cells", "phmm_align_scores", "phmm_align_traceback", "phmm_align_reads", "phmm_align_pairs", "phmm_map_pairs", "phmm_realign_reads", "phmm_genotype_likelihoods", "phmm_populate", "phmm_populate_templates", "phmm_populate_regions",
            "phmm_error_model_create", "phmm_error_model_create_custom", "phmm_error_model_destroy", "phmm_error_model_last_error",
            "phmm_reset_haplotypes", "phmm_tandem_repeats", "phmm_wait_event", "phmm_engine_stream", "phmm_reserve_sms", "phmm_host_alloc", "phmm_host_free",
            "phmm_populate_ld", "phmm_device_alloc", "phmm_device_free", "phmm_ipc_export", "phmm_ipc_open", "phmm_ipc_close",
@@ -97,6 +97,12 @@ def load():
     lib.phmm_align_pairs.restype = C.c_int
     lib.phmm_align_pairs.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p, C.c_void_p, C.c_int64,
                                      C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int]
+    lib.phmm_map_pairs.restype = C.c_int
+    lib.phmm_map_pairs.argtypes = [C.c_void_p, C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                   C.c_int64, C.c_int]
+    lib.phmm_realign_reads.restype = C.c_int
+    lib.phmm_realign_reads.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p, C.c_int64,
+                                       C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int]
     lib.phmm_genotype_likelihoods.restype = C.c_int
     lib.phmm_genotype_likelihoods.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int]
     lib.phmm_populate.restype = C.c_int

@@ -202,6 +202,79 @@ class PairHMMEngine:
         cigars = [bytes(cg[j * cigar_stride:(j + 1) * cigar_stride]).split(b"\0", 1)[0].decode() for j in range(n)]
         return mp, lk, cigars, st
 
+    @staticmethod
+    def _pairs_arg(pairs, dev, device):
+        if dev:
+            import torch
+            t = pairs if _is_torch(pairs) else torch.as_tensor(np.ascontiguousarray(pairs, dtype=np.int32), device=device)
+            t = t.to(device=device, dtype=torch.int32).reshape(-1, 2).contiguous()
+            return t, t.shape[0], t.data_ptr()
+        a = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
+        return a, a.shape[0], a.ctypes.data
+
+    def map_pairs(self, haps: HaplotypeBlock, reads: ReadBlock, pairs):
+        """map_query_to_target(read, haplotype) uncapped, K = 6, for explicit (read, haplotype) pairs (phmm_map_pairs): every mapping
+        begin at the pair's largest k-mer vote count, ascending — what ReadRealigner maps with. Returns the CSR (off[n+1] int64,
+        pos int32) over the pair list: numpy for host blocks, torch CUDA tensors for device-resident ones."""
+        dev = haps.on_device
+        assert dev == reads.on_device, "haplotypes and reads must live in the same memory space"
+        device = haps.seq.device if dev else None
+        pr, n, pp = self._pairs_arg(pairs, dev, device)
+        hs, rs = haps.c_struct(), reads.c_struct()
+        space = _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST
+        cap = 4 * n + 16                # most pairs have one or a few maxima; a second call takes the exact size
+        while True:
+            if dev:
+                import torch
+                off = torch.empty(n + 1, dtype=torch.int64, device=device)
+                pos = torch.empty(cap, dtype=torch.int32, device=device)
+                op, posp = off.data_ptr(), pos.data_ptr()
+            else:
+                off = np.empty(n + 1, dtype=np.int64)
+                pos = np.empty(cap, dtype=np.int32)
+                op, posp = off.ctypes.data, pos.ctypes.data
+            rc = self._lib.phmm_map_pairs(self._h, C.byref(hs), C.byref(rs), pp, n, op, posp, cap, space)
+            if rc != _lib.PHMM_OK:
+                self._raise(rc)
+            total = int(off[-1])
+            if total <= cap:
+                return off, pos[:total]
+            cap = total
+
+    def realign_reads(self, config, haps: HaplotypeBlock, reads: ReadBlock, pairs, flank_state=None, cigar_stride=None):
+        """ReadRealigner::realign for explicit (read, haplotype) pairs (phmm_realign_reads): HaplotypeLikelihoodModel::align at the
+        positions of the uncapped k-mer mapper (map_pairs), mapped on the device (config.map_positions = False: the original position
+        only). pairs: (n, 2) int32 rows (read, hap). Returns (mapping_position[n], likelihood[n], cigars[list of str], status[n]) as
+        align_reads; for device-resident blocks the three arrays are torch CUDA tensors."""
+        dev = haps.on_device
+        assert dev == reads.on_device, "haplotypes and reads must live in the same memory space"
+        device = haps.seq.device if dev else None
+        pr, n, pp = self._pairs_arg(pairs, dev, device)
+        hs, rs, cfg = haps.c_struct(), reads.c_struct(), config.c_struct()
+        if cigar_stride is None:
+            lens = (reads.off[1:] - reads.off[:-1]).max()
+            cigar_stride = 4 * int(lens) + 64
+        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
+        if dev:
+            import torch
+            mp = torch.zeros(n, dtype=torch.int64, device=device)
+            lk = torch.zeros(n, dtype=torch.float64, device=device)
+            st = torch.zeros(n, dtype=torch.int32, device=device)
+            cg = torch.zeros(n * cigar_stride, dtype=torch.uint8, device=device)
+            ptrs = (mp.data_ptr(), lk.data_ptr(), cg.data_ptr(), st.data_ptr())
+        else:
+            mp, lk, st = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=np.float64), np.zeros(n, dtype=np.int32)
+            cg = np.zeros(n * cigar_stride, dtype=np.uint8)
+            ptrs = (mp.ctypes.data, lk.ctypes.data, cg.ctypes.data, st.ctypes.data)
+        rc = self._lib.phmm_realign_reads(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), pp, n,
+                                          C.byref(fstruct) if fstruct is not None else None, ptrs[0], ptrs[1], ptrs[2], cigar_stride, ptrs[3],
+                                          _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST)
+        if rc != _lib.PHMM_OK:
+            self._raise(rc)
+        text = bytes(cg.cpu().numpy() if dev else cg)
+        cigars = [text[j * cigar_stride:(j + 1) * cigar_stride].split(b"\0", 1)[0].decode() for j in range(n)]
+        return mp, lk, cigars, st
+
     def genotype_likelihoods(self, lnl, genotypes):
         """ConstantMixtureGenotypeLikelihoodModel::evaluate for every row of `genotypes` ((G, ploidy) haplotype indices) over the
         (H, R) matrix `lnl` (numpy on the host, or a torch CUDA tensor left where populate produced it). Returns G doubles."""

@@ -79,6 +79,49 @@ public:
         if (rc == PHMM_OK) return;
         throw Error {rc, phmm_last_error(handle_.get())};
     }
+
+    // map_query_to_target(read, haplotype) uncapped for every pair (phmm_map_pairs): pair j's mapping begins are
+    // positions[offsets[j], offsets[j + 1]), ascending. Host memory.
+    struct PairMapping { std::vector<std::int64_t> offsets; std::vector<std::int32_t> positions; };
+    PairMapping map_pairs(const phmm_haplotypes& haplotypes, const phmm_reads& reads, const std::vector<phmm_pair>& pairs) const
+    {
+        PairMapping m;
+        m.offsets.resize(pairs.size() + 1);
+        m.positions.resize(4 * pairs.size() + 16);   // most pairs have one or a few maxima; a second call takes the exact size
+        for (;;) {
+            check(phmm_map_pairs(get(), &haplotypes, &reads, pairs.data(), static_cast<std::int64_t>(pairs.size()), m.offsets.data(),
+                                 m.positions.data(), static_cast<std::int64_t>(m.positions.size()), PHMM_SPACE_HOST));
+            const auto total = static_cast<std::size_t>(m.offsets.back());
+            if (total <= m.positions.size()) { m.positions.resize(total); return m; }
+            m.positions.resize(total);
+        }
+    }
+
+    // ReadRealigner::realign's per-read step for every pair (phmm_realign_reads). Statuses as phmm_align_reads (PHMM_STATUS_*;
+    // SHORT_HAP carries the required extension in the high 16 bits); host memory.
+    struct PairAlignments
+    {
+        std::vector<std::int64_t> mapping_position;
+        std::vector<double> likelihood;
+        std::vector<std::string> cigar;
+        std::vector<std::int32_t> status;
+    };
+    PairAlignments realign_reads(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
+                                 const std::vector<phmm_pair>& pairs, const phmm_flank_state* flank_state = nullptr) const
+    {
+        const std::size_t n = pairs.size();
+        std::int64_t longest = 1;
+        for (std::int32_t r = 0; r < reads.n; ++r) longest = std::max<std::int64_t>(longest, reads.off[r + 1] - reads.off[r]);
+        const auto stride = static_cast<std::int32_t>(4 * longest + 64);
+        PairAlignments a;
+        a.mapping_position.resize(n); a.likelihood.resize(n); a.status.resize(n);
+        std::vector<char> text(std::max<std::size_t>(n, 1) * static_cast<std::size_t>(stride), 0);
+        check(phmm_realign_reads(get(), &config, &haplotypes, &reads, pairs.data(), static_cast<std::int64_t>(n), flank_state,
+                                 a.mapping_position.data(), a.likelihood.data(), text.data(), stride, a.status.data(), PHMM_SPACE_HOST));
+        a.cigar.reserve(n);
+        for (std::size_t j = 0; j < n; ++j) a.cigar.emplace_back(text.data() + j * static_cast<std::size_t>(stride));
+        return a;
+    }
 private:
     std::shared_ptr<phmm_engine> handle_;
 };
@@ -378,6 +421,36 @@ struct TemplateBlock   // AlignedTemplate containers: template t owns the reads 
 };
 
 struct FlankState { std::int64_t lhs_flank, rhs_flank; };   // HaplotypeLikelihoodModel::FlankState
+
+// One read's result of ReadRealigner::realign (read_realigner.cpp:92-103, 128-130): HaplotypeLikelihoodModel::Alignment.
+struct Realignment
+{
+    std::int64_t mapping_position;
+    std::string cigar;
+    double likelihood;
+};
+
+// realign(reads, haplotype, model) (read_realigner.cpp:105-144) for haplotype `haplotype` of the block: every read mapped with the
+// uncapped k-mer mapper and aligned there, on the GPU. When a read's haplotype is too short, throws ShortHaplotypeError for the first
+// such read in read order — the reference's serial loop, whose required extension safe_realign (:196-207) applies.
+inline std::vector<Realignment> realign(const ReadBlock& reads, const HaplotypeBlock& haplotypes, std::size_t haplotype,
+                                        const phmm_config& config, const Engine& engine = Engine {}, const FlankState* flank_state = nullptr)
+{
+    std::vector<phmm_pair> pairs(reads.size());
+    for (std::size_t r = 0; r < reads.size(); ++r) pairs[r] = phmm_pair {static_cast<std::int32_t>(r), static_cast<std::int32_t>(haplotype)};
+    const phmm_flank_state fs {flank_state ? 1 : 0, flank_state ? flank_state->lhs_flank : 0, flank_state ? flank_state->rhs_flank : 0};
+    const auto a = engine.realign_reads(config, haplotypes.view(), reads.view(), pairs, &fs);
+    std::vector<Realignment> result;
+    result.reserve(pairs.size());
+    for (std::size_t r = 0; r < pairs.size(); ++r) {
+        const int code = a.status[r] & 0xFFFF;
+        if (code == PHMM_STATUS_SHORT_HAP) throw ShortHaplotypeError {haplotype, static_cast<unsigned>(static_cast<std::uint32_t>(a.status[r]) >> 16)};
+        if (code == PHMM_STATUS_HMM_OVERFLOW) throw Error {PHMM_ERR_INVALID, "HMMOverflow"};
+        if (code == PHMM_STATUS_CIGAR_TRUNCATED) throw Error {PHMM_ERR_INVALID, "CIGAR truncated"};
+        result.push_back(Realignment {a.mapping_position[r], a.cigar[r], a.likelihood[r]});
+    }
+    return result;
+}
 
 using SampleName = std::string;
 

@@ -66,6 +66,7 @@ struct phmm_engine {
     DBuf tab_f, tab_r, rowhalf, info, flags, best, status, out, slow, counters, pairs, generic_reads, wide_reads, bp, regs, rregion, rpbase, rpstride;
     DBuf tasks_lane, tasks_generic, works, scores, mapq_tab;
     DBuf rhash, kbins, kitems, kpos, kcnt, ftasks, fcnt, gtasks, atasks, gcnt, sched, sorted, fb_scratch, fb_pairs, npre_f, npre_r;
+    DBuf pm_best, pm_cnt, pm_inl, pm_part, pm_misc;   // the pair mapper's first pass (k_kmer_map_pairs) and its offset scan
     std::vector<cudaEvent_t> tile_events;
     std::vector<int2> info_host;
     // per-kernel launch configuration already applied / queried (the runtime calls are not free and need not be repeated)
@@ -330,7 +331,8 @@ void phmm_destroy(phmm_engine* e)
                    &e->r_off, &e->r_bases, &e->r_quals, &e->r_mapq, &e->r_rev, &e->r_begin, &e->c_off, &e->c_pos,
                    &e->tab_f, &e->tab_r, &e->rowhalf, &e->info, &e->flags, &e->best, &e->status, &e->out, &e->slow,
                    &e->counters, &e->pairs, &e->generic_reads, &e->wide_reads, &e->bp, &e->regs, &e->rregion, &e->rpbase, &e->rpstride, &e->tasks_lane, &e->tasks_generic, &e->works, &e->scores, &e->mapq_tab,
-                   &e->rhash, &e->kbins, &e->kitems, &e->kpos, &e->kcnt, &e->ftasks, &e->fcnt, &e->gtasks, &e->atasks, &e->gcnt, &e->sched, &e->sorted, &e->fb_scratch, &e->fb_pairs, &e->npre_f, &e->npre_r};
+                   &e->rhash, &e->kbins, &e->kitems, &e->kpos, &e->kcnt, &e->ftasks, &e->fcnt, &e->gtasks, &e->atasks, &e->gcnt, &e->sched, &e->sorted, &e->fb_scratch, &e->fb_pairs, &e->npre_f, &e->npre_r,
+                   &e->pm_best, &e->pm_cnt, &e->pm_inl, &e->pm_part, &e->pm_misc};
     for (DBuf* b : all) b->release();
     for (cudaEvent_t ev : e->tile_events) cudaEventDestroy(ev);
     if (e->ev0) cudaEventDestroy(e->ev0);
@@ -613,14 +615,91 @@ int phmm_genotype_likelihoods(phmm_engine* e, const double* lnl, int32_t H, int3
 }
 
 // -------------------------------------------------------------------------------------------------------------
+// Uncapped k-mer mapper over a pair list (phmm_map_pairs, phmm_realign_reads)
+// -------------------------------------------------------------------------------------------------------------
+// Pass 1 and the offset scan: k-mer hashes of the reads, tables of the haplotypes, per pair the maximum and how many mapping begins
+// reach it, CSR offsets into off_dev[n + 1] (device). One synchronisation brings the total back; a pair index out of range found on
+// the device fails the call here. *variant remembers the kernel instance for pair_map_emit.
+static int pair_map_count(phmm_engine* e, const Staged& s, const int2* d_pairs, int n, long long* off_dev, long long* total, int* variant)
+{
+    int rc;
+    long long max_hap = 0;
+    for (int h = 0; h < s.hp.n; ++h) max_hap = std::max(max_hap, s.hap_off_host[h + 1] - s.hap_off_host[h]);
+    if ((rc = phmm_checks::mapper_haplotypes(max_hap, s.hap_bases, e->err)) != PHMM_OK) return rc;
+    if (s.read_len_max - kKmer + 1 > 65535) { e->err = "read longer than 65540 bp: the device k-mer mapper counts votes in 16 bits"; return PHMM_ERR_INVALID; }
+    // vote-array capacity by the longest haplotype (longer ones: tiles of 2048 diagonals), byte counters when no read can cast > 255 votes
+    *variant = (max_hap - kKmer + 1 <= 512 ? 0 : 2) + (s.read_len_max - kKmer + 1 <= 255 ? 0 : 1);
+    const int R = s.rd.n, H = s.hp.n;
+    CU(e->rhash.ensure((size_t)s.read_bases * sizeof(uint16_t)));
+    CU(e->kbins.ensure((size_t)H * (kKmerBins + 1) * sizeof(int)));
+    CU(e->kitems.ensure((size_t)s.hap_bases * sizeof(uint16_t)));
+    k_read_kmers<<<(unsigned)(((long long)R * 32 + 255) / 256), 256, 0, e->stream>>>(s.read_bases, R, s.rd.off, s.rd.bases, e->rhash.as<uint16_t>());
+    LAUNCHED();
+    k_build_kmer_table<<<H, 256, 0, e->stream>>>(H, s.hp.off, s.hp.seq, e->kbins.as<uint32_t>(), e->kitems.as<uint16_t>());
+    LAUNCHED();
+    CU(e->pm_best.ensure((size_t)n * sizeof(unsigned)));
+    CU(e->pm_cnt.ensure((size_t)n * sizeof(int)));
+    CU(e->pm_inl.ensure((size_t)n * kPairMapInline * sizeof(int32_t)));
+    const int nb = (n + 1023) / 1024;
+    CU(e->pm_part.ensure((size_t)nb * sizeof(long long)));
+    CU(e->pm_misc.ensure(2 * sizeof(long long)));
+    long long* misc = e->pm_misc.as<long long>();             // [0] total, [1] low word: bad pair index
+    CU(cudaMemsetAsync(misc, 0, 2 * sizeof(long long), e->stream));
+    const unsigned grid = (unsigned)((n + 127) / 128);
+#define PHMM_PAIRMAP_ARGS n, d_pairs, s.hp, s.rd, e->rhash.as<uint16_t>(), e->kbins.as<uint32_t>(), e->kitems.as<uint16_t>(), e->pm_best.as<unsigned>(), \
+                          e->pm_cnt.as<int>(), e->pm_inl.as<int32_t>(), (int*)(misc + 1), nullptr, nullptr
+    switch (*variant) {
+        case 0: k_kmer_map_pairs<512, uint8_t, false><<<grid, 128, 0, e->stream>>>(PHMM_PAIRMAP_ARGS); break;
+        case 1: k_kmer_map_pairs<512, uint16_t, false><<<grid, 128, 0, e->stream>>>(PHMM_PAIRMAP_ARGS); break;
+        case 2: k_kmer_map_pairs<2048, uint8_t, false><<<grid, 128, 0, e->stream>>>(PHMM_PAIRMAP_ARGS); break;
+        default: k_kmer_map_pairs<2048, uint16_t, false><<<grid, 128, 0, e->stream>>>(PHMM_PAIRMAP_ARGS); break;
+    }
+#undef PHMM_PAIRMAP_ARGS
+    LAUNCHED();
+    k_csr_scan_blocks<<<nb, 1024, 0, e->stream>>>(n, e->pm_cnt.as<int>(), off_dev, e->pm_part.as<long long>());
+    LAUNCHED();
+    k_csr_scan_parts<<<1, 1024, 0, e->stream>>>(nb, e->pm_part.as<long long>(), misc);
+    LAUNCHED();
+    k_csr_scan_carry<<<nb, 1024, 0, e->stream>>>(n, e->pm_part.as<long long>(), off_dev);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    long long host_misc[2] = {0, 0};
+    CU(cudaMemcpyAsync(host_misc, misc, sizeof(host_misc), cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    if ((int)host_misc[1] != 0) { e->err = "pair index out of range"; return PHMM_ERR_INVALID; }
+    *total = host_misc[0];
+    return PHMM_OK;
+}
+
+// Pass 2: every mapping begin of every pair into pos_dev[off_dev[j] ..) (device, off_dev[n] entries).
+static int pair_map_emit(phmm_engine* e, const Staged& s, const int2* d_pairs, int n, const long long* off_dev, int32_t* pos_dev, int variant)
+{
+    const unsigned grid = (unsigned)((n + 127) / 128);
+#define PHMM_PAIRMAP_ARGS n, d_pairs, s.hp, s.rd, e->rhash.as<uint16_t>(), e->kbins.as<uint32_t>(), e->kitems.as<uint16_t>(), e->pm_best.as<unsigned>(), \
+                          e->pm_cnt.as<int>(), e->pm_inl.as<int32_t>(), nullptr, off_dev, pos_dev
+    switch (variant) {
+        case 0: k_kmer_map_pairs<512, uint8_t, true><<<grid, 128, 0, e->stream>>>(PHMM_PAIRMAP_ARGS); break;
+        case 1: k_kmer_map_pairs<512, uint16_t, true><<<grid, 128, 0, e->stream>>>(PHMM_PAIRMAP_ARGS); break;
+        case 2: k_kmer_map_pairs<2048, uint8_t, true><<<grid, 128, 0, e->stream>>>(PHMM_PAIRMAP_ARGS); break;
+        default: k_kmer_map_pairs<2048, uint16_t, true><<<grid, 128, 0, e->stream>>>(PHMM_PAIRMAP_ARGS); break;
+    }
+#undef PHMM_PAIRMAP_ARGS
+    LAUNCHED();
+    CU(cudaGetLastError());
+    return PHMM_OK;
+}
+
+// -------------------------------------------------------------------------------------------------------------
 // phmm_align_reads
 // -------------------------------------------------------------------------------------------------------------
-// Shared by phmm_align_reads (HaplotypeLikelihoodModel::align: candidate positions, in-range rule, fallback) and phmm_align_pairs
-// (hmm::align: one explicit offset per pair).
+// Shared by phmm_align_reads (HaplotypeLikelihoodModel::align: candidate positions, in-range rule, fallback), phmm_realign_reads
+// (the same with every pair's positions from the uncapped pair mapper, map_on_device) and phmm_align_pairs (hmm::align: one explicit
+// offset per pair).
 static int align_impl(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
                       const phmm_pair* pairs, int64_t n_pairs, const phmm_positions* positions, const int32_t* raw_offsets,
                       const phmm_flank_state* flank,
-                      int64_t* mapping_position, double* likelihood, char* cigar, int32_t cigar_stride, int32_t* status, int space)
+                      int64_t* mapping_position, double* likelihood, char* cigar, int32_t cigar_stride, int32_t* status, int space,
+                      bool map_on_device = false)
 {
     if (!e) return PHMM_ERR_INVALID;
     e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
@@ -661,6 +740,14 @@ static int align_impl(phmm_engine* e, const phmm_config* cfg, const phmm_haploty
         if ((rc = stage(e, e->c_off, (const long long*)positions->off, (size_t)n + 1, space, &po))) return rc;
         if ((rc = stage(e, e->c_pos, positions->pos, (size_t)std::max<long long>(ends[0], 1), space, &pv))) return rc;
         p.pos_off = po; p.pos = pv;
+    } else if (map_on_device) {
+        long long total = 0;
+        int variant = 0;
+        CU(e->c_off.ensure(((size_t)n + 1) * sizeof(long long)));
+        if ((rc = pair_map_count(e, s, d_pairs, n, e->c_off.as<long long>(), &total, &variant))) return rc;
+        CU(e->c_pos.ensure((size_t)std::max<long long>(total, 1) * sizeof(int32_t)));
+        if ((rc = pair_map_emit(e, s, d_pairs, n, e->c_off.as<long long>(), e->c_pos.as<int32_t>(), variant))) return rc;
+        p.pos_off = e->c_off.as<long long>(); p.pos = e->c_pos.as<int32_t>();
     }
     int Lmax = 1;
     for (int r = 0; r < s.rd.n; ++r) Lmax = std::max(Lmax, e->info_host[r].x);
@@ -755,6 +842,53 @@ int phmm_align_pairs(phmm_engine* e, const phmm_config* cfg,
     if (!e) return PHMM_ERR_INVALID;
     if (!target_offsets) { e->err = "null target offsets"; return PHMM_ERR_INVALID; }
     return align_impl(e, cfg, truths, targets, pairs, n_pairs, nullptr, target_offsets, flank, target_offset_out, likelihood, cigar, cigar_stride, status, space);
+}
+
+int phmm_realign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                       const phmm_pair* pairs, int64_t n_pairs, const phmm_flank_state* flank,
+                       int64_t* mapping_position, double* likelihood, char* cigar, int32_t cigar_stride, int32_t* status, int space)
+{
+    const bool map = cfg && cfg->map_positions;
+    return align_impl(e, cfg, haps, reads, pairs, n_pairs, nullptr, nullptr, flank, mapping_position, likelihood, cigar, cigar_stride, status, space, map);
+}
+
+int phmm_map_pairs(phmm_engine* e, const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_pair* pairs, int64_t n_pairs,
+                   int64_t* off, int32_t* pos, int64_t pos_cap, int space)
+{
+    if (!e) return PHMM_ERR_INVALID;
+    e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
+    if (cudaSetDevice(e->device) != cudaSuccess) { e->err = "cudaSetDevice failed"; return PHMM_ERR_CUDA; }
+    if (!pairs || !off) { e->err = "null pairs / offsets"; return PHMM_ERR_INVALID; }
+    if (n_pairs < 0 || n_pairs > 0x7fffffff) { e->err = "pair count out of range"; return PHMM_ERR_INVALID; }
+    const bool dev = space == PHMM_SPACE_DEVICE;
+    if (n_pairs == 0) {
+        if (!dev) off[0] = 0;
+        else { CU(cudaMemsetAsync(off, 0, sizeof(int64_t), e->stream)); CU(cudaStreamSynchronize(e->stream)); }
+        return PHMM_OK;
+    }
+    Staged s;
+    int rc = stage_batch(e, haps, reads, space, s, false);
+    if (rc != PHMM_OK) return rc;
+    const int n = (int)n_pairs;
+    if (!dev) {
+        for (int i = 0; i < n; ++i) if (pairs[i].read < 0 || pairs[i].read >= s.rd.n || pairs[i].hap < 0 || pairs[i].hap >= s.hp.n) { e->err = "pair index out of range"; return PHMM_ERR_INVALID; }
+    }
+    const int2* d_pairs;
+    if ((rc = stage(e, e->pairs, (const int2*)pairs, (size_t)n, space, &d_pairs))) return rc;
+    long long* off_dev = (long long*)off;
+    if (!dev) { CU(e->c_off.ensure(((size_t)n + 1) * sizeof(long long))); off_dev = e->c_off.as<long long>(); }
+    long long total = 0;
+    int variant = 0;
+    if ((rc = pair_map_count(e, s, d_pairs, n, off_dev, &total, &variant))) return rc;
+    if (pos && pos_cap >= total && total > 0) {
+        int32_t* pos_dev = pos;
+        if (!dev) { CU(e->c_pos.ensure((size_t)total * sizeof(int32_t))); pos_dev = e->c_pos.as<int32_t>(); }
+        if ((rc = pair_map_emit(e, s, d_pairs, n, off_dev, pos_dev, variant))) return rc;
+        if (!dev) CU(cudaMemcpyAsync(pos, pos_dev, (size_t)total * sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
+    }
+    if (!dev) CU(cudaMemcpyAsync(off, off_dev, ((size_t)n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    return PHMM_OK;
 }
 
 // -------------------------------------------------------------------------------------------------------------

@@ -659,6 +659,36 @@ __global__ void k_build_kmer_table(const int H, const long long* __restrict__ of
     }
 }
 
+// One tile of map_query_to_target's vote (:131-146) for one (query, target) pair: counts[t] = votes for the mapping begin d0 + t,
+// t < dn (cleared first), i.e. the query k-mers qi whose k-mer also starts at target position qi + d0 + t. Returns the tile's largest
+// count. rh: the query's k-mer hashes; bs / it: the target's bins (column of the hash-major table, stride H) and items.
+template <typename CountT>
+__device__ __forceinline__ unsigned kmer_vote_tile(uint32_t* words, const int d0, const int dn, const int nq, const uint16_t* __restrict__ rh,
+                                                   const uint32_t* __restrict__ bs, const int H, const uint16_t* __restrict__ it)
+{
+    constexpr int PER = 4 / (int)sizeof(CountT);
+    CountT* counts = reinterpret_cast<CountT*>(words);
+    const int nwords = (dn + PER - 1) / PER;
+    for (int w = 0; w < nwords; ++w) words[w] = 0u;
+    unsigned max_hit = 0;
+    for (int qi = 0; qi < nq; ++qi) {
+        const uint32_t bin = bs[(size_t)rh[qi] * H];
+        const int n = (int)(bin >> 16);
+        if (n == 0) continue;
+        if (n == 1) {                                        // the k-mer's position, inline
+            const int d = (int)(bin & 0xFFFFu) - qi - d0;
+            if (d >= 0 && d < dn) { const unsigned c = ++counts[d]; max_hit = c > max_hit ? c : max_hit; }
+            continue;
+        }
+        const int e0 = (int)(bin & 0xFFFFu);
+        for (int e = e0; e < e0 + n; ++e) {
+            const int d = (int)it[e] - qi - d0;               // the reference keeps target_index >= query_index
+            if (d >= 0 && d < dn) { const unsigned c = ++counts[d]; max_hit = c > max_hit ? c : max_hit; }
+        }
+    }
+    return max_hit;
+}
+
 // map_query_to_target (:120-159) for every (read of the work list, haplotype): the first <= 10 mapping begins (ascending)
 // whose vote count equals the maximum. votes[d] = number of query k-mers qi whose k-mer also starts at target position qi + d.
 // One THREAD per pair, consecutive lanes = consecutive haplotypes of one read: the read's k-mer hash is a broadcast load, the
@@ -695,30 +725,11 @@ __global__ void k_kmer_map(const int* __restrict__ list, const int n_list_max, c
             const int nq = (int)(rd.off[r + 1] - ro) - kKmer + 1, nt = (int)(hp.off[h + 1] - ho) - kKmer + 1;
             if (nq > 0 && nt > 0) {
                 uint32_t words[MAXT / PER];
-                CountT* counts = reinterpret_cast<CountT*>(words);
-                const uint32_t* bs = binsT + h;
-                const uint16_t* it = items + ho;
                 int32_t* out = kpos + (size_t)i * kMaxMapped;
                 unsigned best = 0;
                 for (int d0 = 0; d0 < nt; d0 += MAXT) {
                     const int dn = min(MAXT, nt - d0), nwords = (dn + PER - 1) / PER;
-                    for (int w = 0; w < nwords; ++w) words[w] = 0u;
-                    unsigned max_hit = 0;
-                    for (int qi = 0; qi < nq; ++qi) {
-                        const uint32_t bin = bs[(size_t)rhash[ro + qi] * H];
-                        const int n = (int)(bin >> 16);
-                        if (n == 0) continue;
-                        if (n == 1) {                                        // the k-mer's position, inline
-                            const int d = (int)(bin & 0xFFFFu) - qi - d0;
-                            if (d >= 0 && d < dn) { const unsigned c = ++counts[d]; max_hit = c > max_hit ? c : max_hit; }
-                            continue;
-                        }
-                        const int e0 = (int)(bin & 0xFFFFu);
-                        for (int e = e0; e < e0 + n; ++e) {
-                            const int d = (int)it[e] - qi - d0;               // the reference keeps target_index >= query_index
-                            if (d >= 0 && d < dn) { const unsigned c = ++counts[d]; max_hit = c > max_hit ? c : max_hit; }
-                        }
-                    }
+                    const unsigned max_hit = kmer_vote_tile<CountT>(words, d0, dn, nq, rhash + ro, binsT + h, H, items + ho);
                     if (max_hit > best) { best = max_hit; n_out = 0; }       // a higher count: what earlier tiles listed is void
                     if (max_hit == best && best > 0) {
                         for (int w = 0; w < nwords && n_out < kMaxMapped; ++w) {
@@ -738,6 +749,125 @@ __global__ void k_kmer_map(const int* __restrict__ list, const int n_list_max, c
         }
         kcnt[i] = n_out;
     }
+}
+
+constexpr int kPairMapInline = 4;   // mapping begins k_kmer_map_pairs keeps per pair in its first pass
+
+// map_query_to_target(read, haplotype) UNCAPPED, for an explicit pair list: the vector overload (kmer_mapper.cpp:14-22) leaves
+// max_mapping_positions at SIZE_MAX (:120-123), so every mapping begin whose vote count equals the maximum is listed, ascending.
+// This is what ReadRealigner::realign maps with (read_realigner.cpp:128, 137). One thread per pair; the vote is k_kmer_map's
+// (kmer_vote_tile, tiles of MAXT diagonals, CountT by read length).
+//   EMIT = false (first pass): best[j] = the pair's maximum (0: no vote), cnt[j] = the number of mapping begins at it, inl[j][0..4) =
+//     the first min(cnt, 4) of them. A pair index out of range sets bad[0] and maps to nothing.
+//   EMIT = true (after cnt was scanned into the CSR offsets off): pos[off[j] ..) = all of them — copied from inl where they fit, else
+//     voted again and listed at best[j]: a tile's own maximum can be below the pair's, so only the final maximum decides.
+template <int MAXT, typename CountT, bool EMIT>
+__global__ void k_kmer_map_pairs(const int n_pairs, const int2* __restrict__ pairs, const DevHaps hp, const DevReads rd,
+                                 const uint16_t* __restrict__ rhash, const uint32_t* __restrict__ binsT, const uint16_t* __restrict__ items,
+                                 unsigned* __restrict__ best_of, int* __restrict__ cnt, int32_t* __restrict__ inl, int* __restrict__ bad,
+                                 const long long* __restrict__ off, int32_t* __restrict__ pos)
+{
+    constexpr int PER = 4 / (int)sizeof(CountT);
+    const int j = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+    if (j >= n_pairs) return;
+    int32_t* out = nullptr;
+    unsigned best = 0;
+    if (EMIT) {
+        const int c = cnt[j];
+        if (c == 0) return;
+        out = pos + off[j];
+        if (c <= kPairMapInline) {
+            for (int k = 0; k < c; ++k) out[k] = inl[(size_t)j * kPairMapInline + k];
+            return;
+        }
+        best = best_of[j];
+    }
+    const int r = pairs[j].x, h = pairs[j].y;
+    if (!EMIT && (r < 0 || r >= rd.n || h < 0 || h >= hp.n)) { atomicOr(bad, 1); best_of[j] = 0; cnt[j] = 0; return; }
+    const long long ro = rd.off[r], ho = hp.off[h];
+    const int nq = (int)(rd.off[r + 1] - ro) - kKmer + 1, nt = (int)(hp.off[h + 1] - ho) - kKmer + 1;
+    int n = 0;
+    if (nq > 0 && nt > 0) {
+        uint32_t words[MAXT / PER];
+        for (int d0 = 0; d0 < nt; d0 += MAXT) {
+            const int dn = min(MAXT, nt - d0), nwords = (dn + PER - 1) / PER;
+            const unsigned max_hit = kmer_vote_tile<CountT>(words, d0, dn, nq, rhash + ro, binsT + h, hp.n, items + ho);
+            if (!EMIT && max_hit > best) { best = max_hit; n = 0; }       // a higher count: what earlier tiles listed is void
+            if (max_hit != best || best == 0) continue;
+            for (int w = 0; w < nwords; ++w) {
+                uint32_t v = words[w];
+                if (v == 0u) continue;
+#pragma unroll
+                for (int b = 0; b < PER; ++b) {
+                    const unsigned c = v & ((1u << (8 * sizeof(CountT))) - 1u);
+                    v >>= 4 * sizeof(CountT); v >>= 4 * sizeof(CountT);
+                    const int t = w * PER + b;
+                    if (c == best && t < dn) {
+                        if (EMIT) out[n] = d0 + t;
+                        else if (n < kPairMapInline) inl[(size_t)j * kPairMapInline + n] = d0 + t;
+                        ++n;
+                    }
+                }
+            }
+        }
+    }
+    if (!EMIT) { best_of[j] = best; cnt[j] = n; }
+}
+
+// CSR offsets from per-item counts, off[0] = 0 and off[i + 1] = cnt[0] + ... + cnt[i], in three launches of 1024-thread blocks:
+// block-local inclusive scans (k_csr_scan_blocks, block totals to part[]), one block's exclusive scan of the block totals with
+// the grand total to *total (k_csr_scan_parts), and the carry (k_csr_scan_carry).
+__device__ __forceinline__ long long block_inclusive_scan(long long v, long long* warp_sums)
+{
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const long long u = __shfl_up_sync(0xffffffffu, v, d); if (lane >= d) v += u; }
+    if (lane == 31) warp_sums[w] = v;
+    __syncthreads();
+    if (w == 0) {
+        long long s = warp_sums[lane];
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const long long u = __shfl_up_sync(0xffffffffu, s, d); if (lane >= d) s += u; }
+        warp_sums[lane] = s;
+    }
+    __syncthreads();
+    if (w > 0) v += warp_sums[w - 1];
+    __syncthreads();                                     // warp_sums is free for the next call
+    return v;
+}
+
+__global__ void __launch_bounds__(1024) k_csr_scan_blocks(const int n, const int* __restrict__ cnt, long long* __restrict__ off, long long* __restrict__ part)
+{
+    __shared__ long long ws[32];
+    const long long i = (long long)blockIdx.x * 1024 + threadIdx.x;
+    const long long v = block_inclusive_scan(i < n ? (long long)cnt[i] : 0LL, ws);
+    if (i < n) off[i + 1] = v;
+    if (threadIdx.x == 1023) part[blockIdx.x] = v;
+}
+
+__global__ void __launch_bounds__(1024) k_csr_scan_parts(const int nb, long long* __restrict__ part, long long* __restrict__ total)
+{
+    __shared__ long long ws[32];
+    __shared__ long long chunk_total;
+    long long carry = 0;
+    for (int b0 = 0; b0 < nb; b0 += 1024) {
+        const int b = b0 + (int)threadIdx.x;
+        const long long x = b < nb ? part[b] : 0LL;
+        const long long v = block_inclusive_scan(x, ws);
+        if (b < nb) part[b] = carry + v - x;
+        if (threadIdx.x == 1023) chunk_total = v;
+        __syncthreads();
+        carry += chunk_total;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *total = carry;
+}
+
+__global__ void __launch_bounds__(1024) k_csr_scan_carry(const int n, const long long* __restrict__ part, long long* __restrict__ off)
+{
+    const long long i = (long long)blockIdx.x * 1024 + threadIdx.x;
+    if (i < n) off[i + 1] += part[blockIdx.x];
+    if (i == 0) off[0] = 0;
 }
 
 // Fast-path DP over the task lists the classify pass (k_populate_generic<.., true>) produced. Persistent warps: each warp
