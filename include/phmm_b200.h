@@ -244,6 +244,27 @@ int phmm_populate_regions(phmm_engine* e, const phmm_config* cfg,
                           const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_regions* regions,
                           double* out, int32_t* status, int space);
 
+/* compute_haplotype_support's scoring and choice (core/tools/read_assigner.cpp:231-285, 45-64) for many groups in one kernel chain.
+ * Group g is one genotype after the caller's collapse / reference augmentation (read_assigner.cpp:305-318,
+ * csr/facets/read_assignments.cpp:113-124): haplotypes [hap_first[g], hap_first[g+1]) in genotype order and its reads
+ * [read_first[g], read_first[g+1]). groups as phmm_populate_regions (host memory, flank honoured; NULL flank = none, as the
+ * assigner uses). Every group needs >= 1 haplotype and >= 1 read (leave out genotypes without local reads, read_assignments.cpp:109)
+ * and at most 64 haplotypes.
+ *   lnl (optional): the groups' [H_g][R_g] matrices back to back, as populate_regions. cfg->map_positions = 1: pair (h, r) is
+ *     HaplotypeLikelihoodModel::evaluate(read, map_query_to_target(read, haplotype)) with the UNCAPPED mapper of phmm_map_pairs (every
+ *     mapping begin at the maximum vote, not populate's first 10); a pair with more than 4096 of them fails with PHMM_ERR_INVALID, and
+ *     haplotypes over 65535 bp are refused as phmm_map_pairs refuses them. cfg->map_positions = 0: the original position only (=
+ *     phmm_populate_regions).
+ *   top[r] (required, [R]): bit k set <=> group-local haplotype k is in read r's find_map_haplotypes set: the haplotypes maximising
+ *     lnl + log_priors[h] under maths::almost_equal with the reference's loop order (a value almost equal to the running maximum joins
+ *     the set without raising it; an empty set becomes every haplotype).
+ *   log_priors: [H] per haplotype of the block, or NULL (= 0, get_priors :36-43).
+ * The ambiguity policy (drop / first / all / random) and the recording of ambiguous reads stay with the caller. Errors and statuses as
+ * phmm_populate_regions; on PHMM_ERR_SHORT_HAPLOTYPE the SHORT_HAP statuses carry each pair's extension and top is unspecified.
+ * Two synchronisations in mid-call: the number of mapped positions, and the longest position list. */
+int phmm_assign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                      const phmm_regions* groups, const double* log_priors, uint64_t* top, double* lnl, int32_t* status, int space);
+
 /* phmm_populate with device-resident inputs and an output row stride: out[h * out_ld + r], out_ld >= R (status, optional, stays dense
  * [H][R]). `out` is any device-accessible address — in particular a window of ANOTHER GPU's matrix mapped with phmm_ipc_open: the
  * epilogue kernel then stores this rank's columns of a read-sharded [H, R_total] matrix (or its slab of a per-rank stack) straight

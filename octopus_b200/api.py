@@ -352,6 +352,60 @@ class PairHMMEngine:
             self._raise(rc)
         return (out, off, status) if want_status else (out, off)
 
+    def assign_reads(self, config, haps: HaplotypeBlock, reads: ReadBlock, hap_first, read_first, log_priors=None, want_likelihoods=False,
+                     want_status=False):
+        """compute_haplotype_support's scoring and choice for many genotypes in one call (phmm_assign_reads). Group g (one genotype)
+        owns haplotypes [hap_first[g], hap_first[g+1]) in genotype order and reads [read_first[g], read_first[g+1]); at most 64
+        haplotypes per group. config.map_positions: every pair at the positions of the uncapped k-mer mapper (map_pairs), else at the
+        original position only. log_priors: None or [H] per haplotype of the block.
+        Returns top ([R] uint64: bit k = group-local haplotype k is in the read's find_map_haplotypes set), plus the flat likelihood
+        vector (the groups' [H_g, R_g] matrices back to back, as populate_regions) when want_likelihoods and the per-pair statuses when
+        want_status: numpy for host blocks, torch CUDA tensors for device-resident ones (top then as int64 with the same bits). With want_status a short haplotype does not
+        raise; its statuses carry the extension and top is unspecified."""
+        dev = haps.on_device
+        assert dev == reads.on_device, "haplotypes and reads must live in the same memory space"
+        hf = np.ascontiguousarray(hap_first, dtype=np.int32)
+        rf = np.ascontiguousarray(read_first, dtype=np.int32)
+        G = len(hf) - 1
+        total = int((np.diff(hf).astype(np.int64) * np.diff(rf).astype(np.int64)).sum())
+        regs = _lib.Regions(G, hf.ctypes.data, rf.ctypes.data, None)
+        hs, rs = haps.c_struct(), reads.c_struct()
+        cfg = config.c_struct() if hasattr(config, "c_struct") else config
+        lnl = status = pri = None
+        if dev:
+            import torch
+            device = haps.seq.device
+            top = torch.empty(reads.n, dtype=torch.int64, device=device)
+            if want_likelihoods:
+                lnl = torch.empty(total, dtype=torch.float64, device=device)
+            if want_status:
+                status = torch.empty(total, dtype=torch.int32, device=device)
+            if log_priors is not None:
+                pri = (log_priors if _is_torch(log_priors) else torch.as_tensor(np.asarray(log_priors, dtype=np.float64)))
+                pri = pri.to(device=device, dtype=torch.float64).contiguous()
+            ptr = lambda x: None if x is None else x.data_ptr()
+        else:
+            top = np.empty(reads.n, dtype=np.uint64)
+            if want_likelihoods:
+                lnl = np.empty(total, dtype=np.float64)
+            if want_status:
+                status = np.empty(total, dtype=np.int32)
+            if log_priors is not None:
+                pri = np.ascontiguousarray(log_priors, dtype=np.float64)
+            ptr = lambda x: None if x is None else x.ctypes.data
+        if pri is not None and pri.shape[0] != haps.n:
+            raise ValueError("log_priors needs one value per haplotype of the block")
+        rc = self._lib.phmm_assign_reads(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), C.byref(regs), ptr(pri), ptr(top), ptr(lnl),
+                                         ptr(status), _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST)
+        if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
+            self._raise(rc)
+        out = (top,)
+        if want_likelihoods:
+            out += (lnl,)
+        if want_status:
+            out += (status,)
+        return out[0] if len(out) == 1 else out
+
     @staticmethod
     def split_regions(flat, off, hap_first, read_first):
         """The per-region [H_g, R_g] views of a populate_regions result."""

@@ -122,6 +122,37 @@ public:
         for (std::size_t j = 0; j < n; ++j) a.cigar.emplace_back(text.data() + j * static_cast<std::size_t>(stride));
         return a;
     }
+
+    // compute_haplotype_support's scoring and choice for many genotypes (phmm_assign_reads); host memory. top[r] bit k = group-local
+    // haplotype k is in read r's find_map_haplotypes set. likelihood / status: the groups' [H_g][R_g] matrices back to back. A short
+    // haplotype does not throw here: the return code is PHMM_ERR_SHORT_HAPLOTYPE and the statuses carry the extension.
+    struct ReadAssignment
+    {
+        std::vector<std::uint64_t> top;
+        std::vector<double> likelihood;
+        std::vector<std::int32_t> status;
+        int code = PHMM_OK;
+    };
+    ReadAssignment assign_reads(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
+                                const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
+                                const std::vector<double>* log_priors = nullptr, bool want_likelihoods = false) const
+    {
+        if (hap_first.empty() || hap_first.size() != read_first.size()) throw Error {PHMM_ERR_INVALID, "group bounds need n + 1 entries each"};
+        const auto n = static_cast<std::int32_t>(hap_first.size() - 1);
+        if (log_priors && log_priors->size() != static_cast<std::size_t>(haplotypes.n)) throw Error {PHMM_ERR_INVALID, "one log prior per haplotype"};
+        std::size_t pairs = 0;
+        for (std::int32_t g = 0; g < n; ++g)
+            pairs += static_cast<std::size_t>(std::max(0, hap_first[g + 1] - hap_first[g])) * static_cast<std::size_t>(std::max(0, read_first[g + 1] - read_first[g]));
+        const phmm_regions groups {n, hap_first.data(), read_first.data(), nullptr};
+        ReadAssignment a;
+        a.top.resize(static_cast<std::size_t>(std::max(0, reads.n)));
+        a.status.resize(pairs);
+        if (want_likelihoods) a.likelihood.resize(pairs);
+        a.code = phmm_assign_reads(get(), &config, &haplotypes, &reads, &groups, log_priors ? log_priors->data() : nullptr, a.top.data(),
+                                   want_likelihoods ? a.likelihood.data() : nullptr, a.status.data(), PHMM_SPACE_HOST);
+        if (a.code != PHMM_ERR_SHORT_HAPLOTYPE) check(a.code);
+        return a;
+    }
 private:
     std::shared_ptr<phmm_engine> handle_;
 };
@@ -449,6 +480,61 @@ inline std::vector<Realignment> realign(const ReadBlock& reads, const HaplotypeB
         if (code == PHMM_STATUS_CIGAR_TRUNCATED) throw Error {PHMM_ERR_INVALID, "CIGAR truncated"};
         result.push_back(Realignment {a.mapping_position[r], a.cigar[r], a.likelihood[r]});
     }
+    return result;
+}
+
+// AssignmentConfig::AmbiguousAction (core/tools/read_assigner.hpp). random needs the caller's RNG: apply it to
+// HaplotypeSupport::ambiguous yourself (the helper treats it as drop).
+enum class AmbiguousAction { drop, first, all, random };
+
+// One genotype's result of compute_haplotype_support(genotype, reads, log_priors, model, ambiguous, config): the reads (indices into
+// the read block) supported by each of the genotype's haplotypes, in genotype order, and the ambiguous reads with their top sets
+// (group-local haplotype indices, ascending: AmbiguousRecord::haplotypes, the default), in read order.
+struct HaplotypeSupport
+{
+    std::vector<std::vector<std::size_t>> reads;
+    std::vector<std::pair<std::size_t, std::vector<unsigned>>> ambiguous;
+};
+
+// compute_haplotype_support (core/tools/read_assigner.cpp:322-459) for many genotypes in one GPU call: group g (one genotype, after the
+// caller's collapse) owns haplotypes [hap_first[g], hap_first[g+1]) and reads [read_first[g], read_first[g+1]). log_priors: one per
+// haplotype of the block, or null. When a haplotype is too short, throws ShortHaplotypeError for the first short (haplotype, read)
+// pair in the reference's order (groups in turn, haplotypes in genotype order, then reads), with the block's haplotype index.
+inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& reads, const HaplotypeBlock& haplotypes,
+                                                               const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
+                                                               const std::vector<double>* log_priors, AmbiguousAction action,
+                                                               const phmm_config& config, const Engine& engine = Engine {})
+{
+    const auto a = engine.assign_reads(config, haplotypes.view(), reads.view(), hap_first, read_first, log_priors);
+    std::vector<HaplotypeSupport> result(hap_first.size() - 1);
+    std::size_t slot = 0;
+    for (std::size_t g = 0; g + 1 < hap_first.size(); ++g) {
+        const auto nh = static_cast<std::size_t>(hap_first[g + 1] - hap_first[g]), nr = static_cast<std::size_t>(read_first[g + 1] - read_first[g]);
+        if (a.code == PHMM_ERR_SHORT_HAPLOTYPE) {
+            for (std::size_t i = 0; i < nh * nr; ++i) {
+                if ((a.status[slot + i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP)
+                    throw ShortHaplotypeError {hap_first[g] + i / nr, static_cast<unsigned>(static_cast<std::uint32_t>(a.status[slot + i]) >> 16)};
+            }
+            slot += nh * nr;
+            continue;
+        }
+        HaplotypeSupport& s = result[g];
+        s.reads.resize(nh);
+        for (std::size_t i = 0; i < nr; ++i) {
+            const std::size_t r = static_cast<std::size_t>(read_first[g]) + i;
+            const std::uint64_t top = a.top[r];
+            if ((top & (top - 1)) == 0) {                       // one haplotype
+                for (unsigned k = 0; k < nh; ++k) if (top >> k & 1u) s.reads[k].push_back(r);
+                continue;
+            }
+            std::vector<unsigned> set;
+            for (unsigned k = 0; k < nh; ++k) if (top >> k & 1u) set.push_back(k);
+            if (action == AmbiguousAction::first) s.reads[set.front()].push_back(r);
+            else if (action == AmbiguousAction::all) for (unsigned k : set) s.reads[k].push_back(r);
+            s.ambiguous.emplace_back(r, std::move(set));
+        }
+    }
+    if (a.code == PHMM_ERR_SHORT_HAPLOTYPE) throw Error {a.code, "Haplotype is too short for alignment"};
     return result;
 }
 

@@ -67,6 +67,7 @@ struct phmm_engine {
     DBuf tasks_lane, tasks_generic, works, scores, mapq_tab;
     DBuf rhash, kbins, kitems, kpos, kcnt, ftasks, fcnt, gtasks, atasks, gcnt, sched, sorted, fb_scratch, fb_pairs, npre_f, npre_r;
     DBuf pm_best, pm_cnt, pm_inl, pm_part, pm_misc;   // the pair mapper's first pass (k_kmer_map_pairs) and its offset scan
+    DBuf as_pairs, as_prior, as_top;                  // phmm_assign_reads: slot-ordered pair list, log priors, top sets
     std::vector<cudaEvent_t> tile_events;
     std::vector<int2> info_host;
     // per-kernel launch configuration already applied / queried (the runtime calls are not free and need not be repeated)
@@ -332,7 +333,7 @@ void phmm_destroy(phmm_engine* e)
                    &e->tab_f, &e->tab_r, &e->rowhalf, &e->info, &e->flags, &e->best, &e->status, &e->out, &e->slow,
                    &e->counters, &e->pairs, &e->generic_reads, &e->wide_reads, &e->bp, &e->regs, &e->rregion, &e->rpbase, &e->rpstride, &e->tasks_lane, &e->tasks_generic, &e->works, &e->scores, &e->mapq_tab,
                    &e->rhash, &e->kbins, &e->kitems, &e->kpos, &e->kcnt, &e->ftasks, &e->fcnt, &e->gtasks, &e->atasks, &e->gcnt, &e->sched, &e->sorted, &e->fb_scratch, &e->fb_pairs, &e->npre_f, &e->npre_r,
-                   &e->pm_best, &e->pm_cnt, &e->pm_inl, &e->pm_part, &e->pm_misc};
+                   &e->pm_best, &e->pm_cnt, &e->pm_inl, &e->pm_part, &e->pm_misc, &e->as_pairs, &e->as_prior, &e->as_top};
     for (DBuf* b : all) b->release();
     for (cudaEvent_t ev : e->tile_events) cudaEventDestroy(ev);
     if (e->ev0) cudaEventDestroy(e->ev0);
@@ -904,11 +905,49 @@ struct RegionSetup {
     bool any_flank = false;
 };
 
+// The region list of phmm_populate_regions / phmm_assign_reads, checked and laid out: result offsets, widest region, flank states.
+static int region_setup(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                        const phmm_regions* regions, RegionSetup& setup)
+{
+    if (!regions || regions->n <= 0 || !regions->hap_first || !regions->read_first || !haps || !reads) { e->err = "null / empty region list"; return PHMM_ERR_INVALID; }
+    setup.regs.resize((size_t)regions->n);
+    if (regions->hap_first[0] != 0 || regions->read_first[0] != 0 || regions->hap_first[regions->n] != haps->n || regions->read_first[regions->n] != reads->n) {
+        e->err = "region ranges must cover the haplotype and read blocks exactly"; return PHMM_ERR_INVALID;
+    }
+    for (int g = 0; g < regions->n; ++g) {
+        RegionInfo& r = setup.regs[(size_t)g];
+        r.h0 = regions->hap_first[g]; r.nH = regions->hap_first[g + 1] - r.h0;
+        r.r0 = regions->read_first[g]; r.nR = regions->read_first[g + 1] - r.r0;
+        if (r.nH <= 0 || r.nR <= 0) { e->err = "every region needs at least one haplotype and one read"; return PHMM_ERR_INVALID; }
+        r.out_off = setup.total_out;
+        setup.total_out += (long long)r.nH * r.nR;
+        setup.Hmax = std::max(setup.Hmax, r.nH);
+        const bool fl = regions->flank && regions->flank[g].has_flank && cfg && cfg->use_flank_state;
+        r.use_flanks = fl ? 1 : 0; r.lhs = fl ? (int)regions->flank[g].lhs_flank : 0; r.rhs = fl ? (int)regions->flank[g].rhs_flank : 0; r.pad = 0;
+        setup.any_flank = setup.any_flank || fl;
+    }
+    return PHMM_OK;
+}
+
+// What phmm_assign_reads hands populate_impl: the batch it has staged already (the pair mapper read it), the mapper's CSR over the
+// call's result slots on the device (null: cfg->map_positions = 0), the log priors on the device (or null), and the caller's outputs.
+// populate_impl then keeps its matrix on the device, chooses every read's haplotypes there (k_assign_top) and copies out top and
+// the optional lnl / status only.
+struct AssignArgs {
+    const Staged* staged = nullptr;
+    const long long* pos_off = nullptr;
+    const int32_t* pos = nullptr;
+    long long n_pos = 0;
+    const double* log_priors = nullptr;
+    uint64_t* top = nullptr;
+};
+
 static int populate_impl(phmm_engine* e, const phmm_config* cfg,
                          const phmm_haplotypes* haps, const phmm_reads* reads,
                          const phmm_positions* positions, const phmm_flank_state* flank,
                          double* out, int32_t* status, int space, long long out_pitch,
-                         const int64_t* template_off = nullptr, int n_templates = 0, const RegionSetup* multi = nullptr)
+                         const int64_t* template_off = nullptr, int n_templates = 0, const RegionSetup* multi = nullptr,
+                         const AssignArgs* assign = nullptr)
 {
     if (!e) return PHMM_ERR_INVALID;
     static const bool trace = std::getenv("PHMM_TRACE") != nullptr;
@@ -917,13 +956,14 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
         if (trace) std::fprintf(stderr, "[phmm %p] %-18s %8.3f ms  (abs %.3f)\n", (void*)e, what, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(),
                                 std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count());
     };
-    e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
+    if (!assign) { e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0; }   // assign: counted from its mapper on
     if (cudaSetDevice(e->device) != cudaSuccess) { e->err = "cudaSetDevice failed"; return PHMM_ERR_CUDA; }
-    int rc = phmm_checks::config_and_output(cfg, out, reads, e->err);
+    int rc = phmm_checks::config_and_output(cfg, assign ? (const void*)assign->top : (const void*)out, reads, e->err);
     if (rc != PHMM_OK) return rc;
     const int band = round_band(std::max(1, cfg->max_indel_error));
     Staged s;
-    rc = stage_batch(e, haps, reads, space, s, false, true);
+    if (assign) s = *assign->staged;
+    else rc = stage_batch(e, haps, reads, space, s, false, true);
     if (rc != PHMM_OK) return rc;
     const int H_total = s.hp.n, R = s.rd.n;
     RegionSetup single;
@@ -977,16 +1017,22 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
     // (haplotype_likelihood_model.cpp:211-259); at most (listed + 1) of them reach a DP
     int max_cand = 2, max_dp_per_pair = 1;
     if (positions && positions->off && positions->pos && G > 1) { e->err = "candidate position lists are not supported with several regions"; return PHMM_ERR_INVALID; }
-    if (positions && positions->off && positions->pos) {
+    const bool device_list = assign && assign->pos_off;          // phmm_assign_reads: the pair mapper's CSR, already on the device
+    if ((positions && positions->off && positions->pos) || device_list) {
         // Candidate lists: CSR arrays on the device; the host needs the total (to size the copy) and the longest list (to size the
         // per-read task lists: the reference accepts lists of any length) — reduced on the device, 32 bytes back.
         std::vector<long long> ends(1);
-        if (space == PHMM_SPACE_HOST) ends[0] = positions->off[HR];
-        else { CU(cudaMemcpyAsync(ends.data(), positions->off + HR, sizeof(int64_t), cudaMemcpyDeviceToHost, e->stream)); CU(cudaStreamSynchronize(e->stream)); }
-        if (ends[0] < 0) { e->err = "candidate position offsets must be non-decreasing and start at 0"; return PHMM_ERR_INVALID; }
         const long long* po; const int32_t* pv;
-        if ((rc = stage(e, e->c_off, (const long long*)positions->off, (size_t)HR + 1, space, &po))) return rc;
-        if ((rc = stage(e, e->c_pos, positions->pos, (size_t)std::max<long long>(ends[0], 1), space, &pv))) return rc;
+        if (device_list) {
+            ends[0] = assign->n_pos;
+            po = assign->pos_off; pv = assign->pos;
+        } else {
+            if (space == PHMM_SPACE_HOST) ends[0] = positions->off[HR];
+            else { CU(cudaMemcpyAsync(ends.data(), positions->off + HR, sizeof(int64_t), cudaMemcpyDeviceToHost, e->stream)); CU(cudaStreamSynchronize(e->stream)); }
+            if (ends[0] < 0) { e->err = "candidate position offsets must be non-decreasing and start at 0"; return PHMM_ERR_INVALID; }
+            if ((rc = stage(e, e->c_off, (const long long*)positions->off, (size_t)HR + 1, space, &po))) return rc;
+            if ((rc = stage(e, e->c_pos, positions->pos, (size_t)std::max<long long>(ends[0], 1), space, &pv))) return rc;
+        }
         p.pos_off = po; p.pos = pv;
         OffsetSummary ps {};
         CU(e->scores.ensure(sizeof(OffsetSummary)));
@@ -1003,7 +1049,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
         max_cand = kMaxMapped + 2;   // the mapper emits <= 10 (haplotype_likelihood_array.hpp:103-104)
         max_dp_per_pair = kMaxMapped + 1;
     }
-    const bool use_mapper = !(positions && positions->off && positions->pos) && cfg->map_positions;
+    const bool use_mapper = !(positions && positions->off && positions->pos) && !assign && cfg->map_positions;
     p.single_candidate = max_dp_per_pair == 1 ? 1 : 0;
     // bands 32 / 64 with enough tasks per read to fill a warp: one WARP per chunk of the band (k_populate_roles) instead of one lane
     static const bool no_role_warps = std::getenv("PHMM_NO_ROLE_WARPS") != nullptr;       // measurement hook: the lane-per-chunk kernel for every band
@@ -1098,7 +1144,7 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
     p.best = e->best.as<int>();
     p.status = e->status.as<int>();
     CU(e->out.ensure((size_t)HR * sizeof(double)));
-    double* d_out = (space == PHMM_SPACE_DEVICE && !template_off) ? out : e->out.as<double>();
+    double* d_out = (space == PHMM_SPACE_DEVICE && !template_off && out) ? out : e->out.as<double>();   // out: null only for assign
     p.out = d_out;
     p.out_row_extra = d_out == out && space == PHMM_SPACE_DEVICE && out_pitch > R ? out_pitch - R : 0LL;
     p.out_status = status ? p.status : nullptr;
@@ -1445,6 +1491,20 @@ static int populate_impl(phmm_engine* e, const phmm_config* cfg,
         } else if (status) {
             CU(cudaMemcpyAsync(status, p.status, (size_t)HR * sizeof(int), cudaMemcpyDeviceToDevice, e->stream));
         }
+    } else if (assign) {
+        // every read's top set from the finished matrix; then only top and the optional lnl / status leave the device
+        unsigned long long* d_top = (unsigned long long*)assign->top;
+        if (space == PHMM_SPACE_HOST) { CU(e->as_top.ensure((size_t)R * sizeof(uint64_t))); d_top = e->as_top.as<unsigned long long>(); }
+        k_assign_top<<<(unsigned)((G + 3) / 4), 128, 0, e->stream>>>(G, e->regs.as<RegionInfo>(), d_out, assign->log_priors, d_top);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        if (space == PHMM_SPACE_HOST) {
+            CU(cudaMemcpyAsync(assign->top, d_top, (size_t)R * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+            if (out) CU(cudaMemcpyAsync(out, d_out, (size_t)HR * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            if (status) CU(cudaMemcpyAsync(status, p.status, (size_t)HR * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+        } else if (status) {
+            CU(cudaMemcpyAsync(status, p.status, (size_t)HR * sizeof(int), cudaMemcpyDeviceToDevice, e->stream));
+        }
     } else if (space == PHMM_SPACE_HOST) {
         if (out_pitch == 0 || out_pitch == R) {
             CU(cudaMemcpyAsync(out, d_out, (size_t)HR * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
@@ -1499,25 +1559,48 @@ int phmm_populate_regions(phmm_engine* e, const phmm_config* cfg,
                           double* out, int32_t* status, int space)
 {
     if (!e) return PHMM_ERR_INVALID;
-    if (!regions || regions->n <= 0 || !regions->hap_first || !regions->read_first || !haps || !reads) { e->err = "null / empty region list"; return PHMM_ERR_INVALID; }
     RegionSetup setup;
-    setup.regs.resize((size_t)regions->n);
-    if (regions->hap_first[0] != 0 || regions->read_first[0] != 0 || regions->hap_first[regions->n] != haps->n || regions->read_first[regions->n] != reads->n) {
-        e->err = "region ranges must cover the haplotype and read blocks exactly"; return PHMM_ERR_INVALID;
-    }
-    for (int g = 0; g < regions->n; ++g) {
-        RegionInfo& r = setup.regs[(size_t)g];
-        r.h0 = regions->hap_first[g]; r.nH = regions->hap_first[g + 1] - r.h0;
-        r.r0 = regions->read_first[g]; r.nR = regions->read_first[g + 1] - r.r0;
-        if (r.nH <= 0 || r.nR <= 0) { e->err = "every region needs at least one haplotype and one read"; return PHMM_ERR_INVALID; }
-        r.out_off = setup.total_out;
-        setup.total_out += (long long)r.nH * r.nR;
-        setup.Hmax = std::max(setup.Hmax, r.nH);
-        const bool fl = regions->flank && regions->flank[g].has_flank && cfg && cfg->use_flank_state;
-        r.use_flanks = fl ? 1 : 0; r.lhs = fl ? (int)regions->flank[g].lhs_flank : 0; r.rhs = fl ? (int)regions->flank[g].rhs_flank : 0; r.pad = 0;
-        setup.any_flank = setup.any_flank || fl;
-    }
+    const int rc = region_setup(e, cfg, haps, reads, regions, setup);
+    if (rc != PHMM_OK) return rc;
     return populate_impl(e, cfg, haps, reads, nullptr, nullptr, out, status, space, 0, nullptr, 0, &setup);
+}
+
+int phmm_assign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                      const phmm_regions* groups, const double* log_priors, uint64_t* top, double* lnl, int32_t* status, int space)
+{
+    if (!e) return PHMM_ERR_INVALID;
+    e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
+    RegionSetup setup;
+    int rc = region_setup(e, cfg, haps, reads, groups, setup);
+    if (rc != PHMM_OK) return rc;
+    if ((rc = phmm_checks::config_and_output(cfg, top, reads, e->err)) != PHMM_OK) return rc;
+    if (setup.Hmax > 64) { e->err = "more than 64 haplotypes in one group: a read's top set is a 64-bit mask"; return PHMM_ERR_INVALID; }
+    if (setup.total_out > 0x7fffffffLL) { e->err = "more than 2^31 - 1 (read, haplotype) pairs in one call"; return PHMM_ERR_INVALID; }
+    if (cudaSetDevice(e->device) != cudaSuccess) { e->err = "cudaSetDevice failed"; return PHMM_ERR_CUDA; }
+    // the blocks are staged once: the pair mapper and the DP read the same device copies
+    Staged s;
+    if ((rc = stage_batch(e, haps, reads, space, s, false, true)) != PHMM_OK) return rc;
+    AssignArgs a;
+    a.staged = &s;
+    a.top = top;
+    if ((rc = stage(e, e->as_prior, log_priors, (size_t)haps->n, space, &a.log_priors))) return rc;
+    if (cfg->map_positions) {
+        // every slot's (read, haplotype) pair in slot order, mapped uncapped: a CSR over the result slots (one synchronisation sizes it)
+        const int G = (int)setup.regs.size(), HR = (int)setup.total_out;
+        CU(e->regs.ensure((size_t)G * sizeof(RegionInfo)));
+        CU(cudaMemcpyAsync(e->regs.p, setup.regs.data(), (size_t)G * sizeof(RegionInfo), cudaMemcpyHostToDevice, e->stream));
+        CU(e->as_pairs.ensure((size_t)HR * sizeof(int2)));
+        k_slot_pairs<<<(unsigned)((HR + 255) / 256), 256, 0, e->stream>>>(HR, G, e->regs.as<RegionInfo>(), e->as_pairs.as<int2>());
+        LAUNCHED();
+        long long total = 0;
+        int variant = 0;
+        CU(e->c_off.ensure(((size_t)HR + 1) * sizeof(long long)));
+        if ((rc = pair_map_count(e, s, e->as_pairs.as<int2>(), HR, e->c_off.as<long long>(), &total, &variant))) return rc;
+        CU(e->c_pos.ensure((size_t)std::max<long long>(total, 1) * sizeof(int32_t)));
+        if ((rc = pair_map_emit(e, s, e->as_pairs.as<int2>(), HR, e->c_off.as<long long>(), e->c_pos.as<int32_t>(), variant))) return rc;
+        a.pos_off = e->c_off.as<long long>(); a.pos = e->c_pos.as<int32_t>(); a.n_pos = total;
+    }
+    return populate_impl(e, cfg, haps, reads, nullptr, nullptr, lnl, status, space, 0, nullptr, 0, &setup, &a);
 }
 
 int phmm_populate_ld(phmm_engine* e, const phmm_config* cfg,

@@ -870,6 +870,52 @@ __global__ void __launch_bounds__(1024) k_csr_scan_carry(const int n, const long
     if (i == 0) off[0] = 0;
 }
 
+// phmm_assign_reads: the (read, haplotype) pair of every result slot of a region call, in slot order. Slot i of region g is
+// out_off + (h - h0) * nR + (r - r0) = pair_slot(h, r), so the pair mapper's CSR over this list is indexed as populate_one_pair
+// reads p.pos_off[slot_hr].
+__global__ void k_slot_pairs(const long long n_slots, const int n_regions, const RegionInfo* __restrict__ regs, int2* __restrict__ pairs)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_slots) return;
+    int lo = 0, hi = n_regions;                 // largest g with regs[g].out_off <= i (every region owns >= 1 slot)
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (regs[mid].out_off <= i) lo = mid; else hi = mid; }
+    const RegionInfo g = regs[lo];
+    const long long k = i - g.out_off;
+    const int hl = (int)(k / g.nR), rl = (int)(k - (long long)hl * g.nR);
+    pairs[i] = make_int2(g.r0 + rl, g.h0 + hl);
+}
+
+// maths::almost_equal(l, r, 1) (utils/maths.hpp:68-71): l == r || |l - r| < epsilon * |l + r| * 1, each operation rounded on its own.
+__device__ __forceinline__ bool almost_equal_ulp1(const double l, const double r)
+{
+    constexpr double kEps = 2.220446049250313080847263336181640625e-16;   // std::numeric_limits<double>::epsilon()
+    return l == r || fabs(__dsub_rn(l, r)) < __dmul_rn(kEps, fabs(__dadd_rn(l, r)));
+}
+
+// find_map_haplotypes (core/tools/read_assigner.cpp:45-64) for every read of every region, on the finished values out[pair_slot]:
+// one warp per region, lanes over its reads. The haplotypes are visited in region order from max = lowest(); a value almost equal
+// to the running maximum joins the set and leaves the maximum where it is, a strictly larger one restarts the set and raises it;
+// an empty set (every value -inf or NaN) becomes every haplotype. top[r] bit k = haplotype h0 + k is in read r's set (nH <= 64).
+// log_priors: [H] per haplotype of the block, or null (the reference's vector of zeros, get_priors :36-43).
+__global__ void k_assign_top(const int n_regions, const RegionInfo* __restrict__ regs, const double* __restrict__ out,
+                             const double* __restrict__ log_priors, unsigned long long* __restrict__ top)
+{
+    const int g = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    if (g >= n_regions) return;
+    const RegionInfo reg = regs[g];
+    for (int rl = lane; rl < reg.nR; rl += 32) {
+        double max_value = -1.7976931348623157e308;                      // std::numeric_limits<double>::lowest()
+        unsigned long long set = 0ull;
+        for (int k = 0; k < reg.nH; ++k) {
+            const double cur = __dadd_rn(out[reg.out_off + (long long)k * reg.nR + rl], log_priors ? log_priors[reg.h0 + k] : 0.0);
+            if (almost_equal_ulp1(cur, max_value)) set |= 1ull << k;
+            else if (cur > max_value) { set = 1ull << k; max_value = cur; }
+        }
+        if (set == 0ull) set = reg.nH == 64 ? ~0ull : (1ull << reg.nH) - 1ull;
+        top[reg.r0 + rl] = set;
+    }
+}
+
 // Fast-path DP over the task lists the classify pass (k_populate_generic<.., true>) produced. Persistent warps: each warp
 // repeatedly claims G consecutive read pairs of equal length (G = 1, 2 or 4 lane groups; G > 1 keeps the lanes busy when a
 // read has fewer than 32 tasks, i.e. few haplotypes), stages each pair's row entries in shared memory once, and runs
