@@ -381,6 +381,56 @@ int  phmm_reset_haplotypes(const phmm_error_model* m, int32_t n, const int64_t* 
  * the library's output order. Returns the number of repeats (only the first cap are written), or a negative error code. */
 int  phmm_tandem_repeats(const char* seq, int32_t n, int32_t min_period, int32_t max_period, uint32_t* out_triples, int32_t cap);
 
+/* ---------------------------------------------------------------------------------------------------------------------
+ * DeNovoModel (core/models/mutation/denovo_model.cpp), the mutation model of the trio and cell callers (trio_caller.cpp:406-407,
+ * cell_caller.cpp:361-362) and, through SomaticMutationModel::prime (somatic_mutation_model.cpp:20-23), of the cancer caller.
+ * prime(haplotypes) (:64-84) scores every ordered (target, given) haplotype pair; each pair (evaluate_uncached, :269-293):
+ *   1. the given haplotype's context indel model, IndelMutationModel::evaluate (indel_mutation_model.cpp:67-98): exact tandem
+ *      repeats of period 1-5 (utils/repeat_finder.hpp:33-55: '$'-terminated, N runs collapsed, lib/tandem) pick per base one cell
+ *      [period][min(repeats, max_periodicity)] of the model's repeat table ([0][0] elsewhere);
+ *   2. PairHMM<VariableGapExtendMutationModel, 32, int>::align(target, given padded with 32 N's) (align_with_hmm, :254-262);
+ *   3. target_offset == 32: recalculate_log_probability (:199-218) re-scores the CIGAR: size * ln(snv_prior) per X run,
+ *      ln(calculate_indel_probability(model, pos, size)) per I / D run (indel_mutation_model.cpp:114-123);
+ *   4. otherwise (length distance >= 32, another offset, HMMOverflow): calculate_approx_log_probability over Haplotype::difference,
+ *      which stays with the caller (status APPROX_*).
+ * Step 1 runs in host C++ (bit-identical to the reference, float arithmetic included); steps 2-3 on the device. The model's
+ * min_ln_probability_ is never set in v0.7.4 (denovo_model.cpp:37, 291), so no clamp is applied.
+ * ------------------------------------------------------------------------------------------------------------------- */
+typedef struct phmm_mutation_model phmm_mutation_model;
+
+#define PHMM_MUT_HMM              0   /* out = recalculate_log_probability of the HMM alignment */
+#define PHMM_MUT_SELF             1   /* target == given (the diagonal): out = 0 */
+#define PHMM_MUT_APPROX_LENGTH    2   /* length distance >= 32 (can_try_align_with_hmm, :249-252): approximate path, out unspecified */
+#define PHMM_MUT_APPROX_OFFSET    3   /* alignment target_offset != 32 (is_valid_alignment, :264-267): approximate path, out unspecified */
+#define PHMM_MUT_APPROX_OVERFLOW  4   /* HMMOverflow: approximate path, out unspecified */
+#define PHMM_MUT_OUT_OF_MODEL     5   /* an indel at pos >= len(given): the reference reads past its model vector; out unspecified */
+
+#define PHMM_MUT_MAX_HAPLOTYPES   4096
+#define PHMM_MUT_MAX_LENGTH       65535
+
+/* The model: snv_prior in (0, 1] and IndelMutationModel's repeat table as its constructor computes it for the indel prior
+ * (indel_mutation_model.cpp:40-55): open[p * (max_periodicity + 1) + q] and extend[(p * (max_periodicity + 1) + q) * max_indel_length + k]
+ * for period p in [0, max_period], periods q in [0, max_periodicity], gap k in [0, max_indel_length). Every value in (0, 1];
+ * max_period >= 5 (the repeat finder reports periods up to 5), max_periodicity in [1, 1000], max_indel_length in [2, 1000].
+ * The reference's defaults are 10, 50, 50 (indel_mutation_model.hpp:25-26). Messages in phmm_error_model_last_error. */
+int  phmm_mutation_model_create(phmm_mutation_model** out, double snv_prior, const float* open, const float* extend,
+                                int32_t max_period, int32_t max_periodicity, int32_t max_indel_length);
+void phmm_mutation_model_destroy(phmm_mutation_model* m);
+
+/* The context indel model alone (host, no GPU): for n haplotypes (layout as phmm_haplotypes, host memory) per base the repeat-table
+ * cell (p * (max_periodicity + 1) + q) whose open / extend values IndelMutationModel::evaluate assigns, and the HMM's penalties there
+ * (probability_to_penalty of open and of extend[1], denovo_model.cpp:23-27, 184-197). Any output may be NULL.
+ * n_threads <= 0: one per hardware thread. */
+int  phmm_mutation_context(const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
+                           int32_t* cell, int8_t* open_penalty, int8_t* extend_penalty, int32_t n_threads);
+
+/* DeNovoModel::prime + evaluate for one haplotype set (host memory, layout as phmm_haplotypes; 1 <= n <= PHMM_MUT_MAX_HAPLOTYPES,
+ * every haplotype 1 .. PHMM_MUT_MAX_LENGTH bases): out[t * n + g] = ln p(target t | given g) (the reference's
+ * unguarded_index_cache_[t][g]) and status[t * n + g] = PHMM_MUT_*. The values are those of the prime of <= 50 haplotypes and of the
+ * lazy evaluate of larger sets alike. Large sets run in tiles of pairs; one kernel chain per tile. */
+int  phmm_mutation_prime(phmm_engine* e, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
+                         double* out, int32_t* status);
+
 #ifdef __cplusplus
 }
 #endif

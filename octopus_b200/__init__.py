@@ -5,8 +5,8 @@ the host-side mirror used by the tests and the benchmark: a ctypes binding (``_l
 (``batch``), the reference-shaped wrappers (``api``) and the synthetic workload generator (``synth``).
 There is no CPU fallback: importing works anywhere, computing requires an H100.
 """
-from .api import (ErrorModel, HaplotypeLikelihoodArray, HaplotypeLikelihoodModel, PairHMMEngine, PhmmError, PopulateBatcher,  # noqa: F401
-                  ShortHaplotypeError)
+from .api import (ErrorModel, HaplotypeLikelihoodArray, HaplotypeLikelihoodModel, MutationModel, PairHMMEngine, PhmmError,  # noqa: F401
+                  PopulateBatcher, ShortHaplotypeError)
 from .batch import HaplotypeBlock, ReadBlock, pack_haplotypes, pack_reads  # noqa: F401
 
 __version__ = "0.1.0"

@@ -7,11 +7,14 @@ LIB_PATH = os.path.join(_HERE, "libphmm_b200.so")
 
 PHMM_OK, PHMM_ERR_INVALID, PHMM_ERR_CUDA, PHMM_ERR_BAND, PHMM_ERR_SHORT_HAPLOTYPE, PHMM_ERR_NOMEM = 0, -1, -2, -3, -4, -5
 SPACE_HOST, SPACE_DEVICE = 0, 1
+MUT_HMM, MUT_SELF, MUT_APPROX_LENGTH, MUT_APPROX_OFFSET, MUT_APPROX_OVERFLOW, MUT_OUT_OF_MODEL = 0, 1, 2, 3, 4, 5
+MUT_MAX_HAPLOTYPES, MUT_MAX_LENGTH = 4096, 65535
 
 EXPORTS = ["phmm_version", "phmm_default_config", "phmm_create", "phmm_destroy", "phmm_last_error", "phmm_launch_count",
            "phmm_last_dp_kernel_ms", "phmm_last_dp_cells", "phmm_align_scores", "phmm_align_traceback", "phmm_align_reads", "phmm_align_pairs", "phmm_map_pairs", "phmm_realign_reads", "phmm_genotype_likelihoods", "phmm_populate", "phmm_populate_templates", "phmm_populate_regions", "phmm_assign_reads",
            "phmm_error_model_create", "phmm_error_model_create_custom", "phmm_error_model_destroy", "phmm_error_model_last_error",
-           "phmm_reset_haplotypes", "phmm_tandem_repeats", "phmm_wait_event", "phmm_engine_stream", "phmm_reserve_sms", "phmm_host_alloc", "phmm_host_free",
+           "phmm_reset_haplotypes", "phmm_tandem_repeats", "phmm_mutation_model_create", "phmm_mutation_model_destroy", "phmm_mutation_context",
+           "phmm_mutation_prime", "phmm_wait_event", "phmm_engine_stream", "phmm_reserve_sms", "phmm_host_alloc", "phmm_host_free",
            "phmm_populate_ld", "phmm_device_alloc", "phmm_device_free", "phmm_ipc_export", "phmm_ipc_open", "phmm_ipc_close",
            "phmm_batcher_create", "phmm_batcher_destroy", "phmm_batcher_last_error", "phmm_batcher_populate",
            "phmm_batcher_populate_templates", "phmm_batcher_stats_get"]
@@ -162,5 +165,12 @@ def load():
     lib.phmm_reset_haplotypes.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 9 + [C.c_int32]
     lib.phmm_tandem_repeats.restype = C.c_int
     lib.phmm_tandem_repeats.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32]
+    lib.phmm_mutation_model_create.restype = C.c_int
+    lib.phmm_mutation_model_create.argtypes = [C.POINTER(C.c_void_p), C.c_double, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
+    lib.phmm_mutation_model_destroy.argtypes = [C.c_void_p]
+    lib.phmm_mutation_context.restype = C.c_int
+    lib.phmm_mutation_context.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]
+    lib.phmm_mutation_prime.restype = C.c_int
+    lib.phmm_mutation_prime.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = lib
     return lib

@@ -5,6 +5,7 @@ Names and argument meaning follow the reference:
   * ``HaplotypeLikelihoodModel.Config``       ↔ HaplotypeLikelihoodModel::Config (haplotype_likelihood_model.hpp:36-44)
   * ``HaplotypeLikelihoodArray.populate``     ↔ HaplotypeLikelihoodArray::populate (haplotype_likelihood_array.cpp:51-103)
   * ``ShortHaplotypeError``                   ↔ HaplotypeLikelihoodModel::ShortHaplotypeError (:123-139)
+  * ``MutationModel`` + ``PairHMMEngine.mutation_prime`` ↔ DeNovoModel::prime / evaluate (core/models/mutation/denovo_model.cpp:64-84)
 Every computing call goes through libphmm_b200.so to the GPU; nothing here computes likelihoods on the CPU.
 """
 import ctypes as C
@@ -96,6 +97,20 @@ class PairHMMEngine:
 
     def last_dp_cells(self):
         return int(self._lib.phmm_last_dp_cells(self._h))
+
+    # -- DeNovoModel::prime ------------------------------------------------------------------------------------
+    def mutation_prime(self, model, sequences):
+        """DeNovoModel::prime + evaluate for one haplotype set (phmm_mutation_prime): sequences (list of str / bytes) → (out, status),
+        both [H, H] indexed [target, given]. out[t, g] = ln p(target | given) where status is MUT_HMM or MUT_SELF; the MUT_APPROX_*
+        pairs need the reference's approximate path (Haplotype::difference) and MUT_OUT_OF_MODEL pairs have no defined value."""
+        off, seq = _pack_sequences(sequences)
+        H = len(off) - 1
+        out = np.zeros((H, H), dtype=np.float64)
+        status = np.zeros((H, H), dtype=np.int32)
+        rc = self._lib.phmm_mutation_prime(self._h, model._h, H, off.ctypes.data, seq.ctypes.data, out.ctypes.data, status.ctypes.data)
+        if rc != _lib.PHMM_OK:
+            self._raise(rc)
+        return out, status
 
     # -- raw kernel boundary -----------------------------------------------------------------------------------
     def align_scores(self, band, haps: HaplotypeBlock, reads: ReadBlock, tasks, nuc_prior=2, precision_bits=16):
@@ -561,6 +576,57 @@ class PopulateBatcher:
         if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
             self._raise(rc)
         return (out, status) if want_status else out
+
+
+def _pack_sequences(sequences):
+    parts = [np.frombuffer(x.encode() if isinstance(x, str) else bytes(x), dtype=np.uint8) for x in sequences]
+    off = np.zeros(len(parts) + 1, dtype=np.int64)
+    np.cumsum([len(x) for x in parts], out=off[1:])
+    seq = np.ascontiguousarray(np.concatenate(parts)) if parts else np.zeros(1, dtype=np.uint8)
+    return off, seq
+
+
+class MutationModel:
+    """DeNovoModel's parameters (core/models/mutation/denovo_model.hpp: Parameters{snv_prior, indel_prior}) as the engine holds them:
+    the SNV prior and IndelMutationModel's repeat table for the indel prior (indel_mutation_model.cpp:40-55), open [P+1, Q+1] and
+    extend [P+1, Q+1, X] float32 probabilities. The caller computes the table (it is not part of this library); the reference's
+    defaults are P = 10, Q = 50, X = 50. SomaticMutationModel uses the same model under the cancer caller's priors."""
+
+    def __init__(self, snv_prior, open_table, extend_table):
+        self._lib = _lib.load()
+        self._open = np.ascontiguousarray(open_table, dtype=np.float32)
+        self._extend = np.ascontiguousarray(extend_table, dtype=np.float32)
+        if self._open.ndim != 2 or self._extend.ndim != 3 or self._extend.shape[:2] != self._open.shape:
+            raise ValueError("open must be [P+1, Q+1] and extend [P+1, Q+1, X]")
+        P, Q, X = self._open.shape[0] - 1, self._open.shape[1] - 1, self._extend.shape[2]
+        h = C.c_void_p()
+        rc = self._lib.phmm_mutation_model_create(C.byref(h), float(snv_prior), self._open.ctypes.data, self._extend.ctypes.data, P, Q, X)
+        if rc != _lib.PHMM_OK:
+            raise PhmmError(rc, self._lib.phmm_error_model_last_error().decode())
+        self._h = h
+        self.snv_prior = float(snv_prior)
+        self.max_period, self.max_periodicity, self.max_indel_length = P, Q, X
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                self._lib.phmm_mutation_model_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def context(self, sequences, n_threads=0):
+        """IndelMutationModel::evaluate per haplotype (host): (cell, open_penalty, extend_penalty), flat over the concatenated bases.
+        cell = period * (max_periodicity + 1) + periods of the repeat-table cell each base takes its probabilities from."""
+        off, seq = _pack_sequences(sequences)
+        total = int(off[-1])
+        cell = np.empty(total, dtype=np.int32)
+        op, ep = np.empty(total, dtype=np.int8), np.empty(total, dtype=np.int8)
+        rc = self._lib.phmm_mutation_context(self._h, len(off) - 1, off.ctypes.data, seq.ctypes.data, cell.ctypes.data, op.ctypes.data,
+                                             ep.ctypes.data, int(n_threads))
+        if rc != _lib.PHMM_OK:
+            raise PhmmError(rc, self._lib.phmm_error_model_last_error().decode())
+        return cell, op, ep
 
 
 class ErrorModel:

@@ -19,6 +19,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <cstdlib>
+#include <functional>
 #include <memory>
 #include <new>
 #include <stdexcept>
@@ -539,6 +540,120 @@ inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& 
 }
 
 using SampleName = std::string;
+
+// ---------------------------------------------------------------------------------------------------------------------
+// DeNovoModel (core/models/mutation/denovo_model.{hpp,cpp}) over phmm_mutation_prime
+// ---------------------------------------------------------------------------------------------------------------------
+// IndelMutationModel's repeat table for one indel prior: cell (period p, periods q) at p * (max_periodicity + 1) + q; open[cell],
+// extend[cell * max_indel_length + gap]. The values are Octopus's: with the reference's indel_mutation_model_config.hpp included
+// before this header, from_reference(indel_prior) computes them as IndelMutationModel's constructor does (indel_mutation_model.cpp:17-55).
+struct MutationRepeatTable
+{
+    int max_period = 10, max_periodicity = 50, max_indel_length = 50;   // IndelMutationModel::Parameters defaults (.hpp:25-26)
+    std::vector<float> open, extend;
+#ifdef indel_mutation_model_config_hpp
+    static MutationRepeatTable from_reference(const double indel_prior, const unsigned max_period = 10, const unsigned max_periodicity = 50,
+                                              const unsigned max_indel_length = 50, const double max_open_probability = 0.9,
+                                              const double max_extend_probability = 1.0)
+    {
+        using octopus::enrichment_model;
+        using octopus::extension_model;
+        MutationRepeatTable t;
+        t.max_period = static_cast<int>(max_period);
+        t.max_periodicity = static_cast<int>(max_periodicity);
+        t.max_indel_length = static_cast<int>(max_indel_length);
+        const unsigned e_period = static_cast<unsigned>(enrichment_model.size() - 1), e_periods = static_cast<unsigned>(enrichment_model.front().size() - 1);
+        const unsigned x_period = static_cast<unsigned>(extension_model.size() - 1), x_periods = static_cast<unsigned>(extension_model.front().size() - 1);
+        const unsigned x_gap = static_cast<unsigned>(extension_model.front().front().size() - 1);
+        for (unsigned period = 0; period <= max_period; ++period) {
+            for (unsigned periods = 0; periods <= max_periodicity; ++periods) {
+                // calculate_gap_open_prior / calculate_gap_extend_prior (:17-37)
+                const double open_prior = (period == 0 || periods == 0) ? indel_prior
+                    : std::min(indel_prior * enrichment_model[std::min(period, e_period)][std::min(periods, e_periods)], 1.0);
+                t.open.push_back(static_cast<float>(std::min(open_prior, max_open_probability)));
+                for (unsigned gap = 0; gap < max_indel_length; ++gap) {
+                    const double extend_prior = std::max(open_prior, extension_model[std::min(period, x_period)][std::min(periods, x_periods)][std::min(gap, x_gap)]);
+                    t.extend.push_back(static_cast<float>(std::min(extend_prior, max_extend_probability)));
+                }
+            }
+        }
+        return t;
+    }
+#endif
+};
+
+// DeNovoModel: prime(sequences) scores every ordered (target, given) pair of one region's haplotypes in one GPU call
+// (phmm_mutation_prime); evaluate(target, given) = ln p(target | given), the reference's evaluate(IndexedHaplotype, IndexedHaplotype).
+// Pairs the reference sends to its approximate path (length distance >= 32, another alignment offset, HMMOverflow) need
+// Haplotype::difference, which lives with the caller: evaluate calls approx(target, given) for them, once, and keeps the value. So does
+// a pair whose alignment puts an indel past the given haplotype (PHMM_MUT_OUT_OF_MODEL: the reference's value is undefined there).
+// SomaticMutationModel::prime (somatic_mutation_model.cpp:20-23) is the same model under the cancer caller's priors.
+class DeNovoModel
+{
+public:
+    using LogProbability = double;
+    struct Parameters { double snv_prior, indel_prior; };
+    using ApproxFunction = std::function<LogProbability(std::size_t target_idx, std::size_t given_idx)>;
+
+    DeNovoModel(Parameters parameters, const MutationRepeatTable& table, Engine& engine, ApproxFunction approx = nullptr)
+    : params_ {parameters}, engine_ {&engine}, approx_ {std::move(approx)}
+    {
+        phmm_mutation_model* m = nullptr;
+        const int rc = phmm_mutation_model_create(&m, parameters.snv_prior, table.open.data(), table.extend.data(), table.max_period,
+                                                  table.max_periodicity, table.max_indel_length);
+        if (rc != PHMM_OK) throw Error {rc, phmm_error_model_last_error()};
+        model_.reset(m, [] (phmm_mutation_model* p) { phmm_mutation_model_destroy(p); });
+    }
+#ifdef indel_mutation_model_config_hpp
+    DeNovoModel(Parameters parameters, Engine& engine, ApproxFunction approx = nullptr)
+    : DeNovoModel {parameters, MutationRepeatTable::from_reference(parameters.indel_prior), engine, std::move(approx)} {}
+#endif
+
+    Parameters parameters() const { return params_; }
+
+    void prime(const std::vector<std::string>& haplotypes)
+    {
+        if (is_primed()) throw std::runtime_error {"DeNovoModel: already primed"};
+        const std::size_t n = haplotypes.size();
+        std::vector<std::int64_t> off(n + 1, 0);
+        std::string seq;
+        for (std::size_t h = 0; h < n; ++h) { seq += haplotypes[h]; off[h + 1] = static_cast<std::int64_t>(seq.size()); }
+        values_.assign(n * n, 0.0);
+        status_.assign(n * n, PHMM_MUT_SELF);
+        settled_.assign(n * n, 0);
+        if (n > 0) engine_->check(phmm_mutation_prime(engine_->get(), model_.get(), static_cast<std::int32_t>(n), off.data(), seq.data(),
+                                                      values_.data(), status_.data()));
+        n_ = n;
+    }
+    void unprime() noexcept { values_ = {}; status_ = {}; settled_ = {}; n_ = 0; }
+    bool is_primed() const noexcept { return n_ > 0; }
+
+    // ln p(target | given) for haplotype indices of the primed set
+    LogProbability evaluate(const std::size_t target_idx, const std::size_t given_idx) const
+    {
+        if (target_idx >= n_ || given_idx >= n_) throw std::out_of_range {"DeNovoModel::evaluate: haplotype index"};
+        const std::size_t i = target_idx * n_ + given_idx;
+        if (status_[i] == PHMM_MUT_HMM || status_[i] == PHMM_MUT_SELF || settled_[i]) return values_[i];
+        if (!approx_) throw Error {PHMM_ERR_INVALID, "DeNovoModel: an approximate pair needs the approx function"};
+        values_[i] = approx_(target_idx, given_idx);
+        settled_[i] = 1;
+        return values_[i];
+    }
+    // PHMM_MUT_* of a pair (PHMM_MUT_APPROX_* / OUT_OF_MODEL: evaluate asks approx)
+    std::int32_t status(const std::size_t target_idx, const std::size_t given_idx) const { return status_.at(target_idx * n_ + given_idx); }
+
+private:
+    Parameters params_;
+    Engine* engine_;
+    ApproxFunction approx_;
+    std::shared_ptr<phmm_mutation_model> model_;
+    std::size_t n_ = 0;
+    mutable std::vector<double> values_;
+    std::vector<std::int32_t> status_;
+    mutable std::vector<char> settled_;
+};
+
+using SomaticMutationModel = DeNovoModel;
 
 // A read-only view of one likelihoods_[haplotype][sample] vector (the reference returns const std::vector<double>&).
 struct LikelihoodSpan

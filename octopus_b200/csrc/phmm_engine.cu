@@ -3,6 +3,7 @@
 // computing entry point returns PHMM_ERR_CUDA.
 #include "../../include/phmm_b200.h"
 #include "phmm_checks.h"
+#include "phmm_mutation.h"
 #include "phmm_kernels.cuh"
 
 #include <algorithm>
@@ -68,6 +69,7 @@ struct phmm_engine {
     DBuf rhash, kbins, kitems, kpos, kcnt, ftasks, fcnt, gtasks, atasks, gcnt, sched, sorted, fb_scratch, fb_pairs, npre_f, npre_r;
     DBuf pm_best, pm_cnt, pm_inl, pm_part, pm_misc;   // the pair mapper's first pass (k_kmer_map_pairs) and its offset scan
     DBuf as_pairs, as_prior, as_top;                  // phmm_assign_reads: slot-ordered pair list, log priors, top sets
+    DBuf mu_in, mu_list, mu_res, mu_cig, mu_out;      // phmm_mutation_prime: staged set, DP pair list, per-tile results, CIGARs, matrix
     std::vector<cudaEvent_t> tile_events;
     std::vector<int2> info_host;
     // per-kernel launch configuration already applied / queried (the runtime calls are not free and need not be repeated)
@@ -333,7 +335,8 @@ void phmm_destroy(phmm_engine* e)
                    &e->tab_f, &e->tab_r, &e->rowhalf, &e->info, &e->flags, &e->best, &e->status, &e->out, &e->slow,
                    &e->counters, &e->pairs, &e->generic_reads, &e->wide_reads, &e->bp, &e->regs, &e->rregion, &e->rpbase, &e->rpstride, &e->tasks_lane, &e->tasks_generic, &e->works, &e->scores, &e->mapq_tab,
                    &e->rhash, &e->kbins, &e->kitems, &e->kpos, &e->kcnt, &e->ftasks, &e->fcnt, &e->gtasks, &e->atasks, &e->gcnt, &e->sched, &e->sorted, &e->fb_scratch, &e->fb_pairs, &e->npre_f, &e->npre_r,
-                   &e->pm_best, &e->pm_cnt, &e->pm_inl, &e->pm_part, &e->pm_misc, &e->as_pairs, &e->as_prior, &e->as_top};
+                   &e->pm_best, &e->pm_cnt, &e->pm_inl, &e->pm_part, &e->pm_misc, &e->as_pairs, &e->as_prior, &e->as_top,
+                   &e->mu_in, &e->mu_list, &e->mu_res, &e->mu_cig, &e->mu_out};
     for (DBuf* b : all) b->release();
     for (cudaEvent_t ev : e->tile_events) cudaEventDestroy(ev);
     if (e->ev0) cudaEventDestroy(e->ev0);
@@ -889,6 +892,131 @@ int phmm_map_pairs(phmm_engine* e, const phmm_haplotypes* haps, const phmm_reads
     }
     if (!dev) CU(cudaMemcpyAsync(off, off_dev, ((size_t)n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
+    return PHMM_OK;
+}
+
+// -------------------------------------------------------------------------------------------------------------
+// phmm_mutation_prime
+// -------------------------------------------------------------------------------------------------------------
+// Largest tile of the ordered-pair index space, and the CIGAR scratch a tile may use.
+static constexpr long long kMutTilePairs = 1LL << 19;
+static constexpr long long kMutCigarBudget = 1LL << 30;
+
+int phmm_mutation_prime(phmm_engine* e, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
+                        double* out, int32_t* status)
+{
+    if (!e) return PHMM_ERR_INVALID;
+    e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
+    if (!m || !off || !seq || !out || !status) { e->err = "null argument"; return PHMM_ERR_INVALID; }
+    if (n < 1 || n > PHMM_MUT_MAX_HAPLOTYPES) { e->err = "haplotype count outside [1, 4096]"; return PHMM_ERR_INVALID; }
+    if (off[0] != 0) { e->err = "offset arrays must start at 0"; return PHMM_ERR_INVALID; }
+    long long Lmax = 0;
+    for (int h = 0; h < n; ++h) {
+        const long long len = off[h + 1] - off[h];
+        if (len < 1 || len > PHMM_MUT_MAX_LENGTH) { e->err = "haplotype length outside [1, 65535]"; return PHMM_ERR_INVALID; }
+        Lmax = std::max(Lmax, len);
+    }
+    if (cudaSetDevice(e->device) != cudaSuccess) { e->err = "cudaSetDevice failed"; return PHMM_ERR_CUDA; }
+    const int H = n, X = m->max_indel_length;
+    const long long B = off[H];
+    // 1. the context indel model of every haplotype (host)
+    std::vector<int32_t> cell((size_t)B);
+    std::vector<int8_t> gop((size_t)B), gex((size_t)B);
+    int rc = phmm_mutation_context(m, n, off, seq, cell.data(), gop.data(), gex.data(), 0);
+    if (rc != PHMM_OK) { e->err = phmm_error_model_last_error(); return rc; }
+    // 2. one padded truth per given haplotype: 32 N's, the haplotype, N's up to the longest haplotype + 64 (pad penalty 60), no SNV mask;
+    //    the targets are the haplotypes with every quality = the SNV penalty (denovo_model.cpp:208-262, pair_hmm.hpp:853-856)
+    const long long Lp = Lmax + 64;
+    auto align_up = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    size_t at = 0;
+    const size_t o_tseq = at; at = align_up(at + (size_t)H * Lp);
+    const size_t o_tgo = at;  at = align_up(at + (size_t)H * Lp);
+    const size_t o_tge = at;  at = align_up(at + (size_t)H * Lp);
+    const size_t o_zero = at; at = align_up(at + (size_t)H * Lp);                 // SNV masks / priors, mapq, reverse, begin
+    const size_t o_toff = at; at = align_up(at + ((size_t)H + 1) * sizeof(int64_t));
+    const size_t o_goff = at; at = align_up(at + ((size_t)H + 1) * sizeof(int64_t));
+    const size_t o_bases = at; at = align_up(at + (size_t)B);
+    const size_t o_quals = at; at = align_up(at + (size_t)B);
+    const size_t o_cell = at; at = align_up(at + (size_t)B * sizeof(int32_t));
+    const size_t o_logp = at; at = align_up(at + m->logp.size() * sizeof(float));
+    const long long cigar_stride = 4 * Lmax + 160;                                  // >= 2 characters per alignment column
+    const long long tile = std::max(1LL, std::min(kMutTilePairs, kMutCigarBudget / cigar_stride));
+    const size_t o_offs = at; at = align_up(at + (size_t)tile * sizeof(int32_t));
+    std::vector<char> blob(at, 0);
+    char* bp = blob.data();
+    for (int h = 0; h < H; ++h) {
+        const long long o = off[h], len = off[h + 1] - o, t0 = (long long)h * Lp;
+        std::memset(bp + o_tseq + t0, 'N', (size_t)Lp);
+        std::memcpy(bp + o_tseq + t0 + 32, seq + o, (size_t)len);
+        std::memset(bp + o_tgo + t0, 60, (size_t)Lp);
+        std::memset(bp + o_tge + t0, 60, (size_t)Lp);
+        std::memcpy(bp + o_tgo + t0 + 32, gop.data() + o, (size_t)len);
+        std::memcpy(bp + o_tge + t0 + 32, gex.data() + o, (size_t)len);
+        ((int64_t*)(bp + o_toff))[h] = t0;
+    }
+    ((int64_t*)(bp + o_toff))[H] = (int64_t)H * Lp;
+    std::memcpy(bp + o_goff, off, ((size_t)H + 1) * sizeof(int64_t));
+    std::memcpy(bp + o_bases, seq, (size_t)B);
+    std::memset(bp + o_quals, m->snv_penalty, (size_t)B);
+    std::memcpy(bp + o_cell, cell.data(), (size_t)B * sizeof(int32_t));
+    std::memcpy(bp + o_logp, m->logp.data(), m->logp.size() * sizeof(float));
+    std::fill((int32_t*)(bp + o_offs), (int32_t*)(bp + o_offs) + tile, 32);
+    CU(e->mu_in.ensure(at));
+    CU(cudaMemcpyAsync(e->mu_in.p, blob.data(), at, cudaMemcpyHostToDevice, e->stream));
+    char* d = e->mu_in.as<char>();
+    phmm_haplotypes truths {H, (const int64_t*)(d + o_toff), d + o_tseq, d + o_zero, (const int8_t*)(d + o_zero), d + o_zero,
+                            (const int8_t*)(d + o_zero), (const int8_t*)(d + o_tgo), (const int8_t*)(d + o_tge), nullptr};
+    phmm_reads targets {H, (const int64_t*)(d + o_goff), d + o_bases, (const uint8_t*)(d + o_quals), (const uint8_t*)(d + o_zero),
+                        (const uint8_t*)(d + o_zero), (const int64_t*)(d + o_zero)};
+    phmm_config cfg;
+    phmm_default_config(&cfg);
+    cfg.max_indel_error = 32; cfg.use_mapping_quality = 0; cfg.use_flank_state = 0; cfg.map_positions = 0;
+    const long long all = (long long)H * H;
+    CU(e->mu_out.ensure((size_t)all * (sizeof(double) + sizeof(int32_t))));
+    double* d_out = e->mu_out.as<double>();
+    int* d_status = (int*)(d_out + all);
+    CU(e->mu_list.ensure((size_t)tile * sizeof(int2) + 256));
+    int2* d_list = e->mu_list.as<int2>();
+    int* d_count = (int*)(d_list + tile);
+    CU(e->mu_res.ensure((size_t)tile * (sizeof(int64_t) + sizeof(double) + sizeof(int32_t))));
+    int64_t* d_toff = e->mu_res.as<int64_t>();
+    double* d_lk = (double*)(d_toff + tile);
+    int32_t* d_ast = (int32_t*)(d_lk + tile);
+    CU(e->mu_cig.ensure((size_t)tile * cigar_stride));
+    long long launches = 0;
+    double dp_ms = 0.0;
+    // 3. per tile: list the pairs, align the listed ones (band 32, target offset 32), re-score their CIGARs
+    for (long long lo = 0; lo < all; lo += tile) {
+        const long long hi = std::min(all, lo + tile);
+        CU(cudaMemsetAsync(d_count, 0, sizeof(int), e->stream));
+        k_mutation_pairs<<<(unsigned)std::min<long long>((hi - lo + 255) / 256, 4096), 256, 0, e->stream>>>(lo, hi, H, (const long long*)(d + o_goff),
+                                                                                                          d_out, d_status, d_list, d_count);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        int count = 0;
+        CU(cudaMemcpyAsync(&count, d_count, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaStreamSynchronize(e->stream));
+        if (count == 0) continue;
+        launches += e->launches_last;
+        rc = align_impl(e, &cfg, &truths, &targets, (const phmm_pair*)d_list, count, nullptr, (const int32_t*)(d + o_offs), nullptr,
+                        d_toff, d_lk, e->mu_cig.as<char>(), (int32_t)cigar_stride, d_ast, PHMM_SPACE_DEVICE);
+        launches += e->launches_last;
+        e->launches_last = 0;
+        dp_ms += e->last_dp_ms;
+        if (rc != PHMM_OK) return rc;
+        k_mutation_rescore<<<(unsigned)((count + 127) / 128), 128, 0, e->stream>>>(count, d_list, (const long long*)d_toff, d_ast, e->mu_cig.as<char>(),
+                                                                                 (int)cigar_stride, (const long long*)(d + o_goff),
+                                                                                 (const int*)(d + o_cell), (const float*)(d + o_logp), X,
+                                                                                 m->snv_log_prior, H, d_out, d_status);
+        LAUNCHED();
+        CU(cudaGetLastError());
+    }
+    CU(cudaMemcpyAsync(out, d_out, (size_t)all * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaMemcpyAsync(status, d_status, (size_t)all * sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    e->launches_last += launches;
+    e->last_dp_ms = dp_ms;
+    for (long long i = 0; i < all; ++i) if (status[i] < 0) { e->err = "internal error: CIGAR scratch too small"; return PHMM_ERR_CUDA; }
     return PHMM_OK;
 }
 

@@ -17,10 +17,12 @@
 //                                                                   with previous occurrence → LZ factors → Main's per-factor repetitions
 //                                                                   → Kolpakov-Kucherov propagation.
 #include "../../include/phmm_b200.h"
+#include "phmm_mutation.h"
 
 #include <algorithm>
 #include <atomic>
 #include <cctype>
+#include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <string>
@@ -478,6 +480,71 @@ bool parse_custom_model(const std::string& text, phmm_error_model& m, bool& has_
     return true;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// DeNovoModel's context indel model (IndelMutationModel::evaluate, indel_mutation_model.cpp:67-98)
+// ---------------------------------------------------------------------------------------------------------
+
+// find_exact_tandem_repeats(sequence, region, 1, 5) (utils/repeat_finder.hpp:33-55): the finder runs on the sequence with '$'
+// appended and every run of N collapsed to one N (tandem::collapse, tandem.hpp:528-554), and its positions are mapped back by
+// tandem::rebase (tandem.cpp:138-148). Both are restated as written: collapse's keys count the kept N of earlier runs as removed,
+// so a repeat that ends just before an N run can be shifted past its true position.
+void mutation_repeats(const unsigned char* s, const std::uint32_t n, std::vector<unsigned char>& buf, std::vector<Run>& runs)
+{
+    buf.assign(s, s + n);
+    buf.push_back('$');
+    std::vector<std::pair<std::size_t, std::size_t>> shift;          // collapse's map, keys strictly increasing
+    const std::size_t len = buf.size();
+    std::size_t first = 0, position = 0, removed = 0;
+    while (first < len) {
+        std::size_t it1 = first;
+        while (it1 + 1 < len && !(buf[it1] == 'N' && buf[it1 + 1] == 'N')) ++it1;
+        if (it1 + 1 >= len) break;
+        std::size_t it2 = it1;
+        while (it2 < len && buf[it2] == 'N') ++it2;
+        position += it1 - first;
+        removed += it2 - it1 - 1;
+        shift.emplace_back(position, removed);
+        first = it2;
+    }
+    if (!shift.empty()) {
+        std::size_t w = 0;
+        for (std::size_t r = 0; r < len; ++r) if (!(w > 0 && buf[r] == 'N' && buf[w - 1] == 'N')) buf[w++] = buf[r];
+        buf.resize(w);
+    }
+    tandem_repeats(buf.data(), (std::uint32_t)buf.size(), 1, 5, runs);
+    if (shift.empty()) return;
+    std::size_t k = 0;
+    for (Run& r : runs) {
+        while (k + 1 < shift.size() && shift[k + 1].first <= r.pos) ++k;
+        r.pos += (std::uint32_t)shift[k].second;
+    }
+}
+
+// Per base the repeat-table cell IndelMutationModel::evaluate copies gap_open / gap_extend from (:78-96): cell [0][0], replaced by a
+// later repeat's cell only where that cell's open probability is strictly larger, in the finder's output order.
+void mutation_cells(const phmm_mutation_model& m, const unsigned char* s, const std::uint32_t n, std::int32_t* cell,
+                    std::vector<unsigned char>& buf, std::vector<Run>& runs)
+{
+    std::fill(cell, cell + n, 0);
+    mutation_repeats(s, n, buf, runs);
+    const int width = m.max_periodicity + 1;
+    for (const Run& r : runs) {
+        const std::uint32_t periods = std::min<std::uint32_t>(r.len / r.period, (std::uint32_t)m.max_periodicity);
+        const int c = (int)r.period * width + (int)periods;
+        // the reference asserts the repeat lies inside the haplotype; a rebased position past the end is skipped here
+        for (std::uint32_t pos = r.pos; pos < r.pos + r.period && pos < n; ++pos) {
+            if (m.open[cell[pos]] < m.open[c]) cell[pos] = c;
+        }
+    }
+}
+
+// probability_to_penalty (denovo_model.cpp:23-27)
+std::int8_t mutation_penalty(const double probability)
+{
+    constexpr double ln10_div_10 = 0.230258509299404568401799145468436420760110148862877297603;   // maths::constants::ln10Div10<>
+    return (std::int8_t)std::max(std::min(std::round(std::log(probability) / -ln10_div_10), 127.0), 1.0);
+}
+
 int fail(const char* what) { g_error = what; return PHMM_ERR_INVALID; }
 
 } // namespace
@@ -577,6 +644,80 @@ int phmm_tandem_repeats(const char* seq, int32_t n, int32_t min_period, int32_t 
     if (!tandem_repeats((const unsigned char*)seq, (std::uint32_t)n, (std::uint32_t)min_period, (std::uint32_t)max_period, runs)) return fail("min_period > max_period");
     for (std::size_t i = 0; i < runs.size() && (int32_t)i < cap; ++i) { out_triples[3 * i] = runs[i].pos; out_triples[3 * i + 1] = runs[i].len; out_triples[3 * i + 2] = runs[i].period; }
     return (int)runs.size();
+}
+
+
+int phmm_mutation_model_create(phmm_mutation_model** out, double snv_prior, const float* open, const float* extend,
+                               int32_t max_period, int32_t max_periodicity, int32_t max_indel_length)
+{
+    if (!out) return fail("null output");
+    *out = nullptr;
+    if (!open || !extend) return fail("null repeat table");
+    if (!(snv_prior > 0.0 && snv_prior <= 1.0)) return fail("snv_prior outside (0, 1]");
+    if (max_period < 5 || max_period > 1000 || max_periodicity < 1 || max_periodicity > 1000 || max_indel_length < 2 || max_indel_length > 1000)
+        return fail("repeat table dimensions out of range (max_period 5..1000, max_periodicity 1..1000, max_indel_length 2..1000)");
+    phmm_mutation_model* m = new phmm_mutation_model();
+    m->snv_prior = snv_prior;
+    m->snv_log_prior = std::log(snv_prior);
+    m->snv_penalty = mutation_penalty(snv_prior);
+    m->max_period = max_period; m->max_periodicity = max_periodicity; m->max_indel_length = max_indel_length;
+    const int cells = m->cells(), X = max_indel_length;
+    m->open.assign(open, open + cells);
+    m->extend.assign(extend, extend + (std::size_t)cells * X);
+    for (const float v : m->open) if (!(v > 0.0f && v <= 1.0f)) { delete m; return fail("repeat table open probability outside (0, 1]"); }
+    for (const float v : m->extend) if (!(v > 0.0f && v <= 1.0f)) { delete m; return fail("repeat table extend probability outside (0, 1]"); }
+    m->open_penalty.resize(cells); m->extend_penalty.resize(cells); m->logp.resize((std::size_t)cells * X);
+    for (int c = 0; c < cells; ++c) {
+        const float* ext = m->extend.data() + (std::size_t)c * X;
+        m->open_penalty[c] = mutation_penalty(m->open[c]);
+        m->extend_penalty[c] = mutation_penalty(ext[1]);
+        // calculate_indel_probability: gap_open * gap_extend[1] * ... * gap_extend[length - 1] in float, at most X - 1 factors
+        float product = m->open[c];
+        for (int k = 0; k < X; ++k) {
+            if (k > 0) product = product * ext[k];
+            m->logp[(std::size_t)c * X + k] = std::log(product);
+        }
+    }
+    *out = m;
+    return PHMM_OK;
+}
+
+void phmm_mutation_model_destroy(phmm_mutation_model* m) { delete m; }
+
+int phmm_mutation_context(const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
+                          int32_t* cell, int8_t* open_penalty, int8_t* extend_penalty, int32_t n_threads)
+{
+    if (!m || n < 0 || (n > 0 && (!off || !seq))) return fail("null argument");
+    if (n > 0 && off[0] != 0) return fail("bad haplotype offsets");
+    for (int32_t h = 0; h < n; ++h) if (off[h + 1] < off[h] || off[h + 1] - off[h] > 0x7FFFFFF0LL) return fail("bad haplotype offsets");
+    int workers = n_threads > 0 ? n_threads : (int)std::thread::hardware_concurrency();
+    workers = std::max(1, std::min(workers, (int)std::min<int32_t>(n, 64)));
+    std::atomic<int32_t> next {0};
+    auto work = [&] {
+        std::vector<Run> runs;
+        std::vector<unsigned char> buf;
+        std::vector<std::int32_t> tmp;
+        for (;;) {
+            const int32_t h = next.fetch_add(1);
+            if (h >= n) break;
+            const int64_t o = off[h];
+            const std::uint32_t len = (std::uint32_t)(off[h + 1] - o);
+            std::int32_t* c = cell ? cell + o : (tmp.resize(len), tmp.data());
+            mutation_cells(*m, (const unsigned char*)seq + o, len, c, buf, runs);
+            for (std::uint32_t i = 0; i < len; ++i) {
+                if (open_penalty) open_penalty[o + i] = m->open_penalty[c[i]];
+                if (extend_penalty) extend_penalty[o + i] = m->extend_penalty[c[i]];
+            }
+        }
+    };
+    if (workers == 1) work();
+    else {
+        std::vector<std::thread> pool;
+        for (int w = 1; w < workers; ++w) pool.emplace_back(work);
+        work();
+        for (std::thread& t : pool) t.join();
+    }
+    return PHMM_OK;
 }
 
 } // extern "C"

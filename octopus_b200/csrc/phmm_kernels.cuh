@@ -1870,4 +1870,67 @@ __global__ void k_list_slots(const PopParams p, const bool init)
     }
 }
 
+// -------------------------------------------------------------------------------------------------------------
+// phmm_mutation_prime: DeNovoModel::prime (core/models/mutation/denovo_model.cpp:64-84, 269-293)
+// -------------------------------------------------------------------------------------------------------------
+// Mutation statuses (include/phmm_b200.h PHMM_MUT_*).
+constexpr int kMutHmm = 0, kMutSelf = 1, kMutApproxLength = 2, kMutApproxOffset = 3, kMutApproxOverflow = 4, kMutOutOfModel = 5;
+
+// One tile [lo, hi) of the ordered pairs t * H + g. The diagonal and the pairs whose length distance reaches the band
+// (can_try_align_with_hmm, :249-252) are settled here; every other pair is appended to list (as {target, given}) for the DP.
+__global__ void k_mutation_pairs(const long long lo, const long long hi, const int H, const long long* __restrict__ off,
+                                 double* __restrict__ out, int* __restrict__ status, int2* __restrict__ list, int* __restrict__ count)
+{
+    const long long step = (long long)gridDim.x * blockDim.x;
+    for (long long i = lo + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += step) {
+        const int t = (int)(i / H), g = (int)(i - (long long)t * H);
+        const long long lt = off[t + 1] - off[t], lg = off[g + 1] - off[g];
+        if (t == g) { out[i] = 0.0; status[i] = kMutSelf; continue; }
+        if ((lt > lg ? lt - lg : lg - lt) >= 32) { out[i] = 0.0; status[i] = kMutApproxLength; continue; }
+        list[atomicAdd(count, 1)] = make_int2(t, g);
+    }
+}
+
+// recalculate_log_probability (:199-218) of each listed pair's alignment, from the CIGAR text the traceback kernels wrote (runs
+// merged as make_cigar merges them, so each run's length is the reference's op.size()). pos counts given bases from the alignment
+// start (= given base 0 at target offset 32); '=', 'X' and 'D' advance it. Double arithmetic with explicit rounding so that no FMA
+// is contracted; the float logs come from the host table logp[cell][min(size, X) - 1].
+__global__ void k_mutation_rescore(const int n, const int2* __restrict__ list, const long long* __restrict__ target_offset,
+                                   const int* __restrict__ align_status, const char* __restrict__ cigar, const int cigar_stride,
+                                   const long long* __restrict__ off, const int* __restrict__ cell, const float* __restrict__ logp,
+                                   const int X, const double snv_log_prior, const int H, double* __restrict__ out, int* __restrict__ status)
+{
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const int2 tg = list[j];
+    const long long i = (long long)tg.x * H + tg.y;
+    if (align_status[j] != 0) { out[i] = 0.0; status[i] = align_status[j] == 4 ? kMutApproxOverflow : -1; return; }   // -1: CIGAR truncated
+    if (target_offset[j] != 32) { out[i] = 0.0; status[i] = kMutApproxOffset; return; }
+    const long long g0 = off[tg.y], glen = off[tg.y + 1] - g0;
+    const char* cg = cigar + (size_t)j * cigar_stride;
+    double result = 0.0;
+    long long pos = 0;
+    int st = kMutHmm;
+    unsigned size = 0;
+    for (int k = 0; k < cigar_stride; ++k) {
+        const char c = cg[k];
+        if (c == 0) break;
+        if (c >= '0' && c <= '9') { size = size * 10u + (unsigned)(c - '0'); continue; }
+        if (c == 'X') {
+            result = __dadd_rn(result, __dmul_rn((double)size, snv_log_prior));
+            pos += size;
+        } else if (c == 'I' || c == 'D') {
+            if (pos >= glen) { st = kMutOutOfModel; break; }
+            const int k1 = (int)min(size, (unsigned)X) - 1;
+            result = __dadd_rn(result, (double)logp[(size_t)cell[g0 + pos] * X + k1]);
+            if (c == 'D') pos += size;
+        } else {
+            pos += size;
+        }
+        size = 0;
+    }
+    out[i] = st == kMutHmm ? result : 0.0;
+    status[i] = st;
+}
+
 } // namespace phmm
