@@ -183,6 +183,10 @@ inline uint32_t fma_add(uint32_t a, uint32_t b, uint32_t one) { return a * one +
 //                               x-1, which continues in the unrolled sequence at x-2
 //   epilogue  x > L, x >= 2B    cells k >= x - L; leaves the unrolled sequence after the row-L cell
 //   general   x < 2B, x > L     (reads shorter than the band) both limits, per-cell predicates
+//
+// Around the cells a steady column runs 20 instructions (DESIGN.md §4): at its top the two next-column loads (unclamped, see
+// the loop) and one branch that tests both limits; at its end the carried column state (caps, go / ge, gop / gep) written in
+// place, the loop test and the back edge. No register is copied between columns.
 #define PHMM_REP8(F, b)  F(b + 7) F(b + 6) F(b + 5) F(b + 4) F(b + 3) F(b + 2) F(b + 1) F(b + 0)
 #define PHMM_REP64(F)    PHMM_REP8(F, 56) PHMM_REP8(F, 48) PHMM_REP8(F, 40) PHMM_REP8(F, 32) PHMM_REP8(F, 24) PHMM_REP8(F, 16) PHMM_REP8(F, 8) PHMM_REP8(F, 0)
 // 63 .. 0 as single tokens (for labels built with ##)
@@ -209,8 +213,17 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
 #pragma unroll
     for (int k = 0; k < K; ++k) { M[k] = 0u; D[k] = kInf16x2; }
     const int W = L + K - 1;
-    ColEntry e0 = ldg(t0), e1 = ldg(t1);
-    uint32_t go_prev = 0u, ge_prev = 0u;
+    // The column state carried from column to column: the caps of column x, gap_open[x] / gap_extend[x] (go, ge) and
+    // gap_open[x-1] + nuc_prior / gap_extend[x-1] + nuc_prior (gop, gep; the gap penalties left of column 0 are 0).
+    // All of it is written at the column's end, after the last cell has read the old values, so no register is copied.
+    uint32_t caps0, caps1, go, ge, gop = nucp, gep = nucp;
+    const uint32_t zero = one - 1u;
+    {
+        const ColEntry e0 = ldg(t0), e1 = ldg(t1);
+        caps0 = e0.x; caps1 = e1.x;
+        go = prmt(e0.y, e1.y, 0x3430u);   // gap_open[x]   of both halves (byte 3 of .y is the zero source)
+        ge = prmt(e0.y, e1.y, 0x3531u);   // gap_extend[x]
+    }
     const RowEntry w0 = rows[0];
 
     // Every use of the old m (the insertion's m + gop, the deletion's operands) comes before M[k] is written, so the old value is dead
@@ -232,30 +245,30 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
 #define PHMM_PRO_ENTRY(k)     case (k) + 1: if ((k) + 1 < K) { M[(k) < K ? (k) : 0] = M[K - 1]; PHMM_CELL(k) goto pro_##k; } goto pro_0;
 #define PHMM_PRO_CHAIN(k)     pro_##k: if ((k) >= 1 && (k) <= K) PHMM_CELL((k) >= 1 && (k) <= K ? (k) - 1 : 0)
     // epilogue: cell k, then, if it was the row-L cell, a jump to the column end through a block of its own (PHMM_DISTINCT_PATH)
-#define PHMM_EPI_CELL(k)      if ((k) >= 1 && (k) < K) { PHMM_CELL((k) < K ? (k) : 0) if ((k) == klo) { PHMM_DISTINCT_PATH(#k) goto column_end; } }
+// The epilogue columns x >= W-2 are the ones whose row-L cell is k >= 2B-3: their exits also step the next-column index back (below)
+#define PHMM_EPI_CELL(k)      if ((k) >= 1 && (k) < K) { PHMM_CELL((k) < K ? (k) : 0) if ((k) == klo) { if ((k) >= K - 3) --d; PHMM_DISTINCT_PATH(#k) goto column_end; } }
 
+    // The next column's entries are loaded at the top of every column, before the column picks its body, so that the loads
+    // issue early and the whole column hides their latency: column x loads entry x + d, d = 1. Entries past W - 1 are outside
+    // the window, so the last two columns must read entry W - 1 instead: the columns x >= W - 2 step d back by one, the
+    // epilogue's in the exit blocks of their row-L cells (k >= 2B-3), the general body of a read shorter than the band in the
+    // body. That keeps the index clamp off the steady columns and out of the epilogue's cells. Column W's entry is read only by
+    // its one cell, in the pad row, where every cap gives sub = 0.
+    int d = 1;
     for (int x = 0; x <= W; ++x) {
-        const int xn = (x + 1 < W) ? x + 1 : W - 1;
-        const ColEntry n0 = ldg(t0 + xn * CS), n1 = ldg(t1 + xn * CS);
-        const uint32_t caps0 = e0.x, caps1 = e1.x;
-        const uint32_t go = prmt(e0.y, e1.y, 0x3430u);   // gap_open[x]   of both halves (byte 3 of .y is the zero source)
-        const uint32_t ge = prmt(e0.y, e1.y, 0x3531u);   // gap_extend[x]
-        const uint32_t gop = go_prev + nucp;             // gap_open[x-1] + nuc_prior
-        const uint32_t gep = ge_prev + nucp;             // gap_extend[x-1] + nuc_prior
+        const ColEntry n0 = ldg(t0 + (x + d) * CS), n1 = ldg(t1 + (x + d) * CS);
         const RowEntry* rp = rows + x;
         uint32_t i_run = kInf16x2;
-        if (x >= K) {
-            if (x <= L) {
-                // steady state: every cell of the column exists
+        if (x >= K && x <= L) {
+            // steady state: every cell of the column exists. Both limits are tested with one branch.
 #pragma unroll
-                for (int k = K - 1; k >= 0; --k) PHMM_CELL(k)
-            } else {
-                // epilogue: rows beyond L do not exist; stop after the row-L cell (k = x - L >= 1) so that M[x-L] keeps S(x, L).
-                // Every exit leaves through a block of its own: when they all branch straight to the column end, ptxas puts the
-                // register copies each exit needs on the path that falls through to the next cell, where they run for every cell.
-                const int klo = x - L;
-                PHMM_DESC64(PHMM_EPI_CELL)
-            }
+            for (int k = K - 1; k >= 0; --k) PHMM_CELL(k)
+        } else if (x >= K) {
+            // epilogue: rows beyond L do not exist; stop after the row-L cell (k = x - L >= 1) so that M[x-L] keeps S(x, L).
+            // Every exit leaves through a block of its own: when they all branch straight to the column end, ptxas puts the
+            // register copies each exit needs on the path that falls through to the next cell, where they run for every cell.
+            const int klo = x - L;
+            PHMM_DESC64(PHMM_EPI_CELL)
         } else if (x <= L) {
             // prologue: cell (x, 0) has S = 0, so m(x+1, 1) = sub(x, 0), and i(x, 1) = gap_open[x-1] + nuc for odd x, +inf for even x;
             // cells k = x-1 .. 0 all exist. No cell reads M[2B-1] before column 2B, so it carries m(x+1, 1) to the next column's
@@ -266,6 +279,7 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
             M[K - 1] = vmin2(w0.y, prmt(caps0, caps1, w0.x));
         } else {
             // reads shorter than the band, L < x < 2B: both limits apply; the row-0 value travels in M[2B-1] as in the prologue
+            if (x >= W - 2) --d;
             i_run = (x & 1) ? gop : kInf16x2;
             const int klo = x - L;
 #pragma unroll
@@ -276,13 +290,16 @@ PHMM_HD uint32_t dp_pair(const RowEntry* __restrict__ rows, const int L,
             M[K - 1] = vmin2(w0.y, prmt(caps0, caps1, w0.x));
         }
     column_end:
-        go_prev = go; ge_prev = ge;
         // The next column's entries were loaded at the top of this column and must not be waited for before its end.
-        // Left to itself ptxas copies them into e0 / e1 right after issuing the loads (a full L2 round trip per column,
-        // 13 % of the kernel's stall samples in profiles/r01d). z is always 0 — no lane ever has its sign bit set — but
-        // it is only known once the column's last cell is done, which pins the copy behind the column body.
-        const uint32_t z = i_run & 0x80008000u;
-        e0.x = n0.x + z; e0.y = n0.y + z; e1.x = n1.x + z; e1.y = n1.y + z;
+        // Left to itself ptxas consumes them right after issuing the loads (a full L2 round trip per column, 13 % of the
+        // kernel's stall samples in profiles/r01d). Adding i_run * zero (0, but opaque to the compiler like `one`, and i_run
+        // only known once the column's last cell is done) pins everything derived from the entries behind the column body,
+        // at one IMAD each on the FMA pipe: the caps directly, go / ge through n1.y (each PRMT reads both words).
+        gop = go + nucp; gep = ge + nucp;
+        caps0 = fma_add(i_run, n0.x, zero); caps1 = fma_add(i_run, n1.x, zero);
+        const uint32_t y1 = fma_add(i_run, n1.y, zero);
+        go = prmt(n0.y, y1, 0x3430u);
+        ge = prmt(n0.y, y1, 0x3531u);
     }
 #undef PHMM_CELL
 #undef PHMM_PRO_ENTRY
