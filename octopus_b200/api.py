@@ -13,7 +13,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .batch import HaplotypeBlock, ReadBlock
+from .batch import HaplotypeBlock, ReadBlock, _ptr, _u8, concat_reads, pack_sequences
 
 
 class PhmmError(RuntimeError):
@@ -30,24 +30,156 @@ class TooLargeBandSizeError(PhmmError):
     """Requested band > 256 (simd_pair_hmm_wrapper.hpp:45-61)."""
 
 
+def _error(code, message):
+    """The exception for a failed call's PHMM_ERR_* code."""
+    cls = {_lib.PHMM_ERR_SHORT_HAPLOTYPE: ShortHaplotypeError, _lib.PHMM_ERR_BAND: TooLargeBandSizeError}.get(code, PhmmError)
+    return cls(code, message)
+
+
 def _is_torch(x):
     return hasattr(x, "data_ptr")
 
 
-class PairHMMEngine:
-    """One engine handle (not re-entrant; one per host thread, like the reference's per-thread model copies)."""
+class _Space:
+    """The memory space of one call: numpy arrays on the host, or torch tensors on one CUDA device."""
+    __slots__ = ("device", "on_device", "flag")
 
-    def __init__(self, device=-1):
+    def __init__(self, device=None):
+        self.device = device
+        self.on_device = device is not None
+        self.flag = _lib.SPACE_DEVICE if self.on_device else _lib.SPACE_HOST
+
+    @classmethod
+    def of(cls, haps, reads):
+        assert haps.on_device == reads.on_device, "haplotypes and reads must live in the same memory space"
+        return cls(haps.seq.device if haps.on_device else None)
+
+    def dtype(self, dtype):
+        if self.on_device:
+            import torch
+            return getattr(torch, np.dtype(dtype).name)
+        return np.dtype(dtype)
+
+    def empty(self, shape, dtype, zeroed=False):
+        """An output array; zeroed where the call may leave entries unwritten."""
+        if self.on_device:
+            import torch
+            return (torch.zeros if zeroed else torch.empty)(shape, dtype=self.dtype(dtype), device=self.device)
+        return (np.zeros if zeroed else np.empty)(shape, dtype=dtype)
+
+    def input(self, x, dtype):
+        """x (a sequence, numpy array or torch tensor) as a contiguous array of `dtype` in this space."""
+        if self.on_device:
+            import torch
+            t = x if _is_torch(x) else torch.as_tensor(np.ascontiguousarray(x, dtype=dtype), device=self.device)
+            return t.to(device=self.device, dtype=self.dtype(dtype)).contiguous()
+        return np.ascontiguousarray(x, dtype=dtype)
+
+    ptr = staticmethod(_ptr)        # the data pointer of a numpy array or torch tensor, or None
+
+
+_HOST = _Space()
+
+
+def _ref(s):
+    return None if s is None else C.byref(s)
+
+
+def _config(config):
+    """A HaplotypeLikelihoodModel.Config, or an already built _lib.Config, as the phmm_config argument."""
+    return C.byref(config.c_struct() if hasattr(config, "c_struct") else config)
+
+
+def _flank(flank_state):
+    """(lhs_flank, rhs_flank) → phmm_flank_state; None → None."""
+    return None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
+
+
+def _positions(space, positions):
+    """(off, pos) candidate positions → phmm_positions over arrays in the call's memory space (kept alive by the struct); None → None."""
+    if positions is None:
+        return None
+    off, pos = space.input(positions[0], np.int64), space.input(positions[1], np.int32)
+    s = _lib.Positions(space.ptr(off), space.ptr(pos))
+    s.arrays = off, pos
+    return s
+
+
+def _regions(hap_first, read_first, flank_states=None):
+    """Group bounds (and per-group flank states or None) → (phmm_regions, int64 offsets of the groups' [H_g, R_g] blocks in the flat
+    result, whose last entry is its size)."""
+    hf = np.ascontiguousarray(hap_first, dtype=np.int32)
+    rf = np.ascontiguousarray(read_first, dtype=np.int32)
+    G = len(hf) - 1
+    sizes = np.diff(hf).astype(np.int64) * np.diff(rf).astype(np.int64)
+    off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    fl = None
+    if flank_states is not None:
+        fl = (_lib.FlankState * G)()
+        for g, f in enumerate(flank_states):
+            if f is not None:
+                fl[g] = _flank(f)
+    regs = _lib.Regions(G, hf.ctypes.data, rf.ctypes.data, C.addressof(fl) if fl is not None else None)
+    regs.arrays = hf, rf, fl
+    return regs, off
+
+
+class _Alignments:
+    """The outputs of n alignments: mapping position, likelihood, CIGAR text (n x stride bytes, NUL-terminated) and status, zeroed."""
+
+    def __init__(self, space, reads, n, stride=None):
+        self.n = n
+        self.stride = 4 * int((reads.off[1:] - reads.off[:-1]).max()) + 64 if stride is None else stride
+        self.mp, self.lk, self.st = space.empty(n, np.int64, True), space.empty(n, np.float64, True), space.empty(n, np.int32, True)
+        self.cg = space.empty(n * self.stride, np.uint8, True)
+
+    def pointers(self):
+        """The (mapping_position, likelihood, cigar, cigar_stride, status) arguments of the aligning calls."""
+        return _ptr(self.mp), _ptr(self.lk), _ptr(self.cg), self.stride, _ptr(self.st)
+
+    def result(self):
+        text = bytes(self.cg.cpu().numpy() if _is_torch(self.cg) else self.cg)
+        s = self.stride
+        return self.mp, self.lk, [text[j * s:(j + 1) * s].split(b"\0", 1)[0].decode() for j in range(self.n)], self.st
+
+
+def _grow(attempt, cap):
+    """attempt(cap) → (size needed, result). Most calls fit the first guess; a second call takes the exact size."""
+    while True:
+        total, result = attempt(cap)
+        if total <= cap:
+            return result
+        cap = total
+
+
+class _Handle:
+    """A library handle this object owns: freed by close(), at the end of a with block, or when the object is collected."""
+    _h = None
+    _destroy = None             # the phmm_*_destroy function's name
+
+    def _create(self, create, *args):
         self._lib = _lib.load()
         h = C.c_void_p()
-        rc = self._lib.phmm_create(C.byref(h), int(device))
+        rc = getattr(self._lib, create)(C.byref(h), *args)
         if rc != _lib.PHMM_OK:
-            raise PhmmError(rc, self._lib.phmm_last_error(None).decode())
+            raise PhmmError(rc, self._last_error())
         self._h = h
 
+    def _last_error(self):
+        raise NotImplementedError
+
+    def _raise(self, rc):
+        """Raise the exception for a failed call's code, with this handle's last error message."""
+        raise _error(rc, self._last_error())
+
+    def _check(self, rc, tolerate_short=False):
+        """Raise for a failed call. With tolerate_short (the caller asked for statuses) a short haplotype is no failure."""
+        if rc != _lib.PHMM_OK and not (tolerate_short and rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE):
+            self._raise(rc)
+
     def close(self):
-        if getattr(self, "_h", None):
-            self._lib.phmm_destroy(self._h)
+        if self._h:
+            getattr(self._lib, self._destroy)(self._h)
             self._h = None
 
     def __del__(self):
@@ -62,28 +194,27 @@ class PairHMMEngine:
     def __exit__(self, *a):
         self.close()
 
-    def _raise(self, rc):
-        msg = self._lib.phmm_last_error(self._h).decode()
-        if rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE:
-            raise ShortHaplotypeError(rc, msg)
-        if rc == _lib.PHMM_ERR_BAND:
-            raise TooLargeBandSizeError(rc, msg)
-        raise PhmmError(rc, msg)
+
+class PairHMMEngine(_Handle):
+    """One engine handle (not re-entrant; one per host thread, like the reference's per-thread model copies)."""
+    _destroy = "phmm_destroy"
+
+    def __init__(self, device=-1):
+        self._create("phmm_create", int(device))
+
+    def _last_error(self):
+        return self._lib.phmm_last_error(self._h).decode()
 
     # -- stream ordering -----------------------------------------------------------------------------------------
     def wait_event(self, event):
         """Make the engine's stream wait (on the device) for a CUDA event — a torch.cuda.Event or a raw cudaEvent_t — recorded
         after work on another stream that still reads a buffer the next call will overwrite (phmm_wait_event)."""
         handle = getattr(event, "cuda_event", event)
-        rc = self._lib.phmm_wait_event(self._h, C.c_void_p(int(handle)))
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
+        self._check(self._lib.phmm_wait_event(self._h, C.c_void_p(int(handle))))
 
     def reserve_sms(self, n):
         """Keep the first n SMs free of persistent DP blocks, for a collective running beside the next call (phmm_reserve_sms)."""
-        rc = self._lib.phmm_reserve_sms(self._h, int(n))
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
+        self._check(self._lib.phmm_reserve_sms(self._h, int(n)))
 
     def stream_handle(self):
         return int(self._lib.phmm_engine_stream(self._h) or 0)
@@ -103,50 +234,32 @@ class PairHMMEngine:
         """DeNovoModel::prime + evaluate for one haplotype set (phmm_mutation_prime): sequences (list of str / bytes) → (out, status),
         both [H, H] indexed [target, given]. out[t, g] = ln p(target | given) where status is MUT_HMM or MUT_SELF; the MUT_APPROX_*
         pairs need the reference's approximate path (Haplotype::difference) and MUT_OUT_OF_MODEL pairs have no defined value."""
-        off, seq = _pack_sequences(sequences)
+        off, seq = pack_sequences(sequences)
         H = len(off) - 1
         out = np.zeros((H, H), dtype=np.float64)
         status = np.zeros((H, H), dtype=np.int32)
-        rc = self._lib.phmm_mutation_prime(self._h, model._h, H, off.ctypes.data, seq.ctypes.data, out.ctypes.data, status.ctypes.data)
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
+        self._check(self._lib.phmm_mutation_prime(self._h, model._h, H, off.ctypes.data, seq.ctypes.data, out.ctypes.data,
+                                                  status.ctypes.data))
         return out, status
 
     # -- raw kernel boundary -----------------------------------------------------------------------------------
     def align_scores(self, band, haps: HaplotypeBlock, reads: ReadBlock, tasks, nuc_prior=2, precision_bits=16):
         """tasks: (n, 4) int32 rows (read, hap, win_off, reverse). Returns the integer score of every task, i.e.
         reference ``hmm.align(hap_window, read, quals, L+2*band-1, L, snv_mask, snv_prior, gap_open, gap_extend, nuc_prior)``."""
-        dev = haps.on_device
-        assert dev == reads.on_device, "haplotypes and reads must live in the same memory space"
-        hs, rs = haps.c_struct(), reads.c_struct()
-        if dev:
-            import torch
-            t = tasks if _is_torch(tasks) else torch.as_tensor(np.ascontiguousarray(tasks, dtype=np.int32), device=haps.seq.device)
-            t = t.to(torch.int32).contiguous()
-            n = t.shape[0]
-            out = torch.empty(n, dtype=torch.int32, device=t.device)
-            tp, op = t.data_ptr(), out.data_ptr()
-        else:
-            t = np.ascontiguousarray(tasks, dtype=np.int32).reshape(-1, 4)
-            n = t.shape[0]
-            out = np.empty(n, dtype=np.int32)
-            tp, op = t.ctypes.data, out.ctypes.data
-        rc = self._lib.phmm_align_scores(self._h, int(band), int(precision_bits), int(nuc_prior), C.byref(hs), C.byref(rs),
-                                         tp, n, op, _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
+        sp = _Space.of(haps, reads)
+        t = sp.input(tasks, np.int32)
+        if not sp.on_device:
+            t = t.reshape(-1, 4)
+        n = t.shape[0]
+        out = sp.empty(n, np.int32)
+        self._check(self._lib.phmm_align_scores(self._h, int(band), int(precision_bits), int(nuc_prior), C.byref(haps.c_struct()),
+                                                C.byref(reads.c_struct()), sp.ptr(t), n, sp.ptr(out), sp.flag))
         return out
 
     def align(self, band, truth, target, quals, gap_open, gap_extend, nuc_prior=2, snv_mask=None, snv_prior=None):
         """Per-call seam with traceback ↔ simd::PairHMM::align(..., first_pos, align1, align2) (simd_pair_hmm.hpp:472-509).
         Returns (score, first_pos, aligned_truth, aligned_target). gap_extend may be a scalar (the reference's scalar overload)."""
-        def as_bytes(x):
-            if isinstance(x, str):
-                return x.encode()
-            if isinstance(x, (bytes, bytearray)):
-                return bytes(x)
-            return np.ascontiguousarray(np.asarray(x)).view(np.uint8).tobytes()
-        t, r = as_bytes(truth), as_bytes(target)
+        t, r = _u8(truth).tobytes(), _u8(target).tobytes()
         q = np.ascontiguousarray(np.asarray(quals, dtype=np.int8))
         go = np.ascontiguousarray(np.asarray(gap_open, dtype=np.int8))
         if np.ndim(gap_extend) == 0:
@@ -154,17 +267,15 @@ class PairHMMEngine:
         else:
             ge = np.ascontiguousarray(np.asarray(gap_extend, dtype=np.int8)); gep, ges = ge.ctypes.data, 0
         if snv_mask is not None:
-            m = as_bytes(snv_mask)
+            m = _u8(snv_mask).tobytes()
             sp = np.ascontiguousarray(np.asarray(snv_prior, dtype=np.int8)); spp = sp.ctypes.data
         else:
             m, spp = None, None
         n = 2 * (len(r) + band) + 1
         a1, a2 = C.create_string_buffer(n + 8), C.create_string_buffer(n + 8)
         score, fp = C.c_int(0), C.c_int(0)
-        rc = self._lib.phmm_align_traceback(self._h, int(band), t, r, q.ctypes.data, len(t), len(r), m, spp, go.ctypes.data, gep, ges,
-                                            int(nuc_prior), C.byref(score), C.byref(fp), a1, a2)
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
+        self._check(self._lib.phmm_align_traceback(self._h, int(band), t, r, q.ctypes.data, len(t), len(r), m, spp, go.ctypes.data, gep, ges,
+                                                   int(nuc_prior), C.byref(score), C.byref(fp), a1, a2))
         return score.value, fp.value, a1.value.decode(), a2.value.decode()
 
     def align_reads(self, config, haps: HaplotypeBlock, reads: ReadBlock, pairs, positions=None, flank_state=None, cigar_stride=None):
@@ -173,27 +284,11 @@ class PairHMMEngine:
         assert not haps.on_device and not reads.on_device
         pr = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
         n = pr.shape[0]
-        hs, rs = haps.c_struct(), reads.c_struct()
-        cfg = config.c_struct()
-        if cigar_stride is None:
-            cigar_stride = 4 * int(np.diff(reads.off).max()) + 64
-        pstruct = None
-        if positions is not None:
-            off = np.ascontiguousarray(positions[0], dtype=np.int64)
-            pos = np.ascontiguousarray(positions[1], dtype=np.int32)
-            pstruct = _lib.Positions(off.ctypes.data, pos.ctypes.data)
-        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
-        mp = np.zeros(n, dtype=np.int64)
-        lk = np.zeros(n, dtype=np.float64)
-        st = np.zeros(n, dtype=np.int32)
-        cg = np.zeros(n * cigar_stride, dtype=np.uint8)
-        rc = self._lib.phmm_align_reads(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), pr.ctypes.data, n,
-                                        C.byref(pstruct) if pstruct is not None else None, C.byref(fstruct) if fstruct is not None else None,
-                                        mp.ctypes.data, lk.ctypes.data, cg.ctypes.data, cigar_stride, st.ctypes.data, _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
-        cigars = [bytes(cg[j * cigar_stride:(j + 1) * cigar_stride]).split(b"\0", 1)[0].decode() for j in range(n)]
-        return mp, lk, cigars, st
+        res = _Alignments(_HOST, reads, n, cigar_stride)
+        self._check(self._lib.phmm_align_reads(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), pr.ctypes.data,
+                                               n, _ref(_positions(_HOST, positions)), _ref(_flank(flank_state)), *res.pointers(),
+                                               _lib.SPACE_HOST))
+        return res.result()
 
     def align_pairs(self, config, truths: HaplotypeBlock, targets: ReadBlock, pairs, target_offsets, flank_state=None, cigar_stride=None):
         """hmm::align batched (phmm_align_pairs): pair j = (target pairs[j][0], truth pairs[j][1]) at target_offsets[j]. Host blocks.
@@ -203,111 +298,49 @@ class PairHMMEngine:
         n = pr.shape[0]
         offs = np.ascontiguousarray(target_offsets, dtype=np.int32)
         assert len(offs) == n
-        hs, rs, cfg = truths.c_struct(), targets.c_struct(), config.c_struct()
-        if cigar_stride is None:
-            cigar_stride = 4 * int(np.diff(targets.off).max()) + 64
-        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
-        mp, lk, st = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=np.float64), np.zeros(n, dtype=np.int32)
-        cg = np.zeros(n * cigar_stride, dtype=np.uint8)
-        rc = self._lib.phmm_align_pairs(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), pr.ctypes.data, offs.ctypes.data, n,
-                                        C.byref(fstruct) if fstruct is not None else None,
-                                        mp.ctypes.data, lk.ctypes.data, cg.ctypes.data, cigar_stride, st.ctypes.data, _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
-        cigars = [bytes(cg[j * cigar_stride:(j + 1) * cigar_stride]).split(b"\0", 1)[0].decode() for j in range(n)]
-        return mp, lk, cigars, st
-
-    @staticmethod
-    def _pairs_arg(pairs, dev, device):
-        if dev:
-            import torch
-            t = pairs if _is_torch(pairs) else torch.as_tensor(np.ascontiguousarray(pairs, dtype=np.int32), device=device)
-            t = t.to(device=device, dtype=torch.int32).reshape(-1, 2).contiguous()
-            return t, t.shape[0], t.data_ptr()
-        a = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
-        return a, a.shape[0], a.ctypes.data
+        res = _Alignments(_HOST, targets, n, cigar_stride)
+        self._check(self._lib.phmm_align_pairs(self._h, _config(config), C.byref(truths.c_struct()), C.byref(targets.c_struct()),
+                                               pr.ctypes.data, offs.ctypes.data, n, _ref(_flank(flank_state)), *res.pointers(),
+                                               _lib.SPACE_HOST))
+        return res.result()
 
     def map_pairs(self, haps: HaplotypeBlock, reads: ReadBlock, pairs):
         """map_query_to_target(read, haplotype) uncapped, K = 6, for explicit (read, haplotype) pairs (phmm_map_pairs): every mapping
         begin at the pair's largest k-mer vote count, ascending — what ReadRealigner maps with. Returns the CSR (off[n+1] int64,
         pos int32) over the pair list: numpy for host blocks, torch CUDA tensors for device-resident ones."""
-        dev = haps.on_device
-        assert dev == reads.on_device, "haplotypes and reads must live in the same memory space"
-        device = haps.seq.device if dev else None
-        pr, n, pp = self._pairs_arg(pairs, dev, device)
-        hs, rs = haps.c_struct(), reads.c_struct()
-        space = _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST
-        cap = 4 * n + 16                # most pairs have one or a few maxima; a second call takes the exact size
-        while True:
-            if dev:
-                import torch
-                off = torch.empty(n + 1, dtype=torch.int64, device=device)
-                pos = torch.empty(cap, dtype=torch.int32, device=device)
-                op, posp = off.data_ptr(), pos.data_ptr()
-            else:
-                off = np.empty(n + 1, dtype=np.int64)
-                pos = np.empty(cap, dtype=np.int32)
-                op, posp = off.ctypes.data, pos.ctypes.data
-            rc = self._lib.phmm_map_pairs(self._h, C.byref(hs), C.byref(rs), pp, n, op, posp, cap, space)
-            if rc != _lib.PHMM_OK:
-                self._raise(rc)
+        sp = _Space.of(haps, reads)
+        pr = sp.input(pairs, np.int32).reshape(-1, 2)
+        n = pr.shape[0]
+        hs, rs = C.byref(haps.c_struct()), C.byref(reads.c_struct())
+
+        def attempt(cap):
+            off, pos = sp.empty(n + 1, np.int64), sp.empty(cap, np.int32)
+            self._check(self._lib.phmm_map_pairs(self._h, hs, rs, sp.ptr(pr), n, sp.ptr(off), sp.ptr(pos), cap, sp.flag))
             total = int(off[-1])
-            if total <= cap:
-                return off, pos[:total]
-            cap = total
+            return total, (off, pos[:total])
+        return _grow(attempt, 4 * n + 16)       # most pairs have one or a few maxima
 
     def realign_reads(self, config, haps: HaplotypeBlock, reads: ReadBlock, pairs, flank_state=None, cigar_stride=None):
         """ReadRealigner::realign for explicit (read, haplotype) pairs (phmm_realign_reads): HaplotypeLikelihoodModel::align at the
         positions of the uncapped k-mer mapper (map_pairs), mapped on the device (config.map_positions = False: the original position
         only). pairs: (n, 2) int32 rows (read, hap). Returns (mapping_position[n], likelihood[n], cigars[list of str], status[n]) as
         align_reads; for device-resident blocks the three arrays are torch CUDA tensors."""
-        dev = haps.on_device
-        assert dev == reads.on_device, "haplotypes and reads must live in the same memory space"
-        device = haps.seq.device if dev else None
-        pr, n, pp = self._pairs_arg(pairs, dev, device)
-        hs, rs, cfg = haps.c_struct(), reads.c_struct(), config.c_struct()
-        if cigar_stride is None:
-            lens = (reads.off[1:] - reads.off[:-1]).max()
-            cigar_stride = 4 * int(lens) + 64
-        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
-        if dev:
-            import torch
-            mp = torch.zeros(n, dtype=torch.int64, device=device)
-            lk = torch.zeros(n, dtype=torch.float64, device=device)
-            st = torch.zeros(n, dtype=torch.int32, device=device)
-            cg = torch.zeros(n * cigar_stride, dtype=torch.uint8, device=device)
-            ptrs = (mp.data_ptr(), lk.data_ptr(), cg.data_ptr(), st.data_ptr())
-        else:
-            mp, lk, st = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=np.float64), np.zeros(n, dtype=np.int32)
-            cg = np.zeros(n * cigar_stride, dtype=np.uint8)
-            ptrs = (mp.ctypes.data, lk.ctypes.data, cg.ctypes.data, st.ctypes.data)
-        rc = self._lib.phmm_realign_reads(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), pp, n,
-                                          C.byref(fstruct) if fstruct is not None else None, ptrs[0], ptrs[1], ptrs[2], cigar_stride, ptrs[3],
-                                          _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
-        text = bytes(cg.cpu().numpy() if dev else cg)
-        cigars = [text[j * cigar_stride:(j + 1) * cigar_stride].split(b"\0", 1)[0].decode() for j in range(n)]
-        return mp, lk, cigars, st
+        sp = _Space.of(haps, reads)
+        pr = sp.input(pairs, np.int32).reshape(-1, 2)
+        n = pr.shape[0]
+        res = _Alignments(sp, reads, n, cigar_stride)
+        self._check(self._lib.phmm_realign_reads(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), sp.ptr(pr),
+                                                 n, _ref(_flank(flank_state)), *res.pointers(), sp.flag))
+        return res.result()
 
     def genotype_likelihoods(self, lnl, genotypes):
         """ConstantMixtureGenotypeLikelihoodModel::evaluate for every row of `genotypes` ((G, ploidy) haplotype indices) over the
         (H, R) matrix `lnl` (numpy on the host, or a torch CUDA tensor left where populate produced it). Returns G doubles."""
-        if _is_torch(lnl):
-            import torch
-            m = lnl.contiguous()
-            gt = torch.as_tensor(np.ascontiguousarray(genotypes, dtype=np.int32), device=m.device)
-            out = torch.empty(gt.shape[0], dtype=torch.float64, device=m.device)
-            rc = self._lib.phmm_genotype_likelihoods(self._h, m.data_ptr(), m.shape[0], m.shape[1], gt.data_ptr(), gt.shape[0], gt.shape[1],
-                                                     out.data_ptr(), _lib.SPACE_DEVICE)
-        else:
-            m = np.ascontiguousarray(lnl, dtype=np.float64)
-            gt = np.ascontiguousarray(genotypes, dtype=np.int32)
-            out = np.empty(gt.shape[0], dtype=np.float64)
-            rc = self._lib.phmm_genotype_likelihoods(self._h, m.ctypes.data, m.shape[0], m.shape[1], gt.ctypes.data, gt.shape[0], gt.shape[1],
-                                                     out.ctypes.data, _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
+        sp = _Space(lnl.device if _is_torch(lnl) else None)
+        m, gt = sp.input(lnl, np.float64), sp.input(genotypes, np.int32)
+        out = sp.empty(gt.shape[0], np.float64)
+        self._check(self._lib.phmm_genotype_likelihoods(self._h, sp.ptr(m), m.shape[0], m.shape[1], sp.ptr(gt), gt.shape[0], gt.shape[1],
+                                                        sp.ptr(out), sp.flag))
         return out
 
     # -- batch boundary ----------------------------------------------------------------------------------------
@@ -317,54 +350,24 @@ class PairHMMEngine:
         assert not haps.on_device and not reads.on_device
         toff = np.ascontiguousarray(template_off, dtype=np.int64)
         T = len(toff) - 1
-        hs, rs, cfg = haps.c_struct(), reads.c_struct(), config.c_struct()
-        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
         out = np.empty((haps.n, T), dtype=np.float64)
-        rc = self._lib.phmm_populate_templates(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), toff.ctypes.data, T, None,
-                                               C.byref(fstruct) if fstruct is not None else None, out.ctypes.data, None, _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK:
-            self._raise(rc)
+        self._check(self._lib.phmm_populate_templates(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()),
+                                                      toff.ctypes.data, T, None, _ref(_flank(flank_state)), out.ctypes.data, None,
+                                                      _lib.SPACE_HOST))
         return out
 
     def populate_regions(self, config, haps: HaplotypeBlock, reads: ReadBlock, hap_first, read_first, flank_states=None, out=None, want_status=False):
         """Many regions in one call (phmm_populate_regions): region g owns haplotypes [hap_first[g], hap_first[g+1]) and reads
         [read_first[g], read_first[g+1]). Returns the flat result vector (the regions' [H_g, R_g] matrices back to back) and the
         per-region offsets into it; ``split_regions`` cuts it into matrices. flank_states: None or a list of (lhs, rhs) / None."""
-        dev = haps.on_device
-        assert dev == reads.on_device
-        hf = np.ascontiguousarray(hap_first, dtype=np.int32)
-        rf = np.ascontiguousarray(read_first, dtype=np.int32)
-        G = len(hf) - 1
-        sizes = (np.diff(hf).astype(np.int64) * np.diff(rf).astype(np.int64))
-        off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        sp = _Space.of(haps, reads)
+        regs, off = _regions(hap_first, read_first, flank_states)
         total = int(off[-1])
-        fl = None
-        if flank_states is not None:
-            fl = (_lib.FlankState * G)()
-            for g, f in enumerate(flank_states):
-                if f is not None:
-                    fl[g] = _lib.FlankState(1, int(f[0]), int(f[1]))
-        regs = _lib.Regions(G, hf.ctypes.data, rf.ctypes.data, C.addressof(fl) if fl is not None else None)
-        hs, rs = haps.c_struct(), reads.c_struct()
-        cfg = config.c_struct() if hasattr(config, "c_struct") else config
-        status = None
-        if dev:
-            import torch
-            if out is None:
-                out = torch.empty(total, dtype=torch.float64, device=haps.seq.device)
-            if want_status:
-                status = torch.empty(total, dtype=torch.int32, device=haps.seq.device)
-            op, sp = out.data_ptr(), (status.data_ptr() if want_status else None)
-        else:
-            if out is None:
-                out = np.empty(total, dtype=np.float64)
-            if want_status:
-                status = np.empty(total, dtype=np.int32)
-            op, sp = out.ctypes.data, (status.ctypes.data if want_status else None)
-        rc = self._lib.phmm_populate_regions(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), C.byref(regs), op, sp,
-                                             _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
-            self._raise(rc)
+        if out is None:
+            out = sp.empty(total, np.float64)
+        status = sp.empty(total, np.int32) if want_status else None
+        self._check(self._lib.phmm_populate_regions(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()),
+                                                    C.byref(regs), sp.ptr(out), sp.ptr(status), sp.flag), want_status)
         return (out, off, status) if want_status else (out, off)
 
     def assign_reads(self, config, haps: HaplotypeBlock, reads: ReadBlock, hap_first, read_first, log_priors=None, want_likelihoods=False,
@@ -377,43 +380,17 @@ class PairHMMEngine:
         vector (the groups' [H_g, R_g] matrices back to back, as populate_regions) when want_likelihoods and the per-pair statuses when
         want_status: numpy for host blocks, torch CUDA tensors for device-resident ones (top then as int64 with the same bits). With want_status a short haplotype does not
         raise; its statuses carry the extension and top is unspecified."""
-        dev = haps.on_device
-        assert dev == reads.on_device, "haplotypes and reads must live in the same memory space"
-        hf = np.ascontiguousarray(hap_first, dtype=np.int32)
-        rf = np.ascontiguousarray(read_first, dtype=np.int32)
-        G = len(hf) - 1
-        total = int((np.diff(hf).astype(np.int64) * np.diff(rf).astype(np.int64)).sum())
-        regs = _lib.Regions(G, hf.ctypes.data, rf.ctypes.data, None)
-        hs, rs = haps.c_struct(), reads.c_struct()
-        cfg = config.c_struct() if hasattr(config, "c_struct") else config
-        lnl = status = pri = None
-        if dev:
-            import torch
-            device = haps.seq.device
-            top = torch.empty(reads.n, dtype=torch.int64, device=device)
-            if want_likelihoods:
-                lnl = torch.empty(total, dtype=torch.float64, device=device)
-            if want_status:
-                status = torch.empty(total, dtype=torch.int32, device=device)
-            if log_priors is not None:
-                pri = (log_priors if _is_torch(log_priors) else torch.as_tensor(np.asarray(log_priors, dtype=np.float64)))
-                pri = pri.to(device=device, dtype=torch.float64).contiguous()
-            ptr = lambda x: None if x is None else x.data_ptr()
-        else:
-            top = np.empty(reads.n, dtype=np.uint64)
-            if want_likelihoods:
-                lnl = np.empty(total, dtype=np.float64)
-            if want_status:
-                status = np.empty(total, dtype=np.int32)
-            if log_priors is not None:
-                pri = np.ascontiguousarray(log_priors, dtype=np.float64)
-            ptr = lambda x: None if x is None else x.ctypes.data
+        sp = _Space.of(haps, reads)
+        regs, off = _regions(hap_first, read_first)
+        total = int(off[-1])
+        top = sp.empty(reads.n, np.int64 if sp.on_device else np.uint64)
+        lnl = sp.empty(total, np.float64) if want_likelihoods else None
+        status = sp.empty(total, np.int32) if want_status else None
+        pri = None if log_priors is None else sp.input(log_priors, np.float64)
         if pri is not None and pri.shape[0] != haps.n:
             raise ValueError("log_priors needs one value per haplotype of the block")
-        rc = self._lib.phmm_assign_reads(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), C.byref(regs), ptr(pri), ptr(top), ptr(lnl),
-                                         ptr(status), _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
-            self._raise(rc)
+        self._check(self._lib.phmm_assign_reads(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), C.byref(regs),
+                                                sp.ptr(pri), sp.ptr(top), sp.ptr(lnl), sp.ptr(status), sp.flag), want_status)
         out = (top,)
         if want_likelihoods:
             out += (lnl,)
@@ -431,103 +408,38 @@ class PairHMMEngine:
                  want_status=False):
         """Returns the (H, R) matrix of ln-likelihoods (numpy float64, or a torch CUDA tensor for device-resident blocks).
         positions: None or (off[H*R+1] int64, pos int32) CSR in [H][R] order. flank_state: None or (lhs_flank, rhs_flank)."""
-        dev = haps.on_device
-        assert dev == reads.on_device, "haplotypes and reads must live in the same memory space"
+        sp = _Space.of(haps, reads)
         H, R = haps.n, reads.n
-        hs, rs = haps.c_struct(), reads.c_struct()
-        cfg = config.c_struct() if hasattr(config, "c_struct") else config
-        keep = []
-        pstruct = None
-        if positions is not None:
-            off, pos = positions
-            if dev:
-                import torch
-                off = off if _is_torch(off) else torch.as_tensor(np.ascontiguousarray(off, dtype=np.int64), device=haps.seq.device)
-                pos = pos if _is_torch(pos) else torch.as_tensor(np.ascontiguousarray(pos, dtype=np.int32), device=haps.seq.device)
-                pstruct = _lib.Positions(off.data_ptr(), pos.data_ptr())
-            else:
-                off = np.ascontiguousarray(off, dtype=np.int64)
-                pos = np.ascontiguousarray(pos, dtype=np.int32)
-                pstruct = _lib.Positions(off.ctypes.data, pos.ctypes.data)
-            keep += [off, pos]
-        fstruct = None
-        if flank_state is not None:
-            fstruct = _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
-        status = None
-        if dev:
-            import torch
-            if out is None:
-                out = torch.empty((H, R), dtype=torch.float64, device=haps.seq.device)
-            if want_status:
-                status = torch.empty((H, R), dtype=torch.int32, device=haps.seq.device)
-            op, sp = out.data_ptr(), (status.data_ptr() if want_status else None)
-            if tuple(out.shape) != (H, R) or out.dtype != torch.float64 or (R > 1 and out.stride(1) != 1):
-                raise ValueError("out must be a float64 [H, R] tensor with unit column stride")
-            if H > 1 and out.stride(0) != R:
-                # a column window of a wider matrix — possibly another GPU's (octopus_b200.peer): phmm_populate_ld
-                rc = self._lib.phmm_populate_ld(self._h, C.byref(cfg), C.byref(hs), C.byref(rs),
-                                                C.byref(pstruct) if pstruct is not None else None,
-                                                C.byref(fstruct) if fstruct is not None else None, op, int(out.stride(0)), sp)
-                if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
-                    self._raise(rc)
-                return (out, status) if want_status else out
+        args = (self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), _ref(_positions(sp, positions)),
+                _ref(_flank(flank_state)))
+        if out is None:
+            out = sp.empty((H, R), np.float64)
+        status = sp.empty((H, R), np.int32) if want_status else None
+        if sp.on_device and (tuple(out.shape) != (H, R) or out.dtype != sp.dtype(np.float64) or (R > 1 and out.stride(1) != 1)):
+            raise ValueError("out must be a float64 [H, R] tensor with unit column stride")
+        if sp.on_device and H > 1 and out.stride(0) != R:
+            # a column window of a wider matrix — possibly another GPU's (octopus_b200.peer): phmm_populate_ld
+            rc = self._lib.phmm_populate_ld(*args, sp.ptr(out), int(out.stride(0)), sp.ptr(status))
         else:
-            if out is None:
-                out = np.empty((H, R), dtype=np.float64)
-            if want_status:
-                status = np.empty((H, R), dtype=np.int32)
-            op, sp = out.ctypes.data, (status.ctypes.data if want_status else None)
-        rc = self._lib.phmm_populate(self._h, C.byref(cfg), C.byref(hs), C.byref(rs),
-                                     C.byref(pstruct) if pstruct is not None else None,
-                                     C.byref(fstruct) if fstruct is not None else None,
-                                     op, sp, _lib.SPACE_DEVICE if dev else _lib.SPACE_HOST)
-        if rc != _lib.PHMM_OK:
-            if rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status:
-                return out, status
-            self._raise(rc)
+            rc = self._lib.phmm_populate(*args, sp.ptr(out), sp.ptr(status), sp.flag)
+        self._check(rc, want_status)
         return (out, status) if want_status else out
 
 
-class PopulateBatcher:
+class PopulateBatcher(_Handle):
     """One engine shared by many host threads (phmm_batcher_*): the populate requests that concurrent threads have in flight run
     as one multi-region kernel chain. Calls are thread-safe and block; ctypes releases the GIL during them, so Python threads
     really do wait together. Each result equals what ``PairHMMEngine.populate`` returns for the request alone. Host blocks only."""
+    _destroy = "phmm_batcher_destroy"
 
     def __init__(self, device=-1, clients=0, max_wait_us=None):
-        self._lib = _lib.load()
-        h = C.c_void_p()
         opt = None
         if clients or max_wait_us is not None:
             opt = _lib.BatcherOptions(int(clients), 500 if max_wait_us is None else int(max_wait_us))
-        rc = self._lib.phmm_batcher_create(C.byref(h), int(device), C.byref(opt) if opt is not None else None)
-        if rc != _lib.PHMM_OK:
-            raise PhmmError(rc, self._lib.phmm_batcher_last_error().decode())
-        self._h = h
+        self._create("phmm_batcher_create", int(device), _ref(opt))
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.phmm_batcher_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
-
-    def _raise(self, rc):
-        msg = self._lib.phmm_batcher_last_error().decode()      # this thread's last failing request
-        if rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE:
-            raise ShortHaplotypeError(rc, msg)
-        if rc == _lib.PHMM_ERR_BAND:
-            raise TooLargeBandSizeError(rc, msg)
-        raise PhmmError(rc, msg)
+    def _last_error(self):
+        return self._lib.phmm_batcher_last_error().decode()      # this thread's last failing request
 
     def stats(self):
         """Counters since creation: requests, gpu_calls, merged_calls, max_regions_per_call, dp_cells."""
@@ -541,23 +453,11 @@ class PopulateBatcher:
         """As PairHMMEngine.populate for host blocks: the (H, R) matrix (and the status matrix with want_status)."""
         assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
         H, R = haps.n, reads.n
-        hs, rs = haps.c_struct(), reads.c_struct()
-        cfg = config.c_struct() if hasattr(config, "c_struct") else config
-        pstruct, keep = None, []
-        if positions is not None:
-            off = np.ascontiguousarray(positions[0], dtype=np.int64)
-            pos = np.ascontiguousarray(positions[1], dtype=np.int32)
-            pstruct = _lib.Positions(off.ctypes.data, pos.ctypes.data)
-            keep += [off, pos]
-        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
-        out = np.empty((H, R), dtype=np.float64)
-        status = np.empty((H, R), dtype=np.int32) if want_status else None
-        rc = self._lib.phmm_batcher_populate(self._h, C.byref(cfg), C.byref(hs), C.byref(rs),
-                                             C.byref(pstruct) if pstruct is not None else None,
-                                             C.byref(fstruct) if fstruct is not None else None,
-                                             out.ctypes.data, status.ctypes.data if want_status else None)
-        if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
-            self._raise(rc)
+        out = _HOST.empty((H, R), np.float64)
+        status = _HOST.empty((H, R), np.int32) if want_status else None
+        self._check(self._lib.phmm_batcher_populate(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()),
+                                                    _ref(_positions(_HOST, positions)), _ref(_flank(flank_state)), _ptr(out), _ptr(status)),
+                    want_status)
         return (out, status) if want_status else out
 
     def populate_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, flank_state=None, want_status=False):
@@ -565,116 +465,78 @@ class PopulateBatcher:
         assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
         toff = np.ascontiguousarray(template_off, dtype=np.int64)
         T = len(toff) - 1
-        hs, rs = haps.c_struct(), reads.c_struct()
-        cfg = config.c_struct() if hasattr(config, "c_struct") else config
-        fstruct = None if flank_state is None else _lib.FlankState(1, int(flank_state[0]), int(flank_state[1]))
-        out = np.empty((haps.n, T), dtype=np.float64)
-        status = np.empty((haps.n, reads.n), dtype=np.int32) if want_status else None
-        rc = self._lib.phmm_batcher_populate_templates(self._h, C.byref(cfg), C.byref(hs), C.byref(rs), toff.ctypes.data, T,
-                                                       C.byref(fstruct) if fstruct is not None else None, out.ctypes.data,
-                                                       status.ctypes.data if want_status else None)
-        if rc != _lib.PHMM_OK and not (rc == _lib.PHMM_ERR_SHORT_HAPLOTYPE and want_status):
-            self._raise(rc)
+        out = _HOST.empty((haps.n, T), np.float64)
+        status = _HOST.empty((haps.n, reads.n), np.int32) if want_status else None
+        self._check(self._lib.phmm_batcher_populate_templates(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()),
+                                                              toff.ctypes.data, T, _ref(_flank(flank_state)), _ptr(out), _ptr(status)),
+                    want_status)
         return (out, status) if want_status else out
 
 
-def _pack_sequences(sequences):
-    parts = [np.frombuffer(x.encode() if isinstance(x, str) else bytes(x), dtype=np.uint8) for x in sequences]
-    off = np.zeros(len(parts) + 1, dtype=np.int64)
-    np.cumsum([len(x) for x in parts], out=off[1:])
-    seq = np.ascontiguousarray(np.concatenate(parts)) if parts else np.zeros(1, dtype=np.uint8)
-    return off, seq
-
-
-class MutationModel:
+class MutationModel(_Handle):
     """DeNovoModel's parameters (core/models/mutation/denovo_model.hpp: Parameters{snv_prior, indel_prior}) as the engine holds them:
     the SNV prior and IndelMutationModel's repeat table for the indel prior (indel_mutation_model.cpp:40-55), open [P+1, Q+1] and
     extend [P+1, Q+1, X] float32 probabilities. The caller computes the table (it is not part of this library); the reference's
     defaults are P = 10, Q = 50, X = 50. SomaticMutationModel uses the same model under the cancer caller's priors."""
+    _destroy = "phmm_mutation_model_destroy"
 
     def __init__(self, snv_prior, open_table, extend_table):
-        self._lib = _lib.load()
         self._open = np.ascontiguousarray(open_table, dtype=np.float32)
         self._extend = np.ascontiguousarray(extend_table, dtype=np.float32)
         if self._open.ndim != 2 or self._extend.ndim != 3 or self._extend.shape[:2] != self._open.shape:
             raise ValueError("open must be [P+1, Q+1] and extend [P+1, Q+1, X]")
         P, Q, X = self._open.shape[0] - 1, self._open.shape[1] - 1, self._extend.shape[2]
-        h = C.c_void_p()
-        rc = self._lib.phmm_mutation_model_create(C.byref(h), float(snv_prior), self._open.ctypes.data, self._extend.ctypes.data, P, Q, X)
-        if rc != _lib.PHMM_OK:
-            raise PhmmError(rc, self._lib.phmm_error_model_last_error().decode())
-        self._h = h
+        self._create("phmm_mutation_model_create", float(snv_prior), self._open.ctypes.data, self._extend.ctypes.data, P, Q, X)
         self.snv_prior = float(snv_prior)
         self.max_period, self.max_periodicity, self.max_indel_length = P, Q, X
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                self._lib.phmm_mutation_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+    def _last_error(self):
+        return self._lib.phmm_error_model_last_error().decode()
 
     def context(self, sequences, n_threads=0):
         """IndelMutationModel::evaluate per haplotype (host): (cell, open_penalty, extend_penalty), flat over the concatenated bases.
         cell = period * (max_periodicity + 1) + periods of the repeat-table cell each base takes its probabilities from."""
-        off, seq = _pack_sequences(sequences)
+        off, seq = pack_sequences(sequences)
         total = int(off[-1])
         cell = np.empty(total, dtype=np.int32)
         op, ep = np.empty(total, dtype=np.int8), np.empty(total, dtype=np.int8)
-        rc = self._lib.phmm_mutation_context(self._h, len(off) - 1, off.ctypes.data, seq.ctypes.data, cell.ctypes.data, op.ctypes.data,
-                                             ep.ctypes.data, int(n_threads))
-        if rc != _lib.PHMM_OK:
-            raise PhmmError(rc, self._lib.phmm_error_model_last_error().decode())
+        self._check(self._lib.phmm_mutation_context(self._h, len(off) - 1, off.ctypes.data, seq.ctypes.data, cell.ctypes.data, op.ctypes.data,
+                                                    ep.ctypes.data, int(n_threads)))
         return cell, op, ep
 
 
-class ErrorModel:
+class ErrorModel(_Handle):
     """The reference's sequencing-error models behind HaplotypeLikelihoodModel::reset (haplotype_likelihood_model.cpp:60-78):
     make_error_model(label) / make_error_model(file) (core/models/error/error_model_factory.cpp:531-589). ``reset`` turns
     haplotype sequences into the HaplotypeBlock the engine consumes (host C++ inside libphmm_b200.so, no GPU involved)."""
+    _destroy = "phmm_error_model_destroy"
 
     def __init__(self, label=None, custom_model_text=None):
-        self._lib = _lib.load()
-        h = C.c_void_p()
         if custom_model_text is not None:
-            rc = self._lib.phmm_error_model_create_custom(C.byref(h), custom_model_text.encode() if isinstance(custom_model_text, str) else custom_model_text)
+            self._create("phmm_error_model_create_custom", custom_model_text.encode() if isinstance(custom_model_text, str) else custom_model_text)
         else:
-            rc = self._lib.phmm_error_model_create(C.byref(h), None if label is None else label.encode())
-        if rc != _lib.PHMM_OK:
-            raise PhmmError(rc, self._lib.phmm_error_model_last_error().decode())
-        self._h = h
+            self._create("phmm_error_model_create", None if label is None else label.encode())
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                self._lib.phmm_error_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+    def _last_error(self):
+        return self._lib.phmm_error_model_last_error().decode()
 
     def tandem_repeats(self, sequence, min_period=1, max_period=5):
         """tandem::extract_exact_tandem_repeats (lib/tandem/tandem.hpp:504-521): (n, 3) uint32 rows (pos, length, period)."""
-        s = np.ascontiguousarray(np.frombuffer(sequence.encode() if isinstance(sequence, str) else bytes(sequence), dtype=np.uint8))
-        cap = 4 * len(s) + 16
-        while True:
+        s = _u8(sequence)
+
+        def attempt(cap):
             out = np.zeros((cap, 3), dtype=np.uint32)
             n = self._lib.phmm_tandem_repeats(s.ctypes.data, len(s), int(min_period), int(max_period), out.ctypes.data, cap)
             if n < 0:
-                raise PhmmError(n, self._lib.phmm_error_model_last_error().decode())
-            if n <= cap:
-                return out[:n]
-            cap = n
+                self._raise(n)
+            return n, out[:n]
+        return _grow(attempt, 4 * len(s) + 16)
 
     def reset(self, sequences, begin=None, is_substitution=None, n_threads=0):
         """HaplotypeLikelihoodModel::reset for every haplotype: sequences (list of str / bytes / uint8 arrays) → HaplotypeBlock
         with the SNV masks / priors and gap penalties the reference's models assign. ``is_substitution``: optional list of
         per-base flag arrays (bases that are substitutions in Haplotype::cigar())."""
-        parts = [np.frombuffer(x.encode() if isinstance(x, str) else bytes(x), dtype=np.uint8) if not isinstance(x, np.ndarray) else
-                 np.ascontiguousarray(x).view(np.uint8).reshape(-1) for x in sequences]
-        off = np.zeros(len(parts) + 1, dtype=np.int64)
-        np.cumsum([len(x) for x in parts], out=off[1:])
-        seq = np.ascontiguousarray(np.concatenate(parts)) if parts else np.zeros(0, dtype=np.uint8)
+        off, seq = pack_sequences(sequences)
         return self.reset_block(off, seq, begin, None if is_substitution is None else
                                 np.ascontiguousarray(np.concatenate([np.asarray(x, dtype=np.uint8) for x in is_substitution])), n_threads)
 
@@ -684,11 +546,10 @@ class ErrorModel:
         total = int(off[-1])
         mf, mr = np.empty(total, dtype=np.uint8), np.empty(total, dtype=np.uint8)
         pf, pr, go, ge = (np.empty(total, dtype=np.int8) for _ in range(4))
-        rc = self._lib.phmm_reset_haplotypes(self._h, len(off) - 1, off.ctypes.data, seq.ctypes.data,
-                                             None if is_substitution is None else is_substitution.ctypes.data,
-                                             mf.ctypes.data, pf.ctypes.data, mr.ctypes.data, pr.ctypes.data, go.ctypes.data, ge.ctypes.data, int(n_threads))
-        if rc != _lib.PHMM_OK:
-            raise PhmmError(rc, self._lib.phmm_error_model_last_error().decode())
+        self._check(self._lib.phmm_reset_haplotypes(self._h, len(off) - 1, off.ctypes.data, seq.ctypes.data,
+                                                    None if is_substitution is None else is_substitution.ctypes.data,
+                                                    mf.ctypes.data, pf.ctypes.data, mr.ctypes.data, pr.ctypes.data, go.ctypes.data,
+                                                    ge.ctypes.data, int(n_threads)))
         return HaplotypeBlock(off, seq, mf, pf, mr, pr, go, ge, begin)
 
 
@@ -753,19 +614,6 @@ class HaplotypeLikelihoodArray:
             self._engine = PairHMMEngine()
         return self._engine
 
-    @staticmethod
-    def _concat_reads(blocks):
-        if len(blocks) == 1:
-            return blocks[0]
-        off = [np.zeros(1, dtype=np.int64)]
-        base = 0
-        for b in blocks:
-            off.append(b.off[1:] + base)
-            base += int(b.off[-1])
-        return ReadBlock(np.concatenate(off), np.concatenate([b.bases for b in blocks]), np.concatenate([b.quals for b in blocks]),
-                         np.concatenate([b.mapq for b in blocks]), np.concatenate([b.reverse for b in blocks]),
-                         np.concatenate([b.begin for b in blocks]))
-
     def _set_samples(self, names, widths):
         self._samples = list(names)
         self._off = [0]
@@ -784,7 +632,7 @@ class HaplotypeLikelihoodArray:
         names = list(reads.keys())
         blocks = [reads[k] for k in names]
         self._set_samples(names, [b.n for b in blocks])
-        self.likelihoods = self.engine.populate(self.likelihood_model.config, haplotypes, self._concat_reads(blocks), positions, flank_state)
+        self.likelihoods = self.engine.populate(self.likelihood_model.config, haplotypes, concat_reads(blocks), positions, flank_state)
         return self
 
     def populate_templates(self, templates, haplotypes: HaplotypeBlock, flank_state=None):
@@ -800,7 +648,7 @@ class HaplotypeLikelihoodArray:
             toff.append(off[1:] + base)
             base += rb.n
         self._set_samples(names, [len(templates[k][1]) - 1 for k in names])
-        self.likelihoods = self.engine.populate_templates(self.likelihood_model.config, haplotypes, self._concat_reads(blocks),
+        self.likelihoods = self.engine.populate_templates(self.likelihood_model.config, haplotypes, concat_reads(blocks),
                                                           np.concatenate(toff), flank_state)
         return self
 

@@ -19,7 +19,8 @@ def _u8(x):
     return np.ascontiguousarray(np.asarray(x)).view(np.uint8).reshape(-1)
 
 
-def _concat(seqs, dtype):
+def pack_sequences(seqs, dtype=np.uint8):
+    """One array per entry → (off[n+1] int64, the entries back to back). For uint8, str / bytes / arrays of any dtype give their bytes."""
     off = np.zeros(len(seqs) + 1, dtype=np.int64)
     parts = []
     for i, s in enumerate(seqs):
@@ -27,7 +28,7 @@ def _concat(seqs, dtype):
         parts.append(a)
         off[i + 1] = off[i] + len(a)
     data = np.concatenate(parts) if parts else np.zeros(0, dtype=dtype)
-    return np.ascontiguousarray(data.astype(dtype, copy=False)), off
+    return off, np.ascontiguousarray(data.astype(dtype, copy=False))
 
 
 class _Block:
@@ -141,19 +142,19 @@ class ReadBlock(_Block):
 
 def pack_haplotypes(seqs, snv_mask_fwd, snv_prior_fwd, snv_mask_rev, snv_prior_rev, gap_open, gap_extend, begin=None):
     """Lists (one entry per haplotype) → HaplotypeBlock."""
-    seq, off = _concat(seqs, np.uint8)
-    mf, _ = _concat(snv_mask_fwd, np.uint8)
-    pf, _ = _concat(snv_prior_fwd, np.int8)
-    mr, _ = _concat(snv_mask_rev, np.uint8)
-    pr, _ = _concat(snv_prior_rev, np.int8)
-    go, _ = _concat(gap_open, np.int8)
-    ge, _ = _concat(gap_extend, np.int8)
+    off, seq = pack_sequences(seqs)
+    _, mf = pack_sequences(snv_mask_fwd, np.uint8)
+    _, pf = pack_sequences(snv_prior_fwd, np.int8)
+    _, mr = pack_sequences(snv_mask_rev, np.uint8)
+    _, pr = pack_sequences(snv_prior_rev, np.int8)
+    _, go = pack_sequences(gap_open, np.int8)
+    _, ge = pack_sequences(gap_extend, np.int8)
     return HaplotypeBlock(off, seq, mf, pf, mr, pr, go, ge, begin)
 
 
 def pack_reads(bases, quals, mapq=None, reverse=None, begin=None):
-    b, off = _concat(bases, np.uint8)
-    q, _ = _concat(quals, np.uint8)
+    off, b = pack_sequences(bases)
+    _, q = pack_sequences(quals)
     return ReadBlock(off, b, q, mapq, reverse, begin)
 
 
@@ -171,19 +172,30 @@ def pack_positions(position_lists, H, R):
     return off, np.asarray(flat if flat else [0], dtype=np.int32)[:max(len(flat), 1)]
 
 
+def _cat_off(blocks):
+    off, base = [np.zeros(1, dtype=np.int64)], 0
+    for b in blocks:
+        off.append(b.off[1:] + base)
+        base += int(b.off[-1])
+    return np.concatenate(off)
+
+
+def _cat(blocks, f):
+    return np.concatenate([getattr(b, f) for b in blocks])
+
+
+def concat_reads(blocks):
+    """Host read blocks back to back as one ReadBlock (the block itself when there is one)."""
+    if len(blocks) == 1:
+        return blocks[0]
+    return ReadBlock(_cat_off(blocks), *[_cat(blocks, f) for f in ReadBlock._fields[1:]])
+
+
 def concat_blocks(hap_blocks, read_blocks):
     """Regions back to back for PairHMMEngine.populate_regions: (HaplotypeBlock, ReadBlock, hap_first, read_first) (host blocks)."""
-    def cat_off(blocks):
-        off, base = [np.zeros(1, dtype=np.int64)], 0
-        for b in blocks:
-            off.append(b.off[1:] + base)
-            base += int(b.off[-1])
-        return np.concatenate(off)
-    cat = lambda blocks, f: np.concatenate([getattr(b, f) for b in blocks])     # noqa: E731
-    haps = HaplotypeBlock(cat_off(hap_blocks), *[cat(hap_blocks, f) for f in HaplotypeBlock._fields[1:8]],
+    haps = HaplotypeBlock(_cat_off(hap_blocks), *[_cat(hap_blocks, f) for f in HaplotypeBlock._fields[1:8]],
                           np.concatenate([b.begin if b.begin is not None else np.zeros(b.n, dtype=np.int64) for b in hap_blocks]))
-    reads = ReadBlock(cat_off(read_blocks), cat(read_blocks, "bases"), cat(read_blocks, "quals"), cat(read_blocks, "mapq"),
-                      cat(read_blocks, "reverse"), cat(read_blocks, "begin"))
+    reads = concat_reads(read_blocks)
     hap_first = np.concatenate([[0], np.cumsum([b.n for b in hap_blocks])]).astype(np.int32)
     read_first = np.concatenate([[0], np.cumsum([b.n for b in read_blocks])]).astype(np.int32)
     return haps, reads, hap_first, read_first

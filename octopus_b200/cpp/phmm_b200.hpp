@@ -250,17 +250,24 @@ private:
 // ---------------------------------------------------------------------------------------------------------------------
 // Per-call seam
 // ---------------------------------------------------------------------------------------------------------------------
-template <int BandSize>
-class GpuPairHMM
+// The kernel with a runtime band, like simd::PairHMMWrapper (simd_pair_hmm_wrapper.hpp:218-241: smallest of 8, 16, ..., 256 that
+// holds the request; TooLargeBandSizeError beyond). GpuPairHMM<Band> below fixes the band at compile time.
+class GpuPairHMMDyn
 {
 public:
     using ScoreType = int;
     constexpr static char gap_label = '-';
 
-    explicit GpuPairHMM(Engine engine = Engine {}) : engine_ {std::move(engine)} {}
+    GpuPairHMMDyn() = default;
+    explicit GpuPairHMMDyn(unsigned min_band_size, Engine engine = Engine {}) : engine_ {std::move(engine)} { reset(min_band_size); }
+    void reset(unsigned min_band_size)
+    {
+        for (int b = 8; b <= 256; b <<= 1) if (min_band_size <= static_cast<unsigned>(b)) { band_ = b; return; }
+        throw TooLargeBandSizeError {min_band_size};
+    }
 
     constexpr static const char* name() noexcept { return "H100"; }
-    constexpr static int band_size() noexcept { return BandSize; }
+    int band_size() const noexcept { return band_; }
 
     // score only, no SNV model (simd_pair_hmm.hpp:438-452)
     template <typename GapExtend>
@@ -332,8 +339,12 @@ public:
         return result;
     }
 
+protected:
+    GpuPairHMMDyn(Engine engine, int band) : engine_ {std::move(engine)}, band_ {band} {}   // an exact band (GpuPairHMM<Band>)
+
 private:
     Engine engine_;
+    int band_ = 8;
 
     static int get(const std::int8_t* v, int i) noexcept { return v[i]; }
     template <typename T> static int get(T v, int) noexcept { return static_cast<int>(v); }
@@ -349,12 +360,26 @@ private:
     {
         int score = 0;
         std::vector<char> a1, a2;
-        if (!align1) { a1.assign(2 * (target_len + BandSize) + 1, 0); a2 = a1; align1 = a1.data(); align2 = a2.data(); }
-        const int rc = phmm_align_traceback(engine_.get(), BandSize, truth, target, quals, truth_len, target_len, snv_mask, snv_prior,
+        if (!align1) { a1.assign(2 * (target_len + band_) + 1, 0); a2 = a1; align1 = a1.data(); align2 = a2.data(); }
+        const int rc = phmm_align_traceback(engine_.get(), band_, truth, target, quals, truth_len, target_len, snv_mask, snv_prior,
                                             gap_open, ext_ptr(gap_extend), ext_scalar(gap_extend), nuc_prior, &score, &first_pos, align1, align2);
         if (rc != PHMM_OK) first_pos = -1;   // the reference signals failure through first_pos (simd_pair_hmm.hpp:176-199)
         return score;
     }
+};
+
+template <int BandSize>
+class GpuPairHMM : private GpuPairHMMDyn
+{
+public:
+    using GpuPairHMMDyn::ScoreType;
+    using GpuPairHMMDyn::gap_label;
+    using GpuPairHMMDyn::name;
+    using GpuPairHMMDyn::align;
+    using GpuPairHMMDyn::calculate_flank_score;
+
+    explicit GpuPairHMM(Engine engine = Engine {}) : GpuPairHMMDyn {std::move(engine), BandSize} {}
+    constexpr static int band_size() noexcept { return BandSize; }
 };
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -454,6 +479,26 @@ struct TemplateBlock   // AlignedTemplate containers: template t owns the reads 
 
 struct FlankState { std::int64_t lhs_flank, rhs_flank; };   // HaplotypeLikelihoodModel::FlankState
 
+namespace detail {
+
+inline phmm_flank_state flank_state(const FlankState* f) noexcept
+{
+    return phmm_flank_state {f ? 1 : 0, f ? f->lhs_flank : 0, f ? f->rhs_flank : 0};
+}
+
+// Throws ShortHaplotypeError for the first of n statuses whose code is PHMM_STATUS_SHORT_HAP (its high 16 bits: the required
+// extension); haplotype_of(i) is the haplotype index of status i's pair.
+template <typename HaplotypeOf>
+void throw_first_short_haplotype(const std::int32_t* status, std::size_t n, HaplotypeOf haplotype_of)
+{
+    for (std::size_t i = 0; i < n; ++i) {
+        if ((status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP)
+            throw ShortHaplotypeError {haplotype_of(i), static_cast<unsigned>(static_cast<std::uint32_t>(status[i]) >> 16)};
+    }
+}
+
+} // namespace detail
+
 // One read's result of ReadRealigner::realign (read_realigner.cpp:92-103, 128-130): HaplotypeLikelihoodModel::Alignment.
 struct Realignment
 {
@@ -470,13 +515,13 @@ inline std::vector<Realignment> realign(const ReadBlock& reads, const HaplotypeB
 {
     std::vector<phmm_pair> pairs(reads.size());
     for (std::size_t r = 0; r < reads.size(); ++r) pairs[r] = phmm_pair {static_cast<std::int32_t>(r), static_cast<std::int32_t>(haplotype)};
-    const phmm_flank_state fs {flank_state ? 1 : 0, flank_state ? flank_state->lhs_flank : 0, flank_state ? flank_state->rhs_flank : 0};
+    const phmm_flank_state fs = detail::flank_state(flank_state);
     const auto a = engine.realign_reads(config, haplotypes.view(), reads.view(), pairs, &fs);
     std::vector<Realignment> result;
     result.reserve(pairs.size());
     for (std::size_t r = 0; r < pairs.size(); ++r) {
+        detail::throw_first_short_haplotype(&a.status[r], 1, [haplotype] (std::size_t) { return haplotype; });
         const int code = a.status[r] & 0xFFFF;
-        if (code == PHMM_STATUS_SHORT_HAP) throw ShortHaplotypeError {haplotype, static_cast<unsigned>(static_cast<std::uint32_t>(a.status[r]) >> 16)};
         if (code == PHMM_STATUS_HMM_OVERFLOW) throw Error {PHMM_ERR_INVALID, "HMMOverflow"};
         if (code == PHMM_STATUS_CIGAR_TRUNCATED) throw Error {PHMM_ERR_INVALID, "CIGAR truncated"};
         result.push_back(Realignment {a.mapping_position[r], a.cigar[r], a.likelihood[r]});
@@ -507,18 +552,18 @@ inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& 
                                                                const phmm_config& config, const Engine& engine = Engine {})
 {
     const auto a = engine.assign_reads(config, haplotypes.view(), reads.view(), hap_first, read_first, log_priors);
+    if (a.code == PHMM_ERR_SHORT_HAPLOTYPE) {
+        std::size_t slot = 0;
+        for (std::size_t g = 0; g + 1 < hap_first.size(); ++g) {
+            const auto nh = static_cast<std::size_t>(hap_first[g + 1] - hap_first[g]), nr = static_cast<std::size_t>(read_first[g + 1] - read_first[g]);
+            detail::throw_first_short_haplotype(a.status.data() + slot, nh * nr, [&] (std::size_t i) { return hap_first[g] + i / nr; });
+            slot += nh * nr;
+        }
+        throw Error {a.code, "Haplotype is too short for alignment"};
+    }
     std::vector<HaplotypeSupport> result(hap_first.size() - 1);
-    std::size_t slot = 0;
     for (std::size_t g = 0; g + 1 < hap_first.size(); ++g) {
         const auto nh = static_cast<std::size_t>(hap_first[g + 1] - hap_first[g]), nr = static_cast<std::size_t>(read_first[g + 1] - read_first[g]);
-        if (a.code == PHMM_ERR_SHORT_HAPLOTYPE) {
-            for (std::size_t i = 0; i < nh * nr; ++i) {
-                if ((a.status[slot + i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP)
-                    throw ShortHaplotypeError {hap_first[g] + i / nr, static_cast<unsigned>(static_cast<std::uint32_t>(a.status[slot + i]) >> 16)};
-            }
-            slot += nh * nr;
-            continue;
-        }
         HaplotypeSupport& s = result[g];
         s.reads.resize(nh);
         for (std::size_t i = 0; i < nr; ++i) {
@@ -535,7 +580,6 @@ inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& 
             s.ambiguous.emplace_back(r, std::move(set));
         }
     }
-    if (a.code == PHMM_ERR_SHORT_HAPLOTYPE) throw Error {a.code, "Haplotype is too short for alignment"};
     return result;
 }
 
@@ -679,15 +723,9 @@ public:
     using ReadMap = std::vector<std::pair<SampleName, ReadBlock>>;                 // config/common.hpp:33-37, in sample order
     using TemplateMap = std::vector<std::pair<SampleName, TemplateBlock>>;
 
-    explicit HaplotypeLikelihoodArray(phmm_config config, Engine engine = Engine {}) : engine_ {std::move(engine)}, config_ {config}
-    {
-        if (config.max_indel_error > 256) throw TooLargeBandSizeError {static_cast<unsigned>(config.max_indel_error)};
-    }
+    explicit HaplotypeLikelihoodArray(phmm_config config, Engine engine = Engine {}) : engine_ {std::move(engine)}, config_ {checked(config)} {}
     // populate() goes through a process-wide SharedEngine: any number of threads, each with its own array, share one GPU engine
-    HaplotypeLikelihoodArray(phmm_config config, SharedEngine shared) : engine_ {nullptr}, shared_ {std::move(shared)}, config_ {config}
-    {
-        if (config.max_indel_error > 256) throw TooLargeBandSizeError {static_cast<unsigned>(config.max_indel_error)};
-    }
+    HaplotypeLikelihoodArray(phmm_config config, SharedEngine shared) : engine_ {nullptr}, shared_ {std::move(shared)}, config_ {checked(config)} {}
     static phmm_config default_config() noexcept { phmm_config c; phmm_default_config(&c); return c; }
 
     // populate(const ReadMap&, haplotypes, flank_state) — haplotype_likelihood_array.cpp:51-103.
@@ -794,6 +832,11 @@ private:
     std::size_t num_haplotypes_ = 0;
     mutable std::ptrdiff_t primed_ = -1;
 
+    static phmm_config checked(const phmm_config& config)
+    {
+        if (config.max_indel_error > 256) throw TooLargeBandSizeError {static_cast<unsigned>(config.max_indel_error)};
+        return config;
+    }
     void begin_samples(std::size_t n) { samples_.clear(); samples_.reserve(n); sample_off_.assign(1, 0); unprime(); }
     void add_sample(const SampleName& name, std::size_t n) { samples_.push_back(name); sample_off_.push_back(sample_off_.back() + n); }
     std::size_t total_width() const noexcept { return sample_off_.back(); }
@@ -823,7 +866,7 @@ private:
         if (num_haplotypes_ == 0 || reads.size() == 0) return;
         pinned_vector<std::int32_t>& status = status_;               // page-locked scratch kept across calls: allocating pinned memory costs milliseconds
         status.resize(num_haplotypes_ * reads.size());
-        phmm_flank_state fs {flank_state ? 1 : 0, flank_state ? flank_state->lhs_flank : 0, flank_state ? flank_state->rhs_flank : 0};
+        phmm_flank_state fs = detail::flank_state(flank_state);
         const auto n_templates = template_off ? static_cast<std::int32_t>(template_off->size() - 1) : 0;
         int rc;
         if (shared_.get()) {
@@ -836,11 +879,8 @@ private:
                                           status.data(), PHMM_SPACE_HOST)
                 : phmm_populate(engine_.get(), &config_, &hv, &rv, positions, &fs, likelihoods_.data(), status.data(), PHMM_SPACE_HOST);
         }
-        if (rc == PHMM_ERR_SHORT_HAPLOTYPE) {
-            for (std::size_t i = 0; i < status.size(); ++i) {
-                if ((status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) throw ShortHaplotypeError {i / reads.size(), static_cast<unsigned>(static_cast<std::uint32_t>(status[i]) >> 16)};
-            }
-        }
+        if (rc == PHMM_ERR_SHORT_HAPLOTYPE)
+            detail::throw_first_short_haplotype(status.data(), status.size(), [&reads] (std::size_t i) { return i / reads.size(); });
         if (shared_.get()) shared_.check(rc); else engine_.check(rc);
     }
 };
@@ -850,64 +890,8 @@ private:
 // ---------------------------------------------------------------------------------------------------------------------
 // The reference's class bundles a kernel object with a `const Parameters*` and forwards to the free templates hmm::evaluate /
 // hmm::align. Those templates are the reference's own code, so this type exists only where its header has been included before
-// this one (Octopus's build; tests/cpp/test_dropin.cpp): it differs from octopus::hmm::PairHMM in the kernel member alone.
-// The kernel is GpuPairHMM with a RUNTIME band, like simd::PairHMMWrapper (simd_pair_hmm_wrapper.hpp:218-241: smallest of
-// 8, 16, ..., 256 that holds the request; TooLargeBandSizeError beyond).
-class GpuPairHMMDyn
-{
-public:
-    using ScoreType = int;
-    constexpr static char gap_label = '-';
-    GpuPairHMMDyn() = default;
-    explicit GpuPairHMMDyn(unsigned min_band_size, Engine engine = Engine {}) : engine_ {std::move(engine)} { reset(min_band_size); }
-    void reset(unsigned min_band_size)
-    {
-        for (int b = 8; b <= 256; b <<= 1) if (min_band_size <= static_cast<unsigned>(b)) { band_ = b; return; }
-        throw TooLargeBandSizeError {min_band_size};
-    }
-    constexpr static const char* name() noexcept { return "H100"; }
-    int band_size() const noexcept { return band_; }
-    template <typename GapExtend>
-    int align(const char* truth, const char* target, const std::int8_t* qualities, int truth_len, int target_len,
-              const std::int8_t* gap_open, GapExtend gap_extend, short nuc_prior) const noexcept
-    { int fp; return run(truth, target, qualities, truth_len, target_len, nullptr, nullptr, gap_open, gap_extend, nuc_prior, fp, nullptr, nullptr); }
-    template <typename GapExtend>
-    int align(const char* truth, const char* target, const std::int8_t* qualities, int truth_len, int target_len,
-              const char* snv_mask, const std::int8_t* snv_prior, const std::int8_t* gap_open, GapExtend gap_extend, short nuc_prior) const noexcept
-    { int fp; return run(truth, target, qualities, truth_len, target_len, snv_mask, snv_prior, gap_open, gap_extend, nuc_prior, fp, nullptr, nullptr); }
-    template <typename GapExtend>
-    int align(const char* truth, const char* target, const std::int8_t* qualities, int truth_len, int target_len,
-              const std::int8_t* gap_open, GapExtend gap_extend, short nuc_prior, int& first_pos, char* align1, char* align2) const noexcept
-    { return run(truth, target, qualities, truth_len, target_len, nullptr, nullptr, gap_open, gap_extend, nuc_prior, first_pos, align1, align2); }
-    template <typename GapExtend>
-    int align(const char* truth, const char* target, const std::int8_t* qualities, int truth_len, int target_len,
-              const char* snv_mask, const std::int8_t* snv_prior, const std::int8_t* gap_open, GapExtend gap_extend, short nuc_prior,
-              int& first_pos, char* align1, char* align2) const noexcept
-    { return run(truth, target, qualities, truth_len, target_len, snv_mask, snv_prior, gap_open, gap_extend, nuc_prior, first_pos, align1, align2); }
-    template <typename... Args>
-    int calculate_flank_score(Args&&... args) const noexcept { return GpuPairHMM<8> {engine_}.calculate_flank_score(std::forward<Args>(args)...); }   // band-independent replay
-private:
-    Engine engine_;
-    int band_ = 8;
-    static const std::int8_t* ext_ptr(const std::int8_t* p) noexcept { return p; }
-    template <typename T> static const std::int8_t* ext_ptr(T) noexcept { return nullptr; }
-    static int ext_scalar(const std::int8_t*) noexcept { return 0; }
-    template <typename T> static int ext_scalar(T v) noexcept { return static_cast<int>(v); }
-    template <typename GapExtend>
-    int run(const char* truth, const char* target, const std::int8_t* quals, int truth_len, int target_len,
-            const char* snv_mask, const std::int8_t* snv_prior, const std::int8_t* gap_open, GapExtend gap_extend, short nuc_prior,
-            int& first_pos, char* align1, char* align2) const noexcept
-    {
-        int score = 0;
-        std::vector<char> a1, a2;
-        if (!align1) { a1.assign(2 * (target_len + band_) + 1, 0); a2 = a1; align1 = a1.data(); align2 = a2.data(); }
-        const int rc = phmm_align_traceback(engine_.get(), band_, truth, target, quals, truth_len, target_len, snv_mask, snv_prior,
-                                            gap_open, ext_ptr(gap_extend), ext_scalar(gap_extend), nuc_prior, &score, &first_pos, align1, align2);
-        if (rc != PHMM_OK) first_pos = -1;
-        return score;
-    }
-};
-
+// this one (Octopus's build; tests/cpp/test_dropin.cpp): it differs from octopus::hmm::PairHMM in the kernel member alone, a
+// GpuPairHMMDyn (runtime band).
 #ifdef pair_hmm_hpp   // the include guard of the reference's src/core/models/pairhmm/pair_hmm.hpp
 template <typename Parameters, int BandSize = 0>
 class PairHMM
