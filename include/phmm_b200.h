@@ -315,6 +315,17 @@ int phmm_populate_templates(phmm_engine* e, const phmm_config* cfg,
  * with phmm_populate's checks and messages, before it joins a batch (the [0,127] penalty check included, on the host); a
  * failing request returns at once and never changes another request's result. When a request fails with another code than
  * PHMM_ERR_SHORT_HAPLOTYPE, its out and status are unspecified. Errors of the whole call (CUDA, NOMEM) go to every member.
+ *
+ * Mutation-model requests (phmm_batcher_mutation_prime, declared after the mutation model below): the trio, cell and cancer
+ * callers prime one small haplotype set per region from the same thread pool. Concurrent requests whose models are equal BY
+ * CONTENT (the SNV prior and the repeat table the model was created from; separately created models merge) are merged into one
+ * phmm_mutation_prime_sets call, a set per request, at most PHMM_MUT_MAX_PAIRS ordered pairs per call; requests from models that
+ * differ never share a call. They follow the same policy as populate requests (leader, clients, max_wait_us, one engine call at a
+ * time; populate and mutation calls take turns on the engine) with a page-locked staging of their own. Every request is checked
+ * on its own thread with phmm_mutation_prime's checks and messages; a failing request returns at once. A request's return code,
+ * status and its out at PHMM_MUT_HMM / PHMM_MUT_SELF pairs are bit for bit what phmm_mutation_prime returns for it alone; errors
+ * of the whole call (CUDA, NOMEM, the internal CIGAR-scratch error) go to every member. The statistics count these calls as they
+ * count populate calls (a set is a region).
  * ------------------------------------------------------------------------------------------------------------------- */
 typedef struct phmm_batcher phmm_batcher;
 typedef struct {
@@ -407,6 +418,7 @@ typedef struct phmm_mutation_model phmm_mutation_model;
 
 #define PHMM_MUT_MAX_HAPLOTYPES   4096
 #define PHMM_MUT_MAX_LENGTH       65535
+#define PHMM_MUT_MAX_PAIRS        (1LL << 26)   /* ordered pairs of one call (sum of n_s^2 over its sets); >= 4096^2, so any set fits */
 
 /* The model: snv_prior in (0, 1] and IndelMutationModel's repeat table as its constructor computes it for the indel prior
  * (indel_mutation_model.cpp:40-55): open[p * (max_periodicity + 1) + q] and extend[(p * (max_periodicity + 1) + q) * max_indel_length + k]
@@ -430,6 +442,25 @@ int  phmm_mutation_context(const phmm_mutation_model* m, int32_t n, const int64_
  * lazy evaluate of larger sets alike. Large sets run in tiles of pairs; one kernel chain per tile. */
 int  phmm_mutation_prime(phmm_engine* e, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
                          double* out, int32_t* status);
+
+/* DeNovoModel::prime for n_sets haplotype sets in one kernel chain: Octopus primes one small set per region, and one region's set
+ * does not fill the GPU. The haplotypes of every set lie in one block (off / seq as phmm_mutation_prime, off[set_first[n_sets] + 1]).
+ * Set s owns haplotypes [set_first[s], set_first[s+1]), 0 <= size <= PHMM_MUT_MAX_HAPLOTYPES; an empty set contributes no pairs.
+ * out / status hold the sets' n_s x n_s matrices back to back in set order: set s starts at sum_{s'<s} n_s'^2, and within a set
+ * the layout is phmm_mutation_prime's (t * n_s + g, set-local indices). Every set's status is what phmm_mutation_prime returns for
+ * that set alone, and its out is bit-equal wherever the status is PHMM_MUT_HMM or PHMM_MUT_SELF (each given haplotype is padded
+ * to its own set's longest haplotype, as the one-set call pads it). PHMM_ERR_INVALID, with a message, for a null pointer,
+ * set_first[0] != 0, a decreasing set_first, a set over PHMM_MUT_MAX_HAPLOTYPES, a haplotype whose offsets give a length outside
+ * [1, PHMM_MUT_MAX_LENGTH] (where set_first[n_sets] exceeds the haplotypes the offsets describe, the first haplotype past them
+ * fails this check unless the memory after off happens to hold valid offsets), or more than PHMM_MUT_MAX_PAIRS pairs in all.
+ * n_sets == 0 returns PHMM_OK without touching the GPU. phmm_mutation_prime is the one-set case of this call. */
+int  phmm_mutation_prime_sets(phmm_engine* e, const phmm_mutation_model* m, int32_t n_sets, const int32_t* set_first,
+                              const int64_t* off, const char* seq, double* out, int32_t* status);
+
+/* phmm_mutation_prime through a shared engine (the batcher contract above). Thread-safe and blocking; host memory. Arguments,
+ * return code, out and status as phmm_mutation_prime; the message of a failure in phmm_batcher_last_error. */
+int  phmm_batcher_mutation_prime(phmm_batcher* b, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
+                                 double* out, int32_t* status);
 
 #ifdef __cplusplus
 }

@@ -5,7 +5,8 @@ Names and argument meaning follow the reference:
   * ``HaplotypeLikelihoodModel.Config``       ↔ HaplotypeLikelihoodModel::Config (haplotype_likelihood_model.hpp:36-44)
   * ``HaplotypeLikelihoodArray.populate``     ↔ HaplotypeLikelihoodArray::populate (haplotype_likelihood_array.cpp:51-103)
   * ``ShortHaplotypeError``                   ↔ HaplotypeLikelihoodModel::ShortHaplotypeError (:123-139)
-  * ``MutationModel`` + ``PairHMMEngine.mutation_prime`` ↔ DeNovoModel::prime / evaluate (core/models/mutation/denovo_model.cpp:64-84)
+  * ``MutationModel`` + ``PairHMMEngine.mutation_prime`` ↔ DeNovoModel::prime / evaluate (core/models/mutation/denovo_model.cpp:64-84);
+    ``mutation_prime_sets`` primes many regions' sets in one call, ``PopulateBatcher.mutation_prime`` from many threads on one engine
 Every computing call goes through libphmm_b200.so to the GPU; nothing here computes likelihoods on the CPU.
 """
 import ctypes as C
@@ -124,6 +125,13 @@ def _regions(hap_first, read_first, flank_states=None):
     return regs, off
 
 
+def _mutation_set(sequences):
+    """One haplotype set → (off, seq, out, status): the packed block and its zeroed [H, H] outputs."""
+    off, seq = pack_sequences(sequences)
+    H = len(off) - 1
+    return off, seq, np.zeros((H, H), dtype=np.float64), np.zeros((H, H), dtype=np.int32)
+
+
 class _Alignments:
     """The outputs of n alignments: mapping position, likelihood, CIGAR text (n x stride bytes, NUL-terminated) and status, zeroed."""
 
@@ -234,13 +242,26 @@ class PairHMMEngine(_Handle):
         """DeNovoModel::prime + evaluate for one haplotype set (phmm_mutation_prime): sequences (list of str / bytes) → (out, status),
         both [H, H] indexed [target, given]. out[t, g] = ln p(target | given) where status is MUT_HMM or MUT_SELF; the MUT_APPROX_*
         pairs need the reference's approximate path (Haplotype::difference) and MUT_OUT_OF_MODEL pairs have no defined value."""
-        off, seq = pack_sequences(sequences)
-        H = len(off) - 1
-        out = np.zeros((H, H), dtype=np.float64)
-        status = np.zeros((H, H), dtype=np.int32)
-        self._check(self._lib.phmm_mutation_prime(self._h, model._h, H, off.ctypes.data, seq.ctypes.data, out.ctypes.data,
+        off, seq, out, status = _mutation_set(sequences)
+        self._check(self._lib.phmm_mutation_prime(self._h, model._h, len(off) - 1, off.ctypes.data, seq.ctypes.data, out.ctypes.data,
                                                   status.ctypes.data))
         return out, status
+
+    def mutation_prime_sets(self, model, sets):
+        """DeNovoModel::prime for many haplotype sets in one call (phmm_mutation_prime_sets): sets (list of lists of sequences) → one
+        (out, status) pair of [n_s, n_s] arrays per set, each what mutation_prime returns for that set alone. Empty sets are allowed."""
+        sets = [list(s) for s in sets]
+        sizes = np.array([len(s) for s in sets], dtype=np.int64)
+        set_first = np.zeros(len(sets) + 1, dtype=np.int32)
+        np.cumsum(sizes, out=set_first[1:])
+        pair_first = np.zeros(len(sets) + 1, dtype=np.int64)
+        np.cumsum(sizes * sizes, out=pair_first[1:])
+        off, seq = pack_sequences([x for s in sets for x in s])
+        out = np.zeros(int(pair_first[-1]), dtype=np.float64)
+        status = np.zeros(int(pair_first[-1]), dtype=np.int32)
+        self._check(self._lib.phmm_mutation_prime_sets(self._h, model._h, len(sets), set_first.ctypes.data, off.ctypes.data, seq.ctypes.data,
+                                                       out.ctypes.data, status.ctypes.data))
+        return [(out[a:b].reshape(n, n), status[a:b].reshape(n, n)) for a, b, n in zip(pair_first[:-1], pair_first[1:], sizes)]
 
     # -- raw kernel boundary -----------------------------------------------------------------------------------
     def align_scores(self, band, haps: HaplotypeBlock, reads: ReadBlock, tasks, nuc_prior=2, precision_bits=16):
@@ -428,8 +449,9 @@ class PairHMMEngine(_Handle):
 
 class PopulateBatcher(_Handle):
     """One engine shared by many host threads (phmm_batcher_*): the populate requests that concurrent threads have in flight run
-    as one multi-region kernel chain. Calls are thread-safe and block; ctypes releases the GIL during them, so Python threads
-    really do wait together. Each result equals what ``PairHMMEngine.populate`` returns for the request alone. Host blocks only."""
+    as one multi-region kernel chain, their mutation-prime requests as one multi-set call. Calls are thread-safe and block; ctypes
+    releases the GIL during them, so Python threads really do wait together. Each result equals what ``PairHMMEngine.populate`` /
+    ``mutation_prime`` returns for the request alone. Host blocks only."""
     _destroy = "phmm_batcher_destroy"
 
     def __init__(self, device=-1, clients=0, max_wait_us=None):
@@ -471,6 +493,14 @@ class PopulateBatcher(_Handle):
                                                               toff.ctypes.data, T, _ref(_flank(flank_state)), _ptr(out), _ptr(status)),
                     want_status)
         return (out, status) if want_status else out
+
+    def mutation_prime(self, model, sequences):
+        """As PairHMMEngine.mutation_prime, through the shared engine: concurrent requests whose models are equal by content run as
+        one phmm_mutation_prime_sets call, each with the (out, status) it gets alone."""
+        off, seq, out, status = _mutation_set(sequences)
+        self._check(self._lib.phmm_batcher_mutation_prime(self._h, model._h, len(off) - 1, off.ctypes.data, seq.ctypes.data,
+                                                          out.ctypes.data, status.ctypes.data))
+        return out, status
 
 
 class MutationModel(_Handle):

@@ -640,17 +640,16 @@ public:
     using ApproxFunction = std::function<LogProbability(std::size_t target_idx, std::size_t given_idx)>;
 
     DeNovoModel(Parameters parameters, const MutationRepeatTable& table, Engine& engine, ApproxFunction approx = nullptr)
-    : params_ {parameters}, engine_ {&engine}, approx_ {std::move(approx)}
-    {
-        phmm_mutation_model* m = nullptr;
-        const int rc = phmm_mutation_model_create(&m, parameters.snv_prior, table.open.data(), table.extend.data(), table.max_period,
-                                                  table.max_periodicity, table.max_indel_length);
-        if (rc != PHMM_OK) throw Error {rc, phmm_error_model_last_error()};
-        model_.reset(m, [] (phmm_mutation_model* p) { phmm_mutation_model_destroy(p); });
-    }
+    : DeNovoModel {parameters, table, &engine, SharedEngine {nullptr}, std::move(approx)} {}
+    // prime() through a process-wide SharedEngine: any number of threads, each with its own model object, may prime at once; their
+    // sets run as one phmm_mutation_prime_sets call where the models are equal (trio_caller.cpp:406 builds one per region)
+    DeNovoModel(Parameters parameters, const MutationRepeatTable& table, SharedEngine& shared, ApproxFunction approx = nullptr)
+    : DeNovoModel {parameters, table, nullptr, shared, std::move(approx)} {}
 #ifdef indel_mutation_model_config_hpp
     DeNovoModel(Parameters parameters, Engine& engine, ApproxFunction approx = nullptr)
     : DeNovoModel {parameters, MutationRepeatTable::from_reference(parameters.indel_prior), engine, std::move(approx)} {}
+    DeNovoModel(Parameters parameters, SharedEngine& shared, ApproxFunction approx = nullptr)
+    : DeNovoModel {parameters, MutationRepeatTable::from_reference(parameters.indel_prior), shared, std::move(approx)} {}
 #endif
 
     Parameters parameters() const { return params_; }
@@ -665,8 +664,9 @@ public:
         values_.assign(n * n, 0.0);
         status_.assign(n * n, PHMM_MUT_SELF);
         settled_.assign(n * n, 0);
-        if (n > 0) engine_->check(phmm_mutation_prime(engine_->get(), model_.get(), static_cast<std::int32_t>(n), off.data(), seq.data(),
-                                                      values_.data(), status_.data()));
+        const auto h = static_cast<std::int32_t>(n);
+        if (n > 0 && engine_) engine_->check(phmm_mutation_prime(engine_->get(), model_.get(), h, off.data(), seq.data(), values_.data(), status_.data()));
+        if (n > 0 && !engine_) shared_.check(phmm_batcher_mutation_prime(shared_.get(), model_.get(), h, off.data(), seq.data(), values_.data(), status_.data()));
         n_ = n;
     }
     void unprime() noexcept { values_ = {}; status_ = {}; settled_ = {}; n_ = 0; }
@@ -687,8 +687,19 @@ public:
     std::int32_t status(const std::size_t target_idx, const std::size_t given_idx) const { return status_.at(target_idx * n_ + given_idx); }
 
 private:
+    DeNovoModel(Parameters parameters, const MutationRepeatTable& table, Engine* engine, SharedEngine shared, ApproxFunction approx)
+    : params_ {parameters}, engine_ {engine}, shared_ {std::move(shared)}, approx_ {std::move(approx)}
+    {
+        phmm_mutation_model* m = nullptr;
+        const int rc = phmm_mutation_model_create(&m, parameters.snv_prior, table.open.data(), table.extend.data(), table.max_period,
+                                                  table.max_periodicity, table.max_indel_length);
+        if (rc != PHMM_OK) throw Error {rc, phmm_error_model_last_error()};
+        model_.reset(m, [] (phmm_mutation_model* p) { phmm_mutation_model_destroy(p); });
+    }
+
     Parameters params_;
-    Engine* engine_;
+    Engine* engine_;              // null: prime() goes through shared_
+    SharedEngine shared_;
     ApproxFunction approx_;
     std::shared_ptr<phmm_mutation_model> model_;
     std::size_t n_ = 0;

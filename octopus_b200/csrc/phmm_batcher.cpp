@@ -1,8 +1,10 @@
 // Shared engine for many host threads (include/phmm_b200.h, phmm_batcher_*): the populate requests that concurrent threads
-// have in flight are merged into one phmm_populate_regions call. Host C++ over the public C ABI; the batch runs the engine's
-// existing regions kernel chain. No thread of its own: the first member of a batch (its leader) makes the call.
+// have in flight are merged into one phmm_populate_regions call, their mutation-prime requests into one phmm_mutation_prime_sets
+// call. Host C++ over the public C ABI; a batch runs the engine's existing multi-region / multi-set kernel chain. No thread of its
+// own: the first member of a batch (its leader) makes the call.
 #include "../../include/phmm_b200.h"
 #include "phmm_checks.h"
+#include "phmm_mutation.h"
 
 #include <algorithm>
 #include <chrono>
@@ -88,13 +90,49 @@ struct Staging {
     }
 };
 
+// Element counts of a mutation-prime request or batch.
+struct MutationSizes {
+    long long haps = 0, bases = 0, pairs = 0;
+    MutationSizes& operator+=(const MutationSizes& o) { haps += o.haps; bases += o.bases; pairs += o.pairs; return *this; }
+    bool within(const MutationSizes& cap) const { return haps <= cap.haps && bases <= cap.bases && pairs <= cap.pairs; }
+    static MutationSizes max(const MutationSizes& a, const MutationSizes& b)
+    {
+        MutationSizes s;
+        s.haps = std::max(a.haps, b.haps); s.bases = std::max(a.bases, b.bases); s.pairs = std::max(a.pairs, b.pairs);
+        return s;
+    }
+};
+
+// One mutation batch's page-locked copy of its members' haplotypes and its results.
+struct MutationStaging {
+    Pinned<int64_t> off;
+    Pinned<char> seq;
+    Pinned<double> out;
+    Pinned<int32_t> status;
+    MutationSizes cap;
+    bool busy = false;
+
+    bool grow(const MutationSizes& s)
+    {
+        if (s.within(cap)) return true;
+        if (!(off.ensure(s.haps + 1) && seq.ensure(s.bases) && out.ensure(s.pairs) && status.ensure(s.pairs))) return false;
+        cap.haps = off.cap - 1; cap.bases = seq.cap; cap.pairs = std::min(out.cap, status.cap);
+        return true;
+    }
+};
+
+// A batch of populate requests (cfg, st, ...) or of mutation-prime requests (model, ms, ...); the rest is the shared life cycle.
 struct Batch {
-    phmm_config cfg {};
     std::string key;
+    phmm_config cfg {};
     Staging* st = nullptr;
     Sizes used;
     std::vector<int32_t> hap_first {0}, read_first {0};
     std::vector<phmm_flank_state> flanks;
+    const phmm_mutation_model* model = nullptr;     // the leader's model (the members' are equal by content)
+    MutationStaging* ms = nullptr;
+    MutationSizes mused;
+    std::vector<int32_t> set_first {0};
     Clock::time_point deadline;
     int members = 0;
     int pending_copies = 0;     // members that reserved space and have not finished copying in
@@ -107,6 +145,8 @@ struct Batch {
 };
 
 std::string config_key(const phmm_config* cfg) { return std::string(reinterpret_cast<const char*>(cfg), sizeof(phmm_config)); }
+// never the length of a config key (the model key alone is longer), so the two kinds share one map of open batches
+std::string model_key(const phmm_mutation_model* m) { return "mutation model " + m->key; }
 
 } // namespace
 
@@ -116,9 +156,11 @@ struct phmm_batcher {
     int max_wait_us = kDefaultMaxWaitUs;
     mutable std::mutex m;
     std::condition_variable cv;
-    std::map<std::string, Batch*> open;               // the open batch of each distinct config
+    std::map<std::string, Batch*> open;               // the open batch of each distinct config or mutation model
     std::vector<std::unique_ptr<Staging>> staging;
     Sizes want;                                       // staging high-water mark: what merged batches have asked for
+    std::vector<std::unique_ptr<MutationStaging>> mutation_staging;
+    MutationSizes mutation_want;
     bool engine_busy = false;
     int waiting = 0;                                  // requests in batches not yet sent + requests running alone
     int in_flight = 0;                                // requests inside the batcher
@@ -157,18 +199,23 @@ int run_alone(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* ha
     return rc;
 }
 
-// A batch for `key` with a free staging set large enough for `need` (grown to the high-water mark); nullptr when out of memory.
-Batch* open_batch(phmm_batcher* b, const std::string& key, const phmm_config* cfg, const Sizes& need)
+// A free staging set of `pool`, large enough for `need` (grown to the high-water mark `want`) and marked busy; nullptr when out of memory.
+template <typename S, typename N>
+S* free_staging(std::vector<std::unique_ptr<S>>& pool, const N& need, const N& want)
 {
-    Staging* st = nullptr;
-    for (auto& s : b->staging) if (!s->busy) { st = s.get(); break; }
-    if (!st) { b->staging.emplace_back(new Staging()); st = b->staging.back().get(); }
-    if (!st->grow(Sizes::max(need, b->want))) return nullptr;
+    S* st = nullptr;
+    for (auto& s : pool) if (!s->busy) { st = s.get(); break; }
+    if (!st) { pool.emplace_back(new S()); st = pool.back().get(); }
+    if (!st->grow(N::max(need, want))) return nullptr;
     st->busy = true;
+    return st;
+}
+
+// A new open batch for `key`, sent at the latest max_wait_us from now.
+Batch* open_batch(phmm_batcher* b, const std::string& key)
+{
     Batch* bt = new Batch();
-    bt->cfg = *cfg;
     bt->key = key;
-    bt->st = st;
     bt->deadline = Clock::now() + std::chrono::microseconds(b->max_wait_us);
     b->open[key] = bt;
     return bt;
@@ -243,6 +290,59 @@ int check_request(const phmm_config* cfg, const phmm_haplotypes* haps, const phm
     return PHMM_OK;
 }
 
+// The life of a request in a batch, the same for every kind. Entered under the lock once the request has reserved its slot in bt:
+// copy_in() writes the request into the staging outside the lock (each member its own ranges); the first member leads: it waits
+// until `clients` requests wait, the batch is full or its deadline has passed, and the engine is free, then seals the batch and
+// makes the call run(b, bt); the others wait for it. copy_out() (outside the lock) reads this member's slice and returns its code;
+// the last reader frees the staging and the batch.
+template <typename CopyIn, typename CopyOut>
+int take_part(phmm_batcher* b, std::unique_lock<std::mutex>& lk, Batch* bt, CopyIn copy_in, void (*run)(phmm_batcher*, Batch*), CopyOut copy_out)
+{
+    const bool leader = bt->members == 0;
+    ++bt->members; ++bt->pending_copies; ++bt->readers; ++b->waiting;
+    b->cv.notify_all();
+    lk.unlock();
+
+    copy_in();
+
+    lk.lock();
+    --bt->pending_copies;
+    if (leader) {
+        for (;;) {
+            const bool company = b->clients > 0 && b->waiting >= b->clients;
+            const bool go = bt->full || company || Clock::now() >= bt->deadline;
+            if (go && !b->engine_busy) break;
+            if (go) b->cv.wait(lk);
+            else b->cv.wait_until(lk, bt->deadline);
+        }
+        close_batch(b, bt);
+        b->engine_busy = true;
+        b->waiting -= bt->members;
+        b->cv.wait(lk, [&] { return bt->pending_copies == 0; });
+        lk.unlock();
+        run(b, bt);
+        lk.lock();
+        count_call(b, bt->members);
+        b->engine_busy = false;
+        bt->done = true;
+        b->cv.notify_all();
+    } else {
+        b->cv.notify_all();                       // the leader may be waiting for this copy
+        b->cv.wait(lk, [&] { return bt->done; });
+    }
+    lk.unlock();
+
+    const int rc = copy_out();
+
+    lk.lock();
+    if (--bt->readers == 0) {
+        if (bt->st) bt->st->busy = false;
+        if (bt->ms) bt->ms->busy = false;
+        delete bt;
+    }
+    return rc;
+}
+
 int submit(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_positions* positions,
            const int64_t* template_off, int32_t n_templates, const phmm_flank_state* flank, double* out, int32_t* status)
 {
@@ -260,8 +360,11 @@ int submit(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps,
     for (;;) {
         const auto it = b->open.find(key);
         if (it == b->open.end()) {
-            bt = open_batch(b, key, cfg, need);
-            if (!bt) { t_error = "out of page-locked host memory for the batch staging"; return PHMM_ERR_NOMEM; }
+            Staging* st = free_staging(b->staging, need, b->want);
+            if (!st) { t_error = "out of page-locked host memory for the batch staging"; return PHMM_ERR_NOMEM; }
+            bt = open_batch(b, key);
+            bt->cfg = *cfg;
+            bt->st = st;
             break;
         }
         bt = it->second;
@@ -278,72 +381,89 @@ int submit(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps,
     bt->hap_first.push_back((int32_t)bt->used.haps);
     bt->read_first.push_back((int32_t)bt->used.reads);
     bt->flanks.push_back(flank ? *flank : phmm_flank_state {0, 0, 0});
-    const bool leader = bt->members == 0;
-    ++bt->members; ++bt->pending_copies; ++bt->readers; ++b->waiting;
-    b->cv.notify_all();
-    lk.unlock();
-
-    copy_in(bt->st, at, haps, reads);
-
-    lk.lock();
-    --bt->pending_copies;
-    if (leader) {
-        for (;;) {
-            const bool company = b->clients > 0 && b->waiting >= b->clients;
-            const bool go = bt->full || company || Clock::now() >= bt->deadline;
-            if (go && !b->engine_busy) break;
-            if (go) b->cv.wait(lk);
-            else b->cv.wait_until(lk, bt->deadline);
-        }
-        close_batch(b, bt);
-        b->engine_busy = true;
-        b->waiting -= bt->members;
-        b->cv.wait(lk, [&] { return bt->pending_copies == 0; });
-        lk.unlock();
-        run_batch(b, bt);
-        lk.lock();
-        count_call(b, bt->members);
-        b->engine_busy = false;
-        bt->done = true;
-        b->cv.notify_all();
-    } else {
-        b->cv.notify_all();                       // the leader may be waiting for this copy
-        b->cv.wait(lk, [&] { return bt->done; });
-    }
-    lk.unlock();
-
-    // this member's slice of the result: [H][R] at the pair offset of its region
-    int rc = bt->rc;
-    const int H = haps->n, R = reads->n;
-    const double* res = bt->st->out.p + at.pairs;
-    const int32_t* res_status = bt->st->status.p + at.pairs;
-    if (rc == PHMM_OK || rc == PHMM_ERR_SHORT_HAPLOTYPE) {
-        rc = PHMM_OK;
-        for (long long i = 0; i < need.pairs; ++i) if ((res_status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) { rc = PHMM_ERR_SHORT_HAPLOTYPE; break; }
-        t_error = rc == PHMM_OK ? std::string() : std::string("Haplotype is too short for alignment");
-        if (status) std::memcpy(status, res_status, (size_t)need.pairs * sizeof(int32_t));
-        if (template_off) {
-            // k_template_sum's order: each template's reads left to right from 0.0
-            for (int h = 0; h < H; ++h) {
-                for (int t = 0; t < n_templates; ++t) {
-                    double acc = 0.0;
-                    for (long long r = template_off[t]; r < template_off[t + 1]; ++r) acc += res[(size_t)h * R + r];
-                    out[(size_t)h * n_templates + t] = acc;
+    return take_part(b, lk, bt, [&] { copy_in(bt->st, at, haps, reads); }, run_batch, [&] {
+        // this member's slice of the result: [H][R] at the pair offset of its region
+        int rc = bt->rc;
+        const int H = haps->n, R = reads->n;
+        const double* res = bt->st->out.p + at.pairs;
+        const int32_t* res_status = bt->st->status.p + at.pairs;
+        if (rc == PHMM_OK || rc == PHMM_ERR_SHORT_HAPLOTYPE) {
+            rc = PHMM_OK;
+            for (long long i = 0; i < need.pairs; ++i) if ((res_status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) { rc = PHMM_ERR_SHORT_HAPLOTYPE; break; }
+            t_error = rc == PHMM_OK ? std::string() : std::string("Haplotype is too short for alignment");
+            if (status) std::memcpy(status, res_status, (size_t)need.pairs * sizeof(int32_t));
+            if (template_off) {
+                // k_template_sum's order: each template's reads left to right from 0.0
+                for (int h = 0; h < H; ++h) {
+                    for (int t = 0; t < n_templates; ++t) {
+                        double acc = 0.0;
+                        for (long long r = template_off[t]; r < template_off[t + 1]; ++r) acc += res[(size_t)h * R + r];
+                        out[(size_t)h * n_templates + t] = acc;
+                    }
                 }
+            } else {
+                std::memcpy(out, res, (size_t)need.pairs * sizeof(double));
             }
         } else {
-            std::memcpy(out, res, (size_t)need.pairs * sizeof(double));
+            t_error = bt->err;
         }
-    } else {
-        t_error = bt->err;
-    }
+        return rc;
+    });
+}
 
-    lk.lock();
-    if (--bt->readers == 0) {
-        bt->st->busy = false;
-        delete bt;
+// The leader's call: the batch's members as the sets of one phmm_mutation_prime_sets call.
+void run_mutation_batch(phmm_batcher* b, Batch* bt)
+{
+    MutationStaging* ms = bt->ms;
+    bt->rc = phmm_mutation_prime_sets(b->engine, bt->model, bt->members, bt->set_first.data(), ms->off.p, ms->seq.p, ms->out.p, ms->status.p);
+    if (bt->rc != PHMM_OK) bt->err = phmm_last_error(b->engine);
+}
+
+int submit_mutation(phmm_batcher* b, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq, double* out, int32_t* status)
+{
+    const int rc = phmm_checks::mutation_set(m, n, off, seq, out, status, t_error);
+    if (rc != PHMM_OK) return rc;
+    MutationSizes need;
+    need.haps = n; need.bases = off[n]; need.pairs = (long long)n * n;
+
+    const std::string key = model_key(m);
+    std::unique_lock<std::mutex> lk(b->m);
+    Batch* bt = nullptr;
+    for (;;) {
+        const auto it = b->open.find(key);
+        if (it == b->open.end()) {
+            MutationStaging* ms = free_staging(b->mutation_staging, need, b->mutation_want);
+            if (!ms) { t_error = "out of page-locked host memory for the batch staging"; return PHMM_ERR_NOMEM; }
+            bt = open_batch(b, key);
+            bt->model = m;
+            bt->ms = ms;
+            break;
+        }
+        bt = it->second;
+        MutationSizes total = bt->mused;
+        total += need;
+        if (total.pairs <= PHMM_MUT_MAX_PAIRS && total.within(bt->ms->cap)) break;
+        if (total.pairs <= PHMM_MUT_MAX_PAIRS) b->mutation_want = MutationSizes::max(b->mutation_want, total);   // staging too small
+        bt->full = true;
+        close_batch(b, bt);
+        b->cv.notify_all();
     }
-    return rc;
+    const MutationSizes at = bt->mused;
+    bt->mused += need;
+    bt->set_first.push_back((int32_t)bt->mused.haps);
+    return take_part(b, lk, bt, [&] {
+        MutationStaging* ms = bt->ms;
+        if (at.haps == 0) ms->off.p[0] = 0;
+        for (int h = 0; h < n; ++h) ms->off.p[at.haps + h + 1] = at.bases + off[h + 1];
+        std::memcpy(ms->seq.p + at.bases, seq, (size_t)need.bases);
+    }, run_mutation_batch, [&] {
+        // this member's n x n matrix at the pair offset of its set
+        if (bt->rc != PHMM_OK) { t_error = bt->err; return bt->rc; }
+        std::memcpy(out, bt->ms->out.p + at.pairs, (size_t)need.pairs * sizeof(double));
+        std::memcpy(status, bt->ms->status.p + at.pairs, (size_t)need.pairs * sizeof(int32_t));
+        t_error.clear();
+        return PHMM_OK;
+    });
 }
 
 // Entry and exit of every request: destroy waits until no request is inside.
@@ -370,6 +490,8 @@ int phmm_batcher_create(phmm_batcher** out, int device, const phmm_batcher_optio
     if (opt) { b->clients = opt->clients; b->max_wait_us = opt->max_wait_us; }
     // first staging size: some tens of regions of a few hundred reads; it grows to what merged batches ask for
     b->want.haps = 4096; b->want.hap_bases = 1LL << 20; b->want.reads = 1LL << 16; b->want.read_bases = 8LL << 20; b->want.pairs = 1LL << 20;
+    // and some tens of mutation sets of 50 haplotypes
+    b->mutation_want.haps = 2048; b->mutation_want.bases = 1LL << 20; b->mutation_want.pairs = 1LL << 17;
     *out = b;
     return PHMM_OK;
 }
@@ -404,6 +526,14 @@ int phmm_batcher_populate_templates(phmm_batcher* b, const phmm_config* cfg, con
     if (rc != PHMM_OK) return rc;
     InFlight guard(b);
     return submit(b, cfg, haps, reads, nullptr, template_off, n_templates, flank, out, status);
+}
+
+int phmm_batcher_mutation_prime(phmm_batcher* b, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
+                                double* out, int32_t* status)
+{
+    if (!b) { t_error = "null batcher"; return PHMM_ERR_INVALID; }
+    InFlight guard(b);
+    return submit_mutation(b, m, n, off, seq, out, status);
 }
 
 int phmm_batcher_stats_get(const phmm_batcher* b, phmm_batcher_stats* out)

@@ -1,4 +1,4 @@
-// Host-side argument checks of the populate entry points, shared by the engine (phmm_engine.cu) and the request batcher
+// Host-side argument checks of the populate and mutation-prime entry points, shared by the engine (phmm_engine.cu) and the request batcher
 // (phmm_batcher.cpp) so that both report the same error codes and messages. Each check returns PHMM_OK or an error code and
 // sets `err`; the callers run them in the order populate reports errors in.
 #ifndef PHMM_CHECKS_H
@@ -86,6 +86,31 @@ inline int template_offsets(const int64_t* template_off, int32_t n_templates, co
         for (int t = 0; t < n_templates; ++t) if (template_off[t + 1] < template_off[t]) { err = "template offsets must be non-decreasing"; return PHMM_ERR_INVALID; }
     }
     return PHMM_OK;
+}
+
+// phmm_mutation_prime's checks of one haplotype set (host memory), in its order
+inline int mutation_haplotype_count(int64_t n, std::string& err)
+{
+    if (n < 1 || n > PHMM_MUT_MAX_HAPLOTYPES) { err = "haplotype count outside [1, 4096]"; return PHMM_ERR_INVALID; }
+    return PHMM_OK;
+}
+
+inline int mutation_offsets(int64_t n, const int64_t* off, std::string& err)
+{
+    if (off[0] != 0) { err = "offset arrays must start at 0"; return PHMM_ERR_INVALID; }
+    for (int64_t h = 0; h < n; ++h) {
+        const long long len = off[h + 1] - off[h];
+        if (len < 1 || len > PHMM_MUT_MAX_LENGTH) { err = "haplotype length outside [1, 65535]"; return PHMM_ERR_INVALID; }
+    }
+    return PHMM_OK;
+}
+
+inline int mutation_set(const void* m, int32_t n, const int64_t* off, const char* seq, const double* out, const int32_t* status, std::string& err)
+{
+    if (!m || !off || !seq || !out || !status) { err = "null argument"; return PHMM_ERR_INVALID; }
+    int rc;
+    if ((rc = mutation_haplotype_count(n, err)) != PHMM_OK) return rc;
+    return mutation_offsets(n, off, err);
 }
 
 // Read-chunk size (in pairs) of phmm_populate's pipelined path for a call of all_pairs pairs; the call is pipelined when it

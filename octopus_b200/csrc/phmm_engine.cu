@@ -960,64 +960,90 @@ int phmm_map_pairs(phmm_engine* e, const phmm_haplotypes* haps, const phmm_reads
 }
 
 // -------------------------------------------------------------------------------------------------------------
-// phmm_mutation_prime
+// phmm_mutation_prime_sets, phmm_mutation_prime
 // -------------------------------------------------------------------------------------------------------------
-// Largest tile of the ordered-pair index space, and the CIGAR scratch a tile may use.
+// Largest tile of the call's ordered-pair index space, and the CIGAR scratch a tile may use.
 static constexpr long long kMutTilePairs = 1LL << 19;
 static constexpr long long kMutCigarBudget = 1LL << 30;
 
-int phmm_mutation_prime(phmm_engine* e, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
-                        double* out, int32_t* status)
+// phmm_mutation_prime_sets after begin_call; phmm_mutation_prime is its one-set case.
+static int mutation_prime_sets(phmm_engine* e, const phmm_mutation_model* m, int32_t n_sets, const int32_t* set_first,
+                               const int64_t* off, const char* seq, double* out, int32_t* status)
 {
-    if (int rc0 = begin_call(e)) return rc0;
-    if (!m || !off || !seq || !out || !status) { e->err = "null argument"; return PHMM_ERR_INVALID; }
-    if (n < 1 || n > PHMM_MUT_MAX_HAPLOTYPES) { e->err = "haplotype count outside [1, 4096]"; return PHMM_ERR_INVALID; }
-    if (off[0] != 0) { e->err = "offset arrays must start at 0"; return PHMM_ERR_INVALID; }
-    long long Lmax = 0;
-    for (int h = 0; h < n; ++h) {
-        const long long len = off[h + 1] - off[h];
-        if (len < 1 || len > PHMM_MUT_MAX_LENGTH) { e->err = "haplotype length outside [1, 65535]"; return PHMM_ERR_INVALID; }
-        Lmax = std::max(Lmax, len);
+    if (!m || !set_first || !off || !seq || !out || !status) { e->err = "null argument"; return PHMM_ERR_INVALID; }
+    if (n_sets < 0) { e->err = "negative set count"; return PHMM_ERR_INVALID; }
+    if (n_sets == 0) return PHMM_OK;
+    if (set_first[0] != 0) { e->err = "set_first[0] must be 0"; return PHMM_ERR_INVALID; }
+    int rc;
+    long long all = 0;                                                            // ordered pairs of the call
+    for (int s = 0; s < n_sets; ++s) {
+        const long long size = (long long)set_first[s + 1] - set_first[s];
+        if (size < 0) { e->err = "set_first must be non-decreasing"; return PHMM_ERR_INVALID; }
+        if (size > 0 && (rc = phmm_checks::mutation_haplotype_count(size, e->err)) != PHMM_OK) return rc;
+        all += size * size;
     }
-    const int H = n, X = m->max_indel_length;
+    const int H = set_first[n_sets];
+    if ((rc = phmm_checks::mutation_offsets(H, off, e->err)) != PHMM_OK) return rc;
+    if (all > PHMM_MUT_MAX_PAIRS) { e->err = "more than PHMM_MUT_MAX_PAIRS (2^26) ordered pairs in one call"; return PHMM_ERR_INVALID; }
+    if (H == 0) return PHMM_OK;
+    // per set: its first pair and its longest haplotype; the call's longest haplotype sizes the CIGAR scratch
+    std::vector<long long> pair_first((size_t)n_sets + 1, 0), set_len((size_t)n_sets, 0);
+    long long Lmax = 0;
+    for (int s = 0; s < n_sets; ++s) {
+        const long long size = set_first[s + 1] - set_first[s];
+        pair_first[s + 1] = pair_first[s] + size * size;
+        for (int h = set_first[s]; h < set_first[s + 1]; ++h) set_len[s] = std::max<long long>(set_len[s], off[h + 1] - off[h]);
+        Lmax = std::max(Lmax, set_len[s]);
+    }
+    const int X = m->max_indel_length;
     const long long B = off[H];
-    // 1. the context indel model of every haplotype (host)
+    // 1. the context indel model of every haplotype of the call (host; per haplotype, so the sets' concatenation does not change it)
     std::vector<int32_t> cell((size_t)B);
     std::vector<int8_t> gop((size_t)B), gex((size_t)B);
-    int rc = phmm_mutation_context(m, n, off, seq, cell.data(), gop.data(), gex.data(), 0);
+    rc = phmm_mutation_context(m, H, off, seq, cell.data(), gop.data(), gex.data(), 0);
     if (rc != PHMM_OK) { e->err = phmm_error_model_last_error(); return rc; }
-    // 2. one padded truth per given haplotype: 32 N's, the haplotype, N's up to the longest haplotype + 64 (pad penalty 60), no SNV mask;
-    //    the targets are the haplotypes with every quality = the SNV penalty (denovo_model.cpp:208-262, pair_hmm.hpp:853-856)
-    const long long Lp = Lmax + 64;
+    // 2. one padded truth per given haplotype: 32 N's, the haplotype, N's up to its own set's longest haplotype + 64 (pad penalty 60), no
+    //    SNV mask — byte for byte the truth a call of that set alone builds; the targets are the haplotypes with every quality = the SNV
+    //    penalty (denovo_model.cpp:208-262, pair_hmm.hpp:853-856)
+    long long T = 0;                                                              // truth bases
+    for (int s = 0; s < n_sets; ++s) T += (long long)(set_first[s + 1] - set_first[s]) * (set_len[s] + 64);
     auto align_up = [](size_t x) { return (x + 255) & ~(size_t)255; };
     size_t at = 0;
-    const size_t o_tseq = at; at = align_up(at + (size_t)H * Lp);
-    const size_t o_tgo = at;  at = align_up(at + (size_t)H * Lp);
-    const size_t o_tge = at;  at = align_up(at + (size_t)H * Lp);
-    const size_t o_zero = at; at = align_up(at + (size_t)H * Lp);                 // SNV masks / priors, mapq, reverse, begin
+    const size_t o_tseq = at; at = align_up(at + (size_t)T);
+    const size_t o_tgo = at;  at = align_up(at + (size_t)T);
+    const size_t o_tge = at;  at = align_up(at + (size_t)T);
+    const size_t o_zero = at; at = align_up(at + (size_t)T);                      // SNV masks / priors, mapq, reverse, begin (T >= 65 H)
     const size_t o_toff = at; at = align_up(at + ((size_t)H + 1) * sizeof(int64_t));
     const size_t o_goff = at; at = align_up(at + ((size_t)H + 1) * sizeof(int64_t));
     const size_t o_bases = at; at = align_up(at + (size_t)B);
     const size_t o_quals = at; at = align_up(at + (size_t)B);
     const size_t o_cell = at; at = align_up(at + (size_t)B * sizeof(int32_t));
     const size_t o_logp = at; at = align_up(at + m->logp.size() * sizeof(float));
+    const size_t o_pfirst = at; at = align_up(at + ((size_t)n_sets + 1) * sizeof(int64_t));
+    const size_t o_sfirst = at; at = align_up(at + ((size_t)n_sets + 1) * sizeof(int32_t));
     const long long cigar_stride = 4 * Lmax + 160;                                  // >= 2 characters per alignment column
     const long long tile = std::max(1LL, std::min(kMutTilePairs, kMutCigarBudget / cigar_stride));
     const size_t o_offs = at; at = align_up(at + (size_t)tile * sizeof(int32_t));
     std::vector<char> blob(at, 0);
     char* bp = blob.data();
-    for (int h = 0; h < H; ++h) {
-        const long long o = off[h], len = off[h + 1] - o, t0 = (long long)h * Lp;
-        std::memset(bp + o_tseq + t0, 'N', (size_t)Lp);
-        std::memcpy(bp + o_tseq + t0 + 32, seq + o, (size_t)len);
-        std::memset(bp + o_tgo + t0, 60, (size_t)Lp);
-        std::memset(bp + o_tge + t0, 60, (size_t)Lp);
-        std::memcpy(bp + o_tgo + t0 + 32, gop.data() + o, (size_t)len);
-        std::memcpy(bp + o_tge + t0 + 32, gex.data() + o, (size_t)len);
-        ((int64_t*)(bp + o_toff))[h] = t0;
+    long long t0 = 0;
+    for (int s = 0; s < n_sets; ++s) {
+        const long long Lp = set_len[s] + 64;
+        for (int h = set_first[s]; h < set_first[s + 1]; ++h, t0 += Lp) {
+            const long long o = off[h], len = off[h + 1] - o;
+            std::memset(bp + o_tseq + t0, 'N', (size_t)Lp);
+            std::memcpy(bp + o_tseq + t0 + 32, seq + o, (size_t)len);
+            std::memset(bp + o_tgo + t0, 60, (size_t)Lp);
+            std::memset(bp + o_tge + t0, 60, (size_t)Lp);
+            std::memcpy(bp + o_tgo + t0 + 32, gop.data() + o, (size_t)len);
+            std::memcpy(bp + o_tge + t0 + 32, gex.data() + o, (size_t)len);
+            ((int64_t*)(bp + o_toff))[h] = t0;
+        }
     }
-    ((int64_t*)(bp + o_toff))[H] = (int64_t)H * Lp;
+    ((int64_t*)(bp + o_toff))[H] = t0;
     std::memcpy(bp + o_goff, off, ((size_t)H + 1) * sizeof(int64_t));
+    std::memcpy(bp + o_pfirst, pair_first.data(), pair_first.size() * sizeof(int64_t));
+    std::memcpy(bp + o_sfirst, set_first, ((size_t)n_sets + 1) * sizeof(int32_t));
     std::memcpy(bp + o_bases, seq, (size_t)B);
     std::memset(bp + o_quals, m->snv_penalty, (size_t)B);
     std::memcpy(bp + o_cell, cell.data(), (size_t)B * sizeof(int32_t));
@@ -1033,24 +1059,26 @@ int phmm_mutation_prime(phmm_engine* e, const phmm_mutation_model* m, int32_t n,
     phmm_config cfg;
     phmm_default_config(&cfg);
     cfg.max_indel_error = 32; cfg.use_mapping_quality = 0; cfg.use_flank_state = 0; cfg.map_positions = 0;
-    const long long all = (long long)H * H;
     CU(e->mu_out.ensure((size_t)all * (sizeof(double) + sizeof(int32_t))));
     double* d_out = e->mu_out.as<double>();
     int* d_status = (int*)(d_out + all);
-    CU(e->mu_list.ensure((size_t)tile * sizeof(int2) + 256));
+    CU(e->mu_list.ensure((size_t)tile * (sizeof(int2) + sizeof(long long)) + 256));
     int2* d_list = e->mu_list.as<int2>();
-    int* d_count = (int*)(d_list + tile);
+    long long* d_oidx = (long long*)(d_list + tile);
+    int* d_count = (int*)(d_oidx + tile);
     CU(e->mu_res.ensure((size_t)tile * (sizeof(int64_t) + sizeof(double) + sizeof(int32_t))));
     int64_t* d_toff = e->mu_res.as<int64_t>();
     double* d_lk = (double*)(d_toff + tile);
     int32_t* d_ast = (int32_t*)(d_lk + tile);
     CU(e->mu_cig.ensure((size_t)tile * cigar_stride));
-    // 3. per tile: list the pairs, align the listed ones (band 32, target offset 32), re-score their CIGARs
+    // 3. per tile of the call's pair space (a tile may begin or end inside a set): list the pairs, align the listed ones (band 32, target
+    //    offset 32), re-score their CIGARs
     for (long long lo = 0; lo < all; lo += tile) {
         const long long hi = std::min(all, lo + tile);
         CU(cudaMemsetAsync(d_count, 0, sizeof(int), e->stream));
-        k_mutation_pairs<<<(unsigned)std::min<long long>((hi - lo + 255) / 256, 4096), 256, 0, e->stream>>>(lo, hi, H, (const long long*)(d + o_goff),
-                                                                                                          d_out, d_status, d_list, d_count);
+        k_mutation_pairs<<<(unsigned)std::min<long long>((hi - lo + 255) / 256, 4096), 256, 0, e->stream>>>(lo, hi, n_sets, (const long long*)(d + o_pfirst),
+                                                                                                          (const int*)(d + o_sfirst), (const long long*)(d + o_goff),
+                                                                                                          d_out, d_status, d_list, d_oidx, d_count);
         LAUNCHED();
         CU(cudaGetLastError());
         int count = 0;
@@ -1060,10 +1088,10 @@ int phmm_mutation_prime(phmm_engine* e, const phmm_mutation_model* m, int32_t n,
         rc = align_impl(e, &cfg, &truths, &targets, (const phmm_pair*)d_list, count, nullptr, (const int32_t*)(d + o_offs), nullptr,
                         d_toff, d_lk, e->mu_cig.as<char>(), (int32_t)cigar_stride, d_ast, PHMM_SPACE_DEVICE);
         if (rc != PHMM_OK) return rc;
-        k_mutation_rescore<<<(unsigned)((count + 127) / 128), 128, 0, e->stream>>>(count, d_list, (const long long*)d_toff, d_ast, e->mu_cig.as<char>(),
-                                                                                 (int)cigar_stride, (const long long*)(d + o_goff),
+        k_mutation_rescore<<<(unsigned)((count + 127) / 128), 128, 0, e->stream>>>(count, d_list, d_oidx, (const long long*)d_toff, d_ast,
+                                                                                 e->mu_cig.as<char>(), (int)cigar_stride, (const long long*)(d + o_goff),
                                                                                  (const int*)(d + o_cell), (const float*)(d + o_logp), X,
-                                                                                 m->snv_log_prior, H, d_out, d_status);
+                                                                                 m->snv_log_prior, d_out, d_status);
         LAUNCHED();
         CU(cudaGetLastError());
     }
@@ -1072,6 +1100,22 @@ int phmm_mutation_prime(phmm_engine* e, const phmm_mutation_model* m, int32_t n,
     CU(cudaStreamSynchronize(e->stream));
     for (long long i = 0; i < all; ++i) if (status[i] < 0) { e->err = "internal error: CIGAR scratch too small"; return PHMM_ERR_CUDA; }
     return PHMM_OK;
+}
+
+int phmm_mutation_prime_sets(phmm_engine* e, const phmm_mutation_model* m, int32_t n_sets, const int32_t* set_first,
+                             const int64_t* off, const char* seq, double* out, int32_t* status)
+{
+    if (int rc0 = begin_call(e)) return rc0;
+    return mutation_prime_sets(e, m, n_sets, set_first, off, seq, out, status);
+}
+
+int phmm_mutation_prime(phmm_engine* e, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq,
+                        double* out, int32_t* status)
+{
+    if (int rc0 = begin_call(e)) return rc0;
+    if (int rc = phmm_checks::mutation_set(m, n, off, seq, out, status, e->err)) return rc;
+    const int32_t set_first[2] = {0, n};
+    return mutation_prime_sets(e, m, 1, set_first, off, seq, out, status);
 }
 
 // -------------------------------------------------------------------------------------------------------------

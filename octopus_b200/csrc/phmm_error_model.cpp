@@ -666,6 +666,11 @@ int phmm_mutation_model_create(phmm_mutation_model** out, double snv_prior, cons
     m->extend.assign(extend, extend + (std::size_t)cells * X);
     for (const float v : m->open) if (!(v > 0.0f && v <= 1.0f)) { delete m; return fail("repeat table open probability outside (0, 1]"); }
     for (const float v : m->extend) if (!(v > 0.0f && v <= 1.0f)) { delete m; return fail("repeat table extend probability outside (0, 1]"); }
+    const std::int32_t dims[3] = {max_period, max_periodicity, max_indel_length};
+    m->key.append(reinterpret_cast<const char*>(&snv_prior), sizeof(snv_prior));
+    m->key.append(reinterpret_cast<const char*>(dims), sizeof(dims));
+    m->key.append(reinterpret_cast<const char*>(m->open.data()), m->open.size() * sizeof(float));
+    m->key.append(reinterpret_cast<const char*>(m->extend.data()), m->extend.size() * sizeof(float));
     m->open_penalty.resize(cells); m->extend_penalty.resize(cells); m->logp.resize((std::size_t)cells * X);
     for (int c = 0; c < cells; ++c) {
         const float* ext = m->extend.data() + (std::size_t)c * X;

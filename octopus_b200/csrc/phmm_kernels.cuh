@@ -1876,34 +1876,49 @@ __global__ void k_list_slots(const PopParams p, const bool init)
 // Mutation statuses (include/phmm_b200.h PHMM_MUT_*).
 constexpr int kMutHmm = 0, kMutSelf = 1, kMutApproxLength = 2, kMutApproxOffset = 3, kMutApproxOverflow = 4, kMutOutOfModel = 5;
 
-// One tile [lo, hi) of the ordered pairs t * H + g. The diagonal and the pairs whose length distance reaches the band
-// (can_try_align_with_hmm, :249-252) are settled here; every other pair is appended to list (as {target, given}) for the DP.
-__global__ void k_mutation_pairs(const long long lo, const long long hi, const int H, const long long* __restrict__ off,
-                                 double* __restrict__ out, int* __restrict__ status, int2* __restrict__ list, int* __restrict__ count)
+// One tile [lo, hi) of the call's ordered-pair space: the sets' t * n_s + g spaces back to back, set s from pair_first[s] (its
+// haplotypes from set_first[s] in the block). The diagonal and the pairs whose length distance reaches the band
+// (can_try_align_with_hmm, :249-252) are settled here; every other pair is appended to list (as {target, given}, block indices) for
+// the DP, its index in the pair space (= its place in out / status) beside it in out_index.
+__global__ void k_mutation_pairs(const long long lo, const long long hi, const int n_sets, const long long* __restrict__ pair_first,
+                                 const int* __restrict__ set_first, const long long* __restrict__ off, double* __restrict__ out,
+                                 int* __restrict__ status, int2* __restrict__ list, long long* __restrict__ out_index, int* __restrict__ count)
 {
     const long long step = (long long)gridDim.x * blockDim.x;
     for (long long i = lo + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += step) {
-        const int t = (int)(i / H), g = (int)(i - (long long)t * H);
+        int s = 0, top = n_sets - 1;                           // the last set that starts at or before i (empty sets start where the next one does)
+        while (s < top) {
+            const int mid = (s + top + 1) >> 1;
+            if (pair_first[mid] <= i) s = mid; else top = mid - 1;
+        }
+        const int h0 = set_first[s], n = set_first[s + 1] - h0;
+        const long long local = i - pair_first[s];
+        const int tl = (int)(local / n), gl = (int)(local - (long long)tl * n);
+        const int t = h0 + tl, g = h0 + gl;
         const long long lt = off[t + 1] - off[t], lg = off[g + 1] - off[g];
         if (t == g) { out[i] = 0.0; status[i] = kMutSelf; continue; }
         if ((lt > lg ? lt - lg : lg - lt) >= 32) { out[i] = 0.0; status[i] = kMutApproxLength; continue; }
-        list[atomicAdd(count, 1)] = make_int2(t, g);
+        const int j = atomicAdd(count, 1);
+        list[j] = make_int2(t, g);
+        out_index[j] = i;
     }
 }
 
 // recalculate_log_probability (:199-218) of each listed pair's alignment, from the CIGAR text the traceback kernels wrote (runs
 // merged as make_cigar merges them, so each run's length is the reference's op.size()). pos counts given bases from the alignment
 // start (= given base 0 at target offset 32); '=', 'X' and 'D' advance it. Double arithmetic with explicit rounding so that no FMA
-// is contracted; the float logs come from the host table logp[cell][min(size, X) - 1].
-__global__ void k_mutation_rescore(const int n, const int2* __restrict__ list, const long long* __restrict__ target_offset,
-                                   const int* __restrict__ align_status, const char* __restrict__ cigar, const int cigar_stride,
-                                   const long long* __restrict__ off, const int* __restrict__ cell, const float* __restrict__ logp,
-                                   const int X, const double snv_log_prior, const int H, double* __restrict__ out, int* __restrict__ status)
+// is contracted; the float logs come from the host table logp[cell][min(size, X) - 1]. Each result goes to the pair's place
+// out_index[j] that k_mutation_pairs stored.
+__global__ void k_mutation_rescore(const int n, const int2* __restrict__ list, const long long* __restrict__ out_index,
+                                   const long long* __restrict__ target_offset, const int* __restrict__ align_status,
+                                   const char* __restrict__ cigar, const int cigar_stride, const long long* __restrict__ off,
+                                   const int* __restrict__ cell, const float* __restrict__ logp, const int X, const double snv_log_prior,
+                                   double* __restrict__ out, int* __restrict__ status)
 {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
     const int2 tg = list[j];
-    const long long i = (long long)tg.x * H + tg.y;
+    const long long i = out_index[j];
     if (align_status[j] != 0) { out[i] = 0.0; status[i] = align_status[j] == 4 ? kMutApproxOverflow : -1; return; }   // -1: CIGAR truncated
     if (target_offset[j] != 32) { out[i] = 0.0; status[i] = kMutApproxOffset; return; }
     const long long g0 = off[tg.y], glen = off[tg.y + 1] - g0;

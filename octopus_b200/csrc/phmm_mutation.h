@@ -1,9 +1,10 @@
 // DeNovoModel's mutation model as the engine holds it (include/phmm_b200.h, phmm_mutation_*): shared by the host context model
-// (phmm_error_model.cpp) and phmm_mutation_prime (phmm_engine.cu).
+// (phmm_error_model.cpp), phmm_mutation_prime (phmm_engine.cu) and the batcher's merge key (phmm_batcher.cpp).
 #ifndef PHMM_MUTATION_H
 #define PHMM_MUTATION_H
 
 #include <cstdint>
+#include <string>
 #include <vector>
 
 struct phmm_mutation_model {
@@ -18,6 +19,9 @@ struct phmm_mutation_model {
     // logp[cell][k] = std::log(calculate_indel_probability(...)) for an indel of length k + 1 (indel_mutation_model.cpp:114-123)
     std::vector<std::int8_t> open_penalty, extend_penalty;
     std::vector<float> logp;           // [cells][max_indel_length]
+    // the model's inputs as bytes (snv_prior, the three dimensions, open, extend): equal keys give equal results, so the batcher
+    // merges the requests of separately created models by this key
+    std::string key;
     int cells() const { return (max_period + 1) * (max_periodicity + 1); }
 };
 

@@ -6,11 +6,19 @@ shape, with the card's name and power limit read in the same run.
 Sets: 50 haplotypes (the reference's largest eagerly primed set, 2 450 ordered pairs) of one region, from synth.make_haplotypes's base
 sequence with injected STRs, each haplotype carrying SNVs and 1-20 bp indels (tests/mutation_oracle.py's mutate).
     python tools/bench_mutation_prime.py [--sets 20] [--out results.json]
+
+With --sets-per-call K and / or --threads T, the same seeded sets instead run three ways, alternated round by round in one process
+after a warm-up of every mode and shape: one phmm_mutation_prime per set ("per_set"), K sets per phmm_mutation_prime_sets call
+("sets_per_call"), and T Python threads priming their share of the sets on one PopulateBatcher, each with a model object of its own
+("threads"). One JSON row per mode and shape: sets per second, median call time, median DP kernel time, the batcher's merged-call
+statistics, and whether every status and every HMM / SELF value equals the per-set call's.
+    python tools/bench_mutation_prime.py --sets 20,100 --sets-per-call 20 --threads 8 [--rounds 3]
 """
 import argparse
 import json
 import os
 import sys
+import threading
 import time
 
 import numpy as np
@@ -45,22 +53,140 @@ def synthetic_table():
     return o, e
 
 
+def same(got, want):
+    """Statuses identical and HMM / SELF values bit-equal."""
+    (out, st), (wout, wst) = got, want
+    exact = (wst == 0) | (wst == 1)
+    return bool(np.array_equal(st, wst) and np.array_equal(out[exact].view(np.uint64), wout[exact].view(np.uint64)))
+
+
+def run_per_set(eng, model, sets, K, T):
+    ms, dp, res = [], [], []
+    for seqs in sets:
+        t0 = time.perf_counter()
+        res.append(eng.mutation_prime(model, seqs))
+        ms.append(1e3 * (time.perf_counter() - t0))
+        dp.append(eng.last_dp_kernel_ms())
+    return res, ms, dp
+
+
+def run_sets_per_call(eng, model, sets, K, T):
+    ms, dp, res = [], [], []
+    for i in range(0, len(sets), K):
+        t0 = time.perf_counter()
+        res += eng.mutation_prime_sets(model, sets[i:i + K])
+        ms.append(1e3 * (time.perf_counter() - t0))
+        dp.append(eng.last_dp_kernel_ms())
+    return res, ms, dp
+
+
+def run_threads(batcher, make_model, sets, K, T):
+    """T threads, thread k priming sets k, k + T, ... one after the other, each with a model of its own (as a caller builds one per
+    region). Call time = one request's latency."""
+    res, ms, errors = [None] * len(sets), [], []
+    start = threading.Barrier(T)
+
+    def worker(k):
+        try:
+            start.wait()
+            for i in range(k, len(sets), T):
+                model = make_model()
+                t0 = time.perf_counter()
+                res[i] = batcher.mutation_prime(model, sets[i])
+                ms.append(1e3 * (time.perf_counter() - t0))
+        except Exception as ex:          # noqa: BLE001
+            errors.append(repr(ex))
+    threads = [threading.Thread(target=worker, args=(k,)) for k in range(T)]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    assert not errors, errors
+    return res, ms, []
+
+
+def compare_modes(a, info, snv, o, e):
+    """Per shape: the three modes on the same seeded sets, alternated round by round after a warm-up of each."""
+    from octopus_b200 import MutationModel, PairHMMEngine, PopulateBatcher
+    eng = PairHMMEngine(0)
+    model = MutationModel(snv, o, e)
+    make_model = lambda: MutationModel(snv, o, e)       # noqa: E731
+    rows = []
+    for length in [int(x) for x in a.lengths.split(",")]:
+        for n_sets in [int(x) for x in str(a.sets).split(",")]:
+            rng = np.random.default_rng(1000 * length + n_sets)
+            sets = [trio_set(rng, a.haplotypes, length) for _ in range(n_sets)]
+            K, T = a.sets_per_call or n_sets, a.threads or 1
+            batcher = PopulateBatcher(0, clients=T, max_wait_us=a.max_wait_us)
+            modes = [("per_set", lambda: run_per_set(eng, model, sets, K, T)),
+                     ("sets_per_call", lambda: run_sets_per_call(eng, model, sets, K, T)),
+                     ("threads", lambda: run_threads(batcher, make_model, sets, K, T))]
+            for _, run in modes:                          # warm-up: module load, scratch and staging growth
+                run()
+            acc = {name: dict(wall=[], ms=[], dp=[], same=True, stats=[]) for name, _ in modes}
+            baseline = None
+            for r in range(a.rounds):
+                order = modes if r % 2 == 0 else modes[::-1]
+                for name, run in order:
+                    before = batcher.stats()
+                    t0 = time.perf_counter()
+                    res, ms, dp = run()
+                    acc[name]["wall"].append(time.perf_counter() - t0)
+                    after = batcher.stats()
+                    acc[name]["ms"] += ms
+                    acc[name]["dp"] += dp
+                    if name == "threads":
+                        acc[name]["stats"].append({k: after[k] - before[k] for k in ("requests", "gpu_calls", "merged_calls")})
+                        acc[name]["max_regions_per_call"] = after["max_regions_per_call"]
+                    if name == "per_set" and baseline is None:
+                        baseline = res
+                    acc[name]["res"] = res
+                for name, _ in modes:
+                    if "res" in acc[name]:
+                        acc[name]["same"] &= all(same(g, w) for g, w in zip(acc[name].pop("res"), baseline))
+            batcher.close()
+            for name, _ in modes:
+                m = acc[name]
+                wall = float(np.median(m["wall"]))
+                row = dict(what="mutation_prime_modes", mode=name, haplotypes=a.haplotypes, length=length, sets=n_sets,
+                           sets_per_call=K if name == "sets_per_call" else 1, threads=T if name == "threads" else 1, rounds=a.rounds,
+                           sets_per_s=n_sets / wall, wall_ms=1e3 * wall, median_call_ms=float(np.median(m["ms"])),
+                           dp_kernel_ms=float(np.median(m["dp"])) if m["dp"] else "not measured (the batcher's engine)",
+                           same_as_per_set=m["same"], **info)
+                if name == "threads":
+                    row.update(batcher_calls_per_round=m["stats"], max_regions_per_call=m["max_regions_per_call"], max_wait_us=a.max_wait_us)
+                rows.append(row)
+                print(json.dumps(row), flush=True)
+    return rows
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--sets", type=int, default=20)
+    ap.add_argument("--sets", default="20", help="sets per shape; a comma list with --sets-per-call / --threads")
     ap.add_argument("--haplotypes", type=int, default=50)
     ap.add_argument("--lengths", default="300,1000")
+    ap.add_argument("--sets-per-call", type=int, default=0)
+    ap.add_argument("--threads", type=int, default=0)
+    ap.add_argument("--max-wait-us", type=int, default=2000)
+    ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "bench_mutation_prime needs a GPU"
     from octopus_b200 import MutationModel, PairHMMEngine, _lib
-    eng = PairHMMEngine(0)
     info = device_info()
     print(json.dumps(info), flush=True)
     snv, indel = TRIO_PRIORS
     ref = RefMutation() if RefMutation.available() else None
     o, e = ref.table(indel) if ref else synthetic_table()
+    if a.sets_per_call or a.threads:
+        rows = compare_modes(a, info, snv, o, e)
+        if a.out:
+            with open(a.out, "w") as f:
+                json.dump(rows, f, indent=1)
+        return
+    a.sets = int(a.sets)
+    eng = PairHMMEngine(0)
     model = MutationModel(snv, o, e)
     rows = []
     for length in [int(x) for x in a.lengths.split(",")]:
