@@ -26,16 +26,18 @@ constexpr int kDefaultMaxWaitUs = 500;
 
 using Clock = std::chrono::steady_clock;
 
-// Element counts of a request or a batch.
-struct Sizes {
-    long long haps = 0, hap_bases = 0, reads = 0, read_bases = 0, pairs = 0;
-    Sizes& operator+=(const Sizes& o) { haps += o.haps; hap_bases += o.hap_bases; reads += o.reads; read_bases += o.read_bases; pairs += o.pairs; return *this; }
-    bool within(const Sizes& cap) const { return haps <= cap.haps && hap_bases <= cap.hap_bases && reads <= cap.reads && read_bases <= cap.read_bases && pairs <= cap.pairs; }
-    static Sizes max(const Sizes& a, const Sizes& b)
+// Element counts of a request or a batch; each request kind names its N counts.
+template <int N>
+struct Counts {
+    long long n[N] = {};
+    long long& operator[](int i) { return n[i]; }
+    long long operator[](int i) const { return n[i]; }
+    Counts& operator+=(const Counts& o) { for (int i = 0; i < N; ++i) n[i] += o.n[i]; return *this; }
+    bool within(const Counts& cap) const { for (int i = 0; i < N; ++i) if (n[i] > cap.n[i]) return false; return true; }
+    static Counts max(const Counts& a, const Counts& b)
     {
-        Sizes s;
-        s.haps = std::max(a.haps, b.haps); s.hap_bases = std::max(a.hap_bases, b.hap_bases); s.reads = std::max(a.reads, b.reads);
-        s.read_bases = std::max(a.read_bases, b.read_bases); s.pairs = std::max(a.pairs, b.pairs);
+        Counts s;
+        for (int i = 0; i < N; ++i) s.n[i] = std::max(a.n[i], b.n[i]);
         return s;
     }
 };
@@ -61,78 +63,205 @@ struct Pinned {
     }
 };
 
-// One batch's page-locked copy of its members' blocks and its results.
-struct Staging {
-    Pinned<int64_t> hap_off, hap_begin, read_off, read_begin;
-    Pinned<char> seq, mask_f, mask_r, bases;
-    Pinned<int8_t> prior_f, prior_r, gap_open, gap_extend;
-    Pinned<uint8_t> quals, mapq, reverse;
-    Pinned<double> out;
-    Pinned<int32_t> status;
-    Sizes cap;
-    bool busy = false;
+// The two request kinds. Each supplies what differs between them: its counts, its staging, its merge key and limits, its
+// per-member bookkeeping (a Kind object lives in each batch), the copy in, the merged engine call and the copy out.
 
-    bool grow(const Sizes& s)
-    {
-        if (s.within(cap)) return true;
-        const bool ok = hap_off.ensure(s.haps + 1) && hap_begin.ensure(s.haps) && read_off.ensure(s.reads + 1) && read_begin.ensure(s.reads) &&
-                        seq.ensure(s.hap_bases) && mask_f.ensure(s.hap_bases) && mask_r.ensure(s.hap_bases) && prior_f.ensure(s.hap_bases) &&
-                        prior_r.ensure(s.hap_bases) && gap_open.ensure(s.hap_bases) && gap_extend.ensure(s.hap_bases) &&
-                        bases.ensure(s.read_bases) && quals.ensure(s.read_bases) && mapq.ensure(s.reads) && reverse.ensure(s.reads) &&
-                        out.ensure(s.pairs) && status.ensure(s.pairs);
-        if (!ok) return false;
-        cap.haps = std::min(hap_off.cap - 1, hap_begin.cap);
-        cap.reads = std::min({read_off.cap - 1, read_begin.cap, mapq.cap, reverse.cap});
-        cap.hap_bases = std::min({seq.cap, mask_f.cap, mask_r.cap, prior_f.cap, prior_r.cap, gap_open.cap, gap_extend.cap});
-        cap.read_bases = std::min(bases.cap, quals.cap);
-        cap.pairs = std::min(out.cap, status.cap);
-        return true;
-    }
-};
+// Populate requests: a batch is one phmm_populate_regions call and each member one of its regions; equal configs merge.
+struct Populate {
+    enum { HAPS, HAP_BASES, READS, READ_BASES, PAIRS, N_COUNTS };
+    using Sizes = Counts<N_COUNTS>;
 
-// Element counts of a mutation-prime request or batch.
-struct MutationSizes {
-    long long haps = 0, bases = 0, pairs = 0;
-    MutationSizes& operator+=(const MutationSizes& o) { haps += o.haps; bases += o.bases; pairs += o.pairs; return *this; }
-    bool within(const MutationSizes& cap) const { return haps <= cap.haps && bases <= cap.bases && pairs <= cap.pairs; }
-    static MutationSizes max(const MutationSizes& a, const MutationSizes& b)
-    {
-        MutationSizes s;
-        s.haps = std::max(a.haps, b.haps); s.bases = std::max(a.bases, b.bases); s.pairs = std::max(a.pairs, b.pairs);
-        return s;
-    }
-};
+    struct Request {
+        const phmm_config* cfg; const phmm_haplotypes* haps; const phmm_reads* reads;
+        const int64_t* template_off; int32_t n_templates;     // template_off NULL: a read request
+        const phmm_flank_state* flank; double* out; int32_t* status;
+        Sizes need;
+    };
 
-// One mutation batch's page-locked copy of its members' haplotypes and its results.
-struct MutationStaging {
-    Pinned<int64_t> off;
-    Pinned<char> seq;
-    Pinned<double> out;
-    Pinned<int32_t> status;
-    MutationSizes cap;
-    bool busy = false;
+    // One batch's page-locked copy of its members' blocks and its results.
+    struct Staging {
+        Pinned<int64_t> hap_off, hap_begin, read_off, read_begin;
+        Pinned<char> seq, mask_f, mask_r, bases;
+        Pinned<int8_t> prior_f, prior_r, gap_open, gap_extend;
+        Pinned<uint8_t> quals, mapq, reverse;
+        Pinned<double> out;
+        Pinned<int32_t> status;
+        Sizes cap;
+        bool busy = false;
 
-    bool grow(const MutationSizes& s)
-    {
-        if (s.within(cap)) return true;
-        if (!(off.ensure(s.haps + 1) && seq.ensure(s.bases) && out.ensure(s.pairs) && status.ensure(s.pairs))) return false;
-        cap.haps = off.cap - 1; cap.bases = seq.cap; cap.pairs = std::min(out.cap, status.cap);
-        return true;
-    }
-};
+        bool grow(const Sizes& s)
+        {
+            const bool ok = hap_off.ensure(s[HAPS] + 1) && hap_begin.ensure(s[HAPS]) && read_off.ensure(s[READS] + 1) && read_begin.ensure(s[READS]) &&
+                            seq.ensure(s[HAP_BASES]) && mask_f.ensure(s[HAP_BASES]) && mask_r.ensure(s[HAP_BASES]) && prior_f.ensure(s[HAP_BASES]) &&
+                            prior_r.ensure(s[HAP_BASES]) && gap_open.ensure(s[HAP_BASES]) && gap_extend.ensure(s[HAP_BASES]) &&
+                            bases.ensure(s[READ_BASES]) && quals.ensure(s[READ_BASES]) && mapq.ensure(s[READS]) && reverse.ensure(s[READS]) &&
+                            out.ensure(s[PAIRS]) && status.ensure(s[PAIRS]);
+            if (!ok) return false;
+            cap[HAPS] = std::min(hap_off.cap - 1, hap_begin.cap);
+            cap[READS] = std::min({read_off.cap - 1, read_begin.cap, mapq.cap, reverse.cap});
+            cap[HAP_BASES] = std::min({seq.cap, mask_f.cap, mask_r.cap, prior_f.cap, prior_r.cap, gap_open.cap, gap_extend.cap});
+            cap[READ_BASES] = std::min(bases.cap, quals.cap);
+            cap[PAIRS] = std::min(out.cap, status.cap);
+            return true;
+        }
+    };
 
-// A batch of populate requests (cfg, st, ...) or of mutation-prime requests (model, ms, ...); the rest is the shared life cycle.
-struct Batch {
-    std::string key;
-    phmm_config cfg {};
-    Staging* st = nullptr;
-    Sizes used;
+    // first staging size: some tens of regions of a few hundred reads; it grows to what merged batches ask for
+    static Sizes initial_staging() { return {{4096, 1LL << 20, 1LL << 16, 8LL << 20, 1LL << 20}}; }
+    static bool within_limits(const Sizes& s) { return s[HAPS] <= kMaxBatchHaps && s[PAIRS] <= kMaxBatchPairs; }
+    static std::string key(const Request& q) { return std::string(reinterpret_cast<const char*>(q.cfg), sizeof(phmm_config)); }
+
+    phmm_config cfg;
     std::vector<int32_t> hap_first {0}, read_first {0};
     std::vector<phmm_flank_state> flanks;
-    const phmm_mutation_model* model = nullptr;     // the leader's model (the members' are equal by content)
-    MutationStaging* ms = nullptr;
-    MutationSizes mused;
+
+    explicit Populate(const Request& q) : cfg(*q.cfg) {}
+
+    // a new member's region, ending at the batch's counts `used`
+    void add(const Request& q, const Sizes& used)
+    {
+        hap_first.push_back((int32_t)used[HAPS]);
+        read_first.push_back((int32_t)used[READS]);
+        flanks.push_back(q.flank ? *q.flank : phmm_flank_state {0, 0, 0});
+    }
+
+    // the request into its slot at `at` (outside the lock: each member writes its own ranges only)
+    static void copy_in(Staging& st, const Sizes& at, const Request& q)
+    {
+        const phmm_haplotypes* haps = q.haps;
+        const phmm_reads* reads = q.reads;
+        const int H = haps->n, R = reads->n;
+        const long long hb = haps->off[H], rb = reads->off[R];
+        if (at[HAPS] == 0) st.hap_off.p[0] = 0;
+        for (int h = 0; h < H; ++h) st.hap_off.p[at[HAPS] + h + 1] = at[HAP_BASES] + haps->off[h + 1];
+        if (haps->begin) std::memcpy(st.hap_begin.p + at[HAPS], haps->begin, (size_t)H * sizeof(int64_t));
+        else std::memset(st.hap_begin.p + at[HAPS], 0, (size_t)H * sizeof(int64_t));
+        std::memcpy(st.seq.p + at[HAP_BASES], haps->seq, (size_t)hb);
+        std::memcpy(st.mask_f.p + at[HAP_BASES], haps->snv_mask_fwd, (size_t)hb);
+        std::memcpy(st.prior_f.p + at[HAP_BASES], haps->snv_prior_fwd, (size_t)hb);
+        std::memcpy(st.mask_r.p + at[HAP_BASES], haps->snv_mask_rev, (size_t)hb);
+        std::memcpy(st.prior_r.p + at[HAP_BASES], haps->snv_prior_rev, (size_t)hb);
+        std::memcpy(st.gap_open.p + at[HAP_BASES], haps->gap_open, (size_t)hb);
+        std::memcpy(st.gap_extend.p + at[HAP_BASES], haps->gap_extend, (size_t)hb);
+        if (at[READS] == 0) st.read_off.p[0] = 0;
+        for (int r = 0; r < R; ++r) st.read_off.p[at[READS] + r + 1] = at[READ_BASES] + reads->off[r + 1];
+        if (reads->begin) std::memcpy(st.read_begin.p + at[READS], reads->begin, (size_t)R * sizeof(int64_t));
+        else std::memset(st.read_begin.p + at[READS], 0, (size_t)R * sizeof(int64_t));
+        std::memcpy(st.bases.p + at[READ_BASES], reads->bases, (size_t)rb);
+        std::memcpy(st.quals.p + at[READ_BASES], reads->quals, (size_t)rb);
+        std::memcpy(st.mapq.p + at[READS], reads->mapq, (size_t)R);
+        std::memcpy(st.reverse.p + at[READS], reads->reverse, (size_t)R);
+    }
+
+    // the leader's call: the batch's members as the regions of one phmm_populate_regions call
+    int run(phmm_engine* e, Staging& st, const Sizes& used) const
+    {
+        const phmm_haplotypes hv {(int32_t)used[HAPS], st.hap_off.p, st.seq.p, st.mask_f.p, st.prior_f.p, st.mask_r.p, st.prior_r.p,
+                                  st.gap_open.p, st.gap_extend.p, st.hap_begin.p};
+        const phmm_reads rv {(int32_t)used[READS], st.read_off.p, st.bases.p, st.quals.p, st.mapq.p, st.reverse.p, st.read_begin.p};
+        const phmm_regions regions {(int32_t)flanks.size(), hap_first.data(), read_first.data(), flanks.data()};
+        return phmm_populate_regions(e, &cfg, &hv, &rv, &regions, st.out.p, st.status.p, PHMM_SPACE_HOST);
+    }
+
+    // this member's slice of the call's result, [H][R] at the pair offset of its region
+    static int copy_out(const Staging& st, const Sizes& at, const Request& q, int rc, const std::string& err)
+    {
+        if (rc != PHMM_OK && rc != PHMM_ERR_SHORT_HAPLOTYPE) { t_error = err; return rc; }
+        const int H = q.haps->n, R = q.reads->n;
+        const double* res = st.out.p + at[PAIRS];
+        const int32_t* res_status = st.status.p + at[PAIRS];
+        rc = PHMM_OK;
+        for (long long i = 0; i < q.need[PAIRS]; ++i) if ((res_status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) { rc = PHMM_ERR_SHORT_HAPLOTYPE; break; }
+        t_error = rc == PHMM_OK ? std::string() : std::string("Haplotype is too short for alignment");
+        if (q.status) std::memcpy(q.status, res_status, (size_t)q.need[PAIRS] * sizeof(int32_t));
+        if (q.template_off) {
+            // k_template_sum's order: each template's reads left to right from 0.0
+            for (int h = 0; h < H; ++h) {
+                for (int t = 0; t < q.n_templates; ++t) {
+                    double acc = 0.0;
+                    for (long long r = q.template_off[t]; r < q.template_off[t + 1]; ++r) acc += res[(size_t)h * R + r];
+                    q.out[(size_t)h * q.n_templates + t] = acc;
+                }
+            }
+        } else {
+            std::memcpy(q.out, res, (size_t)q.need[PAIRS] * sizeof(double));
+        }
+        return rc;
+    }
+};
+
+// Mutation-prime requests: a batch is one phmm_mutation_prime_sets call and each member one of its sets; models equal by content
+// (phmm_mutation_model::key) merge.
+struct MutationPrime {
+    enum { HAPS, BASES, PAIRS, N_COUNTS };
+    using Sizes = Counts<N_COUNTS>;
+
+    struct Request {
+        const phmm_mutation_model* m; int32_t n; const int64_t* off; const char* seq; double* out; int32_t* status;
+        Sizes need;
+    };
+
+    // One batch's page-locked copy of its members' haplotypes and its results.
+    struct Staging {
+        Pinned<int64_t> off;
+        Pinned<char> seq;
+        Pinned<double> out;
+        Pinned<int32_t> status;
+        Sizes cap;
+        bool busy = false;
+
+        bool grow(const Sizes& s)
+        {
+            if (!(off.ensure(s[HAPS] + 1) && seq.ensure(s[BASES]) && out.ensure(s[PAIRS]) && status.ensure(s[PAIRS]))) return false;
+            cap[HAPS] = off.cap - 1; cap[BASES] = seq.cap; cap[PAIRS] = std::min(out.cap, status.cap);
+            return true;
+        }
+    };
+
+    // first staging size: some tens of mutation sets of 50 haplotypes
+    static Sizes initial_staging() { return {{2048, 1LL << 20, 1LL << 17}}; }
+    static bool within_limits(const Sizes& s) { return s[PAIRS] <= PHMM_MUT_MAX_PAIRS; }
+    static std::string key(const Request& q) { return q.m->key; }
+
+    const phmm_mutation_model* model;     // the leader's model (the members' are equal by content)
     std::vector<int32_t> set_first {0};
+
+    explicit MutationPrime(const Request& q) : model(q.m) {}
+
+    void add(const Request&, const Sizes& used) { set_first.push_back((int32_t)used[HAPS]); }
+
+    static void copy_in(Staging& st, const Sizes& at, const Request& q)
+    {
+        if (at[HAPS] == 0) st.off.p[0] = 0;
+        for (int h = 0; h < q.n; ++h) st.off.p[at[HAPS] + h + 1] = at[BASES] + q.off[h + 1];
+        std::memcpy(st.seq.p + at[BASES], q.seq, (size_t)q.need[BASES]);
+    }
+
+    int run(phmm_engine* e, Staging& st, const Sizes&) const
+    {
+        return phmm_mutation_prime_sets(e, model, (int32_t)set_first.size() - 1, set_first.data(), st.off.p, st.seq.p, st.out.p, st.status.p);
+    }
+
+    // this member's n x n matrix at the pair offset of its set
+    static int copy_out(const Staging& st, const Sizes& at, const Request& q, int rc, const std::string& err)
+    {
+        if (rc != PHMM_OK) { t_error = err; return rc; }
+        std::memcpy(q.out, st.out.p + at[PAIRS], (size_t)q.need[PAIRS] * sizeof(double));
+        std::memcpy(q.status, st.status.p + at[PAIRS], (size_t)q.need[PAIRS] * sizeof(int32_t));
+        t_error.clear();
+        return PHMM_OK;
+    }
+};
+
+// A batch of one kind's requests: the kind's own data and the shared life cycle.
+template <typename Kind>
+struct Batch {
+    Batch(const typename Kind::Request& q, std::string k, typename Kind::Staging* s, Clock::time_point d)
+        : kind(q), key(std::move(k)), st(s), deadline(d) {}
+    Kind kind;
+    std::string key;
+    typename Kind::Staging* st;
+    typename Kind::Sizes used;
     Clock::time_point deadline;
     int members = 0;
     int pending_copies = 0;     // members that reserved space and have not finished copying in
@@ -144,9 +273,13 @@ struct Batch {
     std::string err;
 };
 
-std::string config_key(const phmm_config* cfg) { return std::string(reinterpret_cast<const char*>(cfg), sizeof(phmm_config)); }
-// never the length of a config key (the model key alone is longer), so the two kinds share one map of open batches
-std::string model_key(const phmm_mutation_model* m) { return "mutation model " + m->key; }
+// One kind's open batches (one per merge key), its staging pool and the pool's high-water mark: what merged batches have asked for.
+template <typename Kind>
+struct Lane {
+    std::map<std::string, Batch<Kind>*> open;
+    std::vector<std::unique_ptr<typename Kind::Staging>> staging;
+    typename Kind::Sizes want = Kind::initial_staging();
+};
 
 } // namespace
 
@@ -156,11 +289,8 @@ struct phmm_batcher {
     int max_wait_us = kDefaultMaxWaitUs;
     mutable std::mutex m;
     std::condition_variable cv;
-    std::map<std::string, Batch*> open;               // the open batch of each distinct config or mutation model
-    std::vector<std::unique_ptr<Staging>> staging;
-    Sizes want;                                       // staging high-water mark: what merged batches have asked for
-    std::vector<std::unique_ptr<MutationStaging>> mutation_staging;
-    MutationSizes mutation_want;
+    Lane<Populate> populate;
+    Lane<MutationPrime> mutation;
     bool engine_busy = false;
     int waiting = 0;                                  // requests in batches not yet sent + requests running alone
     int in_flight = 0;                                // requests inside the batcher
@@ -199,78 +329,124 @@ int run_alone(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* ha
     return rc;
 }
 
-// A free staging set of `pool`, large enough for `need` (grown to the high-water mark `want`) and marked busy; nullptr when out of memory.
-template <typename S, typename N>
-S* free_staging(std::vector<std::unique_ptr<S>>& pool, const N& need, const N& want)
+// A free staging set of the lane's pool, large enough for `need` (grown to the high-water mark) and marked busy; nullptr when out
+// of memory.
+template <typename Kind>
+typename Kind::Staging* free_staging(Lane<Kind>& lane, const typename Kind::Sizes& need)
 {
-    S* st = nullptr;
-    for (auto& s : pool) if (!s->busy) { st = s.get(); break; }
-    if (!st) { pool.emplace_back(new S()); st = pool.back().get(); }
-    if (!st->grow(N::max(need, want))) return nullptr;
+    typename Kind::Staging* st = nullptr;
+    for (auto& s : lane.staging) if (!s->busy) { st = s.get(); break; }
+    if (!st) { lane.staging.emplace_back(new typename Kind::Staging()); st = lane.staging.back().get(); }
+    const typename Kind::Sizes size = Kind::Sizes::max(need, lane.want);
+    if (!size.within(st->cap) && !st->grow(size)) return nullptr;
     st->busy = true;
     return st;
 }
 
-// A new open batch for `key`, sent at the latest max_wait_us from now.
-Batch* open_batch(phmm_batcher* b, const std::string& key)
-{
-    Batch* bt = new Batch();
-    bt->key = key;
-    bt->deadline = Clock::now() + std::chrono::microseconds(b->max_wait_us);
-    b->open[key] = bt;
-    return bt;
-}
-
-void close_batch(phmm_batcher* b, Batch* bt)
+template <typename Kind>
+void close_batch(Lane<Kind>& lane, Batch<Kind>* bt)
 {
     if (!bt->open) return;
     bt->open = false;
-    const auto it = b->open.find(bt->key);
-    if (it != b->open.end() && it->second == bt) b->open.erase(it);
+    const auto it = lane.open.find(bt->key);
+    if (it != lane.open.end() && it->second == bt) lane.open.erase(it);
 }
 
-// Copy one request into its reserved slot of the staging (outside the lock: each member writes its own ranges only).
-void copy_in(Staging* st, const Sizes& at, const phmm_haplotypes* haps, const phmm_reads* reads)
+// Under the lock: the batch the request joins, with its slot at *at reserved. That is the open batch of the request's merge key if
+// the request fits it (the kind's limits and the batch's staging); a batch it does not fit is marked full and closed (when only
+// the staging was too small, the high-water mark rises), and a new batch with a free staging set, sent at the latest max_wait_us
+// from now, takes the request. nullptr when out of page-locked memory.
+template <typename Kind>
+Batch<Kind>* join(phmm_batcher* b, Lane<Kind>& lane, const std::string& key, const typename Kind::Request& q, typename Kind::Sizes* at)
 {
-    const int H = haps->n, R = reads->n;
-    const long long hb = haps->off[H], rb = reads->off[R];
-    if (at.haps == 0) st->hap_off.p[0] = 0;
-    for (int h = 0; h < H; ++h) st->hap_off.p[at.haps + h + 1] = at.hap_bases + haps->off[h + 1];
-    if (haps->begin) std::memcpy(st->hap_begin.p + at.haps, haps->begin, (size_t)H * sizeof(int64_t));
-    else std::memset(st->hap_begin.p + at.haps, 0, (size_t)H * sizeof(int64_t));
-    std::memcpy(st->seq.p + at.hap_bases, haps->seq, (size_t)hb);
-    std::memcpy(st->mask_f.p + at.hap_bases, haps->snv_mask_fwd, (size_t)hb);
-    std::memcpy(st->prior_f.p + at.hap_bases, haps->snv_prior_fwd, (size_t)hb);
-    std::memcpy(st->mask_r.p + at.hap_bases, haps->snv_mask_rev, (size_t)hb);
-    std::memcpy(st->prior_r.p + at.hap_bases, haps->snv_prior_rev, (size_t)hb);
-    std::memcpy(st->gap_open.p + at.hap_bases, haps->gap_open, (size_t)hb);
-    std::memcpy(st->gap_extend.p + at.hap_bases, haps->gap_extend, (size_t)hb);
-    if (at.reads == 0) st->read_off.p[0] = 0;
-    for (int r = 0; r < R; ++r) st->read_off.p[at.reads + r + 1] = at.read_bases + reads->off[r + 1];
-    if (reads->begin) std::memcpy(st->read_begin.p + at.reads, reads->begin, (size_t)R * sizeof(int64_t));
-    else std::memset(st->read_begin.p + at.reads, 0, (size_t)R * sizeof(int64_t));
-    std::memcpy(st->bases.p + at.read_bases, reads->bases, (size_t)rb);
-    std::memcpy(st->quals.p + at.read_bases, reads->quals, (size_t)rb);
-    std::memcpy(st->mapq.p + at.reads, reads->mapq, (size_t)R);
-    std::memcpy(st->reverse.p + at.reads, reads->reverse, (size_t)R);
+    Batch<Kind>* bt = nullptr;
+    for (;;) {
+        const auto it = lane.open.find(key);
+        if (it == lane.open.end()) {
+            typename Kind::Staging* st = free_staging(lane, q.need);
+            if (!st) return nullptr;
+            bt = new Batch<Kind>(q, key, st, Clock::now() + std::chrono::microseconds(b->max_wait_us));
+            lane.open[key] = bt;
+            break;
+        }
+        bt = it->second;
+        typename Kind::Sizes total = bt->used;
+        total += q.need;
+        const bool limits = Kind::within_limits(total);
+        if (limits && total.within(bt->st->cap)) break;
+        if (limits) lane.want = Kind::Sizes::max(lane.want, total);   // staging too small
+        bt->full = true;
+        close_batch(lane, bt);
+        b->cv.notify_all();
+    }
+    *at = bt->used;
+    bt->used += q.need;
+    bt->kind.add(q, bt->used);
+    return bt;
 }
 
-// The leader's call: the batch's members as the regions of one phmm_populate_regions call.
-void run_batch(phmm_batcher* b, Batch* bt)
+// The life of a request in a batch, the same for every kind: it joins a batch under the lock, then copies itself into its slot of
+// the staging outside the lock (each member its own ranges). The first member leads: it waits until `clients` requests wait, the
+// batch is full or its deadline has passed, and the engine is free, then seals the batch and makes the kind's call; the others
+// wait for it. Each member copies its own slice out (outside the lock) and returns its code; the last reader frees the staging
+// and the batch.
+template <typename Kind>
+int take_part(phmm_batcher* b, Lane<Kind>& lane, const typename Kind::Request& q)
 {
-    Staging* st = bt->st;
-    const phmm_haplotypes hv {(int32_t)bt->used.haps, st->hap_off.p, st->seq.p, st->mask_f.p, st->prior_f.p, st->mask_r.p, st->prior_r.p,
-                              st->gap_open.p, st->gap_extend.p, st->hap_begin.p};
-    const phmm_reads rv {(int32_t)bt->used.reads, st->read_off.p, st->bases.p, st->quals.p, st->mapq.p, st->reverse.p, st->read_begin.p};
-    const phmm_regions regions {bt->members, bt->hap_first.data(), bt->read_first.data(), bt->flanks.data()};
-    bt->rc = phmm_populate_regions(b->engine, &bt->cfg, &hv, &rv, &regions, st->out.p, st->status.p, PHMM_SPACE_HOST);
-    if (bt->rc != PHMM_OK) bt->err = phmm_last_error(b->engine);
+    const std::string key = Kind::key(q);
+    std::unique_lock<std::mutex> lk(b->m);
+    typename Kind::Sizes at;
+    Batch<Kind>* bt = join(b, lane, key, q, &at);
+    if (!bt) { t_error = "out of page-locked host memory for the batch staging"; return PHMM_ERR_NOMEM; }
+    const bool leader = bt->members == 0;
+    ++bt->members; ++bt->pending_copies; ++bt->readers; ++b->waiting;
+    b->cv.notify_all();
+    lk.unlock();
+
+    Kind::copy_in(*bt->st, at, q);
+
+    lk.lock();
+    --bt->pending_copies;
+    if (leader) {
+        for (;;) {
+            const bool company = b->clients > 0 && b->waiting >= b->clients;
+            const bool go = bt->full || company || Clock::now() >= bt->deadline;
+            if (go && !b->engine_busy) break;
+            if (go) b->cv.wait(lk);
+            else b->cv.wait_until(lk, bt->deadline);
+        }
+        close_batch(lane, bt);
+        b->engine_busy = true;
+        b->waiting -= bt->members;
+        b->cv.wait(lk, [&] { return bt->pending_copies == 0; });
+        lk.unlock();
+        bt->rc = bt->kind.run(b->engine, *bt->st, bt->used);
+        if (bt->rc != PHMM_OK) bt->err = phmm_last_error(b->engine);
+        lk.lock();
+        count_call(b, bt->members);
+        b->engine_busy = false;
+        bt->done = true;
+        b->cv.notify_all();
+    } else {
+        b->cv.notify_all();                       // the leader may be waiting for this copy
+        b->cv.wait(lk, [&] { return bt->done; });
+    }
+    lk.unlock();
+
+    const int rc = Kind::copy_out(*bt->st, at, q, bt->rc, bt->err);
+
+    lk.lock();
+    if (--bt->readers == 0) {
+        bt->st->busy = false;
+        delete bt;
+    }
+    return rc;
 }
 
 // The host-side checks of phmm_populate, in its order, for a request without position lists. Sets *alone when the request has to
 // run on its own (pipelined size, too many haplotypes, a haplotype too long for the task word); the remaining checks are then
 // phmm_populate's own.
-int check_request(const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads, const double* out, bool* alone, Sizes* need)
+int check_request(const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads, const double* out, bool* alone, Populate::Sizes* need)
 {
     int rc;
     if ((rc = phmm_checks::config_and_output(cfg, out, reads, t_error)) != PHMM_OK) return rc;
@@ -286,184 +462,21 @@ int check_request(const phmm_config* cfg, const phmm_haplotypes* haps, const phm
     if (cfg->map_positions && (rc = phmm_checks::mapper_haplotypes(max_hap, hap_bases, t_error)) != PHMM_OK) return rc;
     if (max_hap > 65535) { *alone = true; return PHMM_OK; }
     if ((rc = phmm_checks::penalties(haps, hap_bases, t_error)) != PHMM_OK) return rc;
-    need->haps = haps->n; need->hap_bases = hap_bases; need->reads = reads->n; need->read_bases = read_bases; need->pairs = pairs;
+    *need = {{haps->n, hap_bases, reads->n, read_bases, pairs}};
     return PHMM_OK;
-}
-
-// The life of a request in a batch, the same for every kind. Entered under the lock once the request has reserved its slot in bt:
-// copy_in() writes the request into the staging outside the lock (each member its own ranges); the first member leads: it waits
-// until `clients` requests wait, the batch is full or its deadline has passed, and the engine is free, then seals the batch and
-// makes the call run(b, bt); the others wait for it. copy_out() (outside the lock) reads this member's slice and returns its code;
-// the last reader frees the staging and the batch.
-template <typename CopyIn, typename CopyOut>
-int take_part(phmm_batcher* b, std::unique_lock<std::mutex>& lk, Batch* bt, CopyIn copy_in, void (*run)(phmm_batcher*, Batch*), CopyOut copy_out)
-{
-    const bool leader = bt->members == 0;
-    ++bt->members; ++bt->pending_copies; ++bt->readers; ++b->waiting;
-    b->cv.notify_all();
-    lk.unlock();
-
-    copy_in();
-
-    lk.lock();
-    --bt->pending_copies;
-    if (leader) {
-        for (;;) {
-            const bool company = b->clients > 0 && b->waiting >= b->clients;
-            const bool go = bt->full || company || Clock::now() >= bt->deadline;
-            if (go && !b->engine_busy) break;
-            if (go) b->cv.wait(lk);
-            else b->cv.wait_until(lk, bt->deadline);
-        }
-        close_batch(b, bt);
-        b->engine_busy = true;
-        b->waiting -= bt->members;
-        b->cv.wait(lk, [&] { return bt->pending_copies == 0; });
-        lk.unlock();
-        run(b, bt);
-        lk.lock();
-        count_call(b, bt->members);
-        b->engine_busy = false;
-        bt->done = true;
-        b->cv.notify_all();
-    } else {
-        b->cv.notify_all();                       // the leader may be waiting for this copy
-        b->cv.wait(lk, [&] { return bt->done; });
-    }
-    lk.unlock();
-
-    const int rc = copy_out();
-
-    lk.lock();
-    if (--bt->readers == 0) {
-        if (bt->st) bt->st->busy = false;
-        if (bt->ms) bt->ms->busy = false;
-        delete bt;
-    }
-    return rc;
 }
 
 int submit(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_positions* positions,
            const int64_t* template_off, int32_t n_templates, const phmm_flank_state* flank, double* out, int32_t* status)
 {
     bool alone = positions && positions->off && positions->pos;
-    Sizes need;
+    Populate::Request q {cfg, haps, reads, template_off, n_templates, flank, out, status, {}};
     if (!alone) {
-        const int rc = check_request(cfg, haps, reads, out, &alone, &need);
+        const int rc = check_request(cfg, haps, reads, out, &alone, &q.need);
         if (rc != PHMM_OK) return rc;
     }
     if (alone) return run_alone(b, cfg, haps, reads, positions, template_off, n_templates, flank, out, status);
-
-    const std::string key = config_key(cfg);
-    std::unique_lock<std::mutex> lk(b->m);
-    Batch* bt = nullptr;
-    for (;;) {
-        const auto it = b->open.find(key);
-        if (it == b->open.end()) {
-            Staging* st = free_staging(b->staging, need, b->want);
-            if (!st) { t_error = "out of page-locked host memory for the batch staging"; return PHMM_ERR_NOMEM; }
-            bt = open_batch(b, key);
-            bt->cfg = *cfg;
-            bt->st = st;
-            break;
-        }
-        bt = it->second;
-        Sizes total = bt->used;
-        total += need;
-        if (total.haps <= kMaxBatchHaps && total.pairs <= kMaxBatchPairs && total.within(bt->st->cap)) break;
-        if (total.haps <= kMaxBatchHaps && total.pairs <= kMaxBatchPairs) b->want = Sizes::max(b->want, total);   // staging too small
-        bt->full = true;
-        close_batch(b, bt);
-        b->cv.notify_all();
-    }
-    const Sizes at = bt->used;
-    bt->used += need;
-    bt->hap_first.push_back((int32_t)bt->used.haps);
-    bt->read_first.push_back((int32_t)bt->used.reads);
-    bt->flanks.push_back(flank ? *flank : phmm_flank_state {0, 0, 0});
-    return take_part(b, lk, bt, [&] { copy_in(bt->st, at, haps, reads); }, run_batch, [&] {
-        // this member's slice of the result: [H][R] at the pair offset of its region
-        int rc = bt->rc;
-        const int H = haps->n, R = reads->n;
-        const double* res = bt->st->out.p + at.pairs;
-        const int32_t* res_status = bt->st->status.p + at.pairs;
-        if (rc == PHMM_OK || rc == PHMM_ERR_SHORT_HAPLOTYPE) {
-            rc = PHMM_OK;
-            for (long long i = 0; i < need.pairs; ++i) if ((res_status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) { rc = PHMM_ERR_SHORT_HAPLOTYPE; break; }
-            t_error = rc == PHMM_OK ? std::string() : std::string("Haplotype is too short for alignment");
-            if (status) std::memcpy(status, res_status, (size_t)need.pairs * sizeof(int32_t));
-            if (template_off) {
-                // k_template_sum's order: each template's reads left to right from 0.0
-                for (int h = 0; h < H; ++h) {
-                    for (int t = 0; t < n_templates; ++t) {
-                        double acc = 0.0;
-                        for (long long r = template_off[t]; r < template_off[t + 1]; ++r) acc += res[(size_t)h * R + r];
-                        out[(size_t)h * n_templates + t] = acc;
-                    }
-                }
-            } else {
-                std::memcpy(out, res, (size_t)need.pairs * sizeof(double));
-            }
-        } else {
-            t_error = bt->err;
-        }
-        return rc;
-    });
-}
-
-// The leader's call: the batch's members as the sets of one phmm_mutation_prime_sets call.
-void run_mutation_batch(phmm_batcher* b, Batch* bt)
-{
-    MutationStaging* ms = bt->ms;
-    bt->rc = phmm_mutation_prime_sets(b->engine, bt->model, bt->members, bt->set_first.data(), ms->off.p, ms->seq.p, ms->out.p, ms->status.p);
-    if (bt->rc != PHMM_OK) bt->err = phmm_last_error(b->engine);
-}
-
-int submit_mutation(phmm_batcher* b, const phmm_mutation_model* m, int32_t n, const int64_t* off, const char* seq, double* out, int32_t* status)
-{
-    const int rc = phmm_checks::mutation_set(m, n, off, seq, out, status, t_error);
-    if (rc != PHMM_OK) return rc;
-    MutationSizes need;
-    need.haps = n; need.bases = off[n]; need.pairs = (long long)n * n;
-
-    const std::string key = model_key(m);
-    std::unique_lock<std::mutex> lk(b->m);
-    Batch* bt = nullptr;
-    for (;;) {
-        const auto it = b->open.find(key);
-        if (it == b->open.end()) {
-            MutationStaging* ms = free_staging(b->mutation_staging, need, b->mutation_want);
-            if (!ms) { t_error = "out of page-locked host memory for the batch staging"; return PHMM_ERR_NOMEM; }
-            bt = open_batch(b, key);
-            bt->model = m;
-            bt->ms = ms;
-            break;
-        }
-        bt = it->second;
-        MutationSizes total = bt->mused;
-        total += need;
-        if (total.pairs <= PHMM_MUT_MAX_PAIRS && total.within(bt->ms->cap)) break;
-        if (total.pairs <= PHMM_MUT_MAX_PAIRS) b->mutation_want = MutationSizes::max(b->mutation_want, total);   // staging too small
-        bt->full = true;
-        close_batch(b, bt);
-        b->cv.notify_all();
-    }
-    const MutationSizes at = bt->mused;
-    bt->mused += need;
-    bt->set_first.push_back((int32_t)bt->mused.haps);
-    return take_part(b, lk, bt, [&] {
-        MutationStaging* ms = bt->ms;
-        if (at.haps == 0) ms->off.p[0] = 0;
-        for (int h = 0; h < n; ++h) ms->off.p[at.haps + h + 1] = at.bases + off[h + 1];
-        std::memcpy(ms->seq.p + at.bases, seq, (size_t)need.bases);
-    }, run_mutation_batch, [&] {
-        // this member's n x n matrix at the pair offset of its set
-        if (bt->rc != PHMM_OK) { t_error = bt->err; return bt->rc; }
-        std::memcpy(out, bt->ms->out.p + at.pairs, (size_t)need.pairs * sizeof(double));
-        std::memcpy(status, bt->ms->status.p + at.pairs, (size_t)need.pairs * sizeof(int32_t));
-        t_error.clear();
-        return PHMM_OK;
-    });
+    return take_part(b, b->populate, q);
 }
 
 // Entry and exit of every request: destroy waits until no request is inside.
@@ -488,10 +501,6 @@ int phmm_batcher_create(phmm_batcher** out, int device, const phmm_batcher_optio
     phmm_batcher* b = new phmm_batcher();
     b->engine = e;
     if (opt) { b->clients = opt->clients; b->max_wait_us = opt->max_wait_us; }
-    // first staging size: some tens of regions of a few hundred reads; it grows to what merged batches ask for
-    b->want.haps = 4096; b->want.hap_bases = 1LL << 20; b->want.reads = 1LL << 16; b->want.read_bases = 8LL << 20; b->want.pairs = 1LL << 20;
-    // and some tens of mutation sets of 50 haplotypes
-    b->mutation_want.haps = 2048; b->mutation_want.bases = 1LL << 20; b->mutation_want.pairs = 1LL << 17;
     *out = b;
     return PHMM_OK;
 }
@@ -533,7 +542,10 @@ int phmm_batcher_mutation_prime(phmm_batcher* b, const phmm_mutation_model* m, i
 {
     if (!b) { t_error = "null batcher"; return PHMM_ERR_INVALID; }
     InFlight guard(b);
-    return submit_mutation(b, m, n, off, seq, out, status);
+    const int rc = phmm_checks::mutation_set(m, n, off, seq, out, status, t_error);
+    if (rc != PHMM_OK) return rc;
+    const MutationPrime::Request q {m, n, off, seq, out, status, {{n, off[n], (long long)n * n}}};
+    return take_part(b, b->mutation, q);
 }
 
 int phmm_batcher_stats_get(const phmm_batcher* b, phmm_batcher_stats* out)
