@@ -365,9 +365,9 @@ int phmm_genotype_likelihoods(phmm_engine* e, const double* lnl, int32_t n_haplo
 
 /* ---------------------------------------------------------------------------------------------------------------------
  * HaplotypeLikelihoodModel::reset (haplotype_likelihood_model.cpp:60-78): the per-haplotype penalty arrays of phmm_haplotypes
- * from the haplotype sequences, by the reference's error models — host C++ (octopus_b200/csrc/phmm_error_model.cpp), no GPU
- * needed, bit-identical to core/models/error/ (repeat_based_indel_error_model.cpp:67-83, repeat_based_snv_error_model.cpp:144-179)
- * including the exact output of the tandem-repeat finder they call (lib/tandem).
+ * from the haplotype sequences, by the reference's error models — on host threads (phmm_reset_haplotypes, no GPU needed) or on
+ * the GPU (phmm_engine_reset_haplotypes), both running the one core of octopus_b200/csrc/phmm_reset.cuh, bit-identical to
+ * core/models/error/ (repeat_based_indel_error_model.cpp:67-83, repeat_based_snv_error_model.cpp:144-179) including the exact output of the tandem-repeat finder they call (lib/tandem).
  * ------------------------------------------------------------------------------------------------------------------- */
 typedef struct phmm_error_model phmm_error_model;
 
@@ -387,6 +387,15 @@ const char* phmm_error_model_last_error(void);   /* thread-local message of the 
 int  phmm_reset_haplotypes(const phmm_error_model* m, int32_t n, const int64_t* off, const char* seq, const uint8_t* is_substitution,
                            char* snv_mask_fwd, int8_t* snv_prior_fwd, char* snv_mask_rev, int8_t* snv_prior_rev,
                            int8_t* gap_open, int8_t* gap_extend, int32_t n_threads);
+
+/* phmm_reset_haplotypes on the GPU: the same arguments, layout and output — all six arrays byte-identical to the host call — for
+ * arrays in `space` (off included). The arithmetic is the host call's own (phmm_reset.cuh), one haplotype per GPU thread; a haplotype
+ * whose tandem repeats overflow the device scratch is recomputed by the host before the call returns. PHMM_ERR_INVALID, with a message
+ * in phmm_last_error(e), for a null pointer, bad offsets (off[0] < 0, decreasing) or a haplotype longer than 65535 bases.
+ * n == 0 returns PHMM_OK without touching the GPU. phmm_last_dp_kernel_ms(e) then holds the reset kernel's time. */
+int  phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int32_t n, const int64_t* off, const char* seq,
+                                  const uint8_t* is_substitution, char* snv_mask_fwd, int8_t* snv_prior_fwd, char* snv_mask_rev,
+                                  int8_t* snv_prior_rev, int8_t* gap_open, int8_t* gap_extend, int space);
 
 /* tandem::extract_exact_tandem_repeats(seq, min_period, max_period) (lib/tandem/tandem.hpp:504-521): (pos, length, period) triples in
  * the library's output order. Returns the number of repeats (only the first cap are written), or a negative error code. */

@@ -562,15 +562,21 @@ class ErrorModel(_Handle):
             return n, out[:n]
         return _grow(attempt, 4 * len(s) + 16)
 
-    def reset(self, sequences, begin=None, is_substitution=None, n_threads=0):
+    def reset(self, sequences, begin=None, is_substitution=None, n_threads=0, engine=None):
         """HaplotypeLikelihoodModel::reset for every haplotype: sequences (list of str / bytes / uint8 arrays) → HaplotypeBlock
         with the SNV masks / priors and gap penalties the reference's models assign. ``is_substitution``: optional list of
-        per-base flag arrays (bases that are substitutions in Haplotype::cigar())."""
+        per-base flag arrays (bases that are substitutions in Haplotype::cigar()). ``engine``: a PairHMMEngine to compute them
+        on its GPU (byte-identical to the host threads)."""
         off, seq = pack_sequences(sequences)
         return self.reset_block(off, seq, begin, None if is_substitution is None else
-                                np.ascontiguousarray(np.concatenate([np.asarray(x, dtype=np.uint8) for x in is_substitution])), n_threads)
+                                np.ascontiguousarray(np.concatenate([np.asarray(x, dtype=np.uint8) for x in is_substitution])), n_threads,
+                                engine)
 
-    def reset_block(self, off, seq, begin=None, is_substitution=None, n_threads=0):
+    def reset_block(self, off, seq, begin=None, is_substitution=None, n_threads=0, engine=None):
+        """reset for a packed block (off[n + 1], seq). Without ``engine``: host threads, numpy in and out. With a PairHMMEngine: its
+        GPU computes the arrays; numpy inputs give a host block, CUDA torch tensors (off, seq, is_substitution) a device block."""
+        if engine is not None:
+            return self._reset_on(engine, off, seq, begin, is_substitution)
         off = np.ascontiguousarray(off, dtype=np.int64)
         seq = np.ascontiguousarray(seq, dtype=np.uint8)
         total = int(off[-1])
@@ -581,6 +587,19 @@ class ErrorModel(_Handle):
                                                     mf.ctypes.data, pf.ctypes.data, mr.ctypes.data, pr.ctypes.data, go.ctypes.data,
                                                     ge.ctypes.data, int(n_threads)))
         return HaplotypeBlock(off, seq, mf, pf, mr, pr, go, ge, begin)
+
+    def _reset_on(self, engine, off, seq, begin, is_substitution):
+        sp = _Space(seq.device if _is_torch(seq) else None)
+        off, seq = sp.input(off, np.int64), sp.input(seq, np.uint8)
+        sub = None if is_substitution is None else sp.input(is_substitution, np.uint8)
+        total = int(off[-1])
+        mf, mr = sp.empty(total, np.uint8), sp.empty(total, np.uint8)
+        pf, pr, go, ge = (sp.empty(total, np.int8) for _ in range(4))
+        engine._check(self._lib.phmm_engine_reset_haplotypes(engine._h, self._h, len(off) - 1, sp.ptr(off), sp.ptr(seq), sp.ptr(sub),
+                                                             sp.ptr(mf), sp.ptr(pf), sp.ptr(mr), sp.ptr(pr), sp.ptr(go), sp.ptr(ge), sp.flag))
+        if not sp.on_device:
+            return HaplotypeBlock(off, seq, mf, pf, mr, pr, go, ge, begin)
+        return HaplotypeBlock.of_device(off, seq, mf, pf, mr, pr, go, ge, begin)
 
 
 class HaplotypeLikelihoodModel:

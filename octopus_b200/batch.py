@@ -94,6 +94,19 @@ class HaplotypeBlock(_Block):
         for f in self._fields[1:8]:
             assert len(getattr(self, f)) == total, f
 
+    @classmethod
+    def of_device(cls, off, seq, snv_mask_fwd, snv_prior_fwd, snv_mask_rev, snv_prior_rev, gap_open, gap_extend, begin=None):
+        """A block over torch CUDA tensors as they are (begin: host array or None, copied to the tensors' device)."""
+        import torch
+        out = object.__new__(cls)
+        out.n = len(off) - 1
+        out.off, out.seq = off, seq
+        out.snv_mask_fwd, out.snv_prior_fwd, out.snv_mask_rev, out.snv_prior_rev = snv_mask_fwd, snv_prior_fwd, snv_mask_rev, snv_prior_rev
+        out.gap_open, out.gap_extend = gap_open, gap_extend
+        out.begin = None if begin is None else torch.as_tensor(np.ascontiguousarray(begin, dtype=np.int64), device=seq.device)
+        out.on_device = True
+        return out
+
     def c_struct(self):
         s = _lib.Haplotypes()
         s.n = self.n

@@ -412,6 +412,16 @@ struct HaplotypeBlock   // what HaplotypeLikelihoodModel::reset derives per hapl
                                              gap_open.data(), gap_extend.data(), n_threads);
         if (rc != PHMM_OK) throw Error {rc, phmm_error_model_last_error()};
     }
+    // The same arrays, byte for byte, computed on the engine's GPU (phmm_engine_reset_haplotypes).
+    void reset(const ErrorModel& model, Engine& engine)
+    {
+        const std::size_t n = seq.size();
+        snv_mask_fwd.resize(n); snv_mask_rev.resize(n); snv_prior_fwd.resize(n); snv_prior_rev.resize(n); gap_open.resize(n); gap_extend.resize(n);
+        is_substitution.resize(n, 0);
+        engine.check(phmm_engine_reset_haplotypes(engine.get(), model.get(), static_cast<std::int32_t>(size()), off.data(), seq.data(),
+                                                  is_substitution.data(), snv_mask_fwd.data(), snv_prior_fwd.data(), snv_mask_rev.data(),
+                                                  snv_prior_rev.data(), gap_open.data(), gap_extend.data(), PHMM_SPACE_HOST));
+    }
 
     void add(const std::string& sequence, const std::vector<char>& fwd_mask, const std::vector<std::int8_t>& fwd_priors,
              const std::vector<char>& rev_mask, const std::vector<std::int8_t>& rev_priors,

@@ -75,6 +75,7 @@ struct phmm_engine {
     DBuf pm_best, pm_cnt, pm_inl, pm_part, pm_misc;   // the pair mapper's first pass (k_kmer_map_pairs) and its offset scan
     DBuf as_pairs, as_prior, as_top;                  // phmm_assign_reads: slot-ordered pair list, log priors, top sets
     DBuf mu_in, mu_list, mu_res, mu_cig, mu_out;      // phmm_mutation_prime: staged set, DP pair list, per-tile results, CIGARs, matrix
+    DBuf rs_sub, rs_model, rs_words, rs_runs, rs_flags;   // phmm_engine_reset_haplotypes: flags, model tables, scratch slots, overflow
     std::vector<cudaEvent_t> tile_events;
     std::vector<int2> info_host;
     // per-kernel launch configuration already applied / queried (the runtime calls are not free and need not be repeated)
@@ -722,6 +723,136 @@ int phmm_genotype_likelihoods(phmm_engine* e, const double* lnl, int32_t H, int3
     CU(cudaGetLastError());
     if (space == PHMM_SPACE_HOST) CU(cudaMemcpyAsync(out, d_out, (size_t)G * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
+    return PHMM_OK;
+}
+
+// -------------------------------------------------------------------------------------------------------------
+// phmm_engine_reset_haplotypes
+// -------------------------------------------------------------------------------------------------------------
+// Device memory the scratch slots of one call may take: slots = min(haplotypes, budget / slot size, resident threads). The slots
+// are spread over at least kResetWarpsPerSm warps per SM (fewer working lanes per warp) before warps are filled.
+static constexpr size_t kResetScratchBudget = (size_t)1 << 30;
+static constexpr int kResetWarpsPerSm = 16;
+
+int phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int32_t n, const int64_t* off, const char* seq,
+                                 const uint8_t* is_substitution, char* snv_mask_fwd, int8_t* snv_prior_fwd, char* snv_mask_rev,
+                                 int8_t* snv_prior_rev, int8_t* gap_open, int8_t* gap_extend, int space)
+{
+    if (!e) return PHMM_ERR_INVALID;
+    e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
+    if (!m || n < 0 || (n > 0 && (!off || !seq || !snv_mask_fwd || !snv_prior_fwd || !snv_mask_rev || !snv_prior_rev || !gap_open || !gap_extend))) {
+        e->err = "null argument"; return PHMM_ERR_INVALID;
+    }
+    if (space != PHMM_SPACE_HOST && space != PHMM_SPACE_DEVICE) { e->err = "bad memory space"; return PHMM_ERR_INVALID; }
+    if (n == 0) return PHMM_OK;
+    if (int rc0 = begin_call(e)) return rc0;
+    int rc;
+    std::vector<long long> hoff;
+    if ((rc = fetch_offsets(e, off, n, space, hoff)) != PHMM_OK) return rc;
+    if (hoff[0] < 0) { e->err = "bad haplotype offsets"; return PHMM_ERR_INVALID; }
+    long long L = 0;
+    for (int h = 0; h < n; ++h) {
+        if (hoff[h + 1] < hoff[h]) { e->err = "bad haplotype offsets"; return PHMM_ERR_INVALID; }
+        L = std::max(L, hoff[h + 1] - hoff[h]);
+    }
+    if (L > 65535) { e->err = "haplotype longer than 65535 bases"; return PHMM_ERR_INVALID; }
+    // host space: the bases off[0] .. off[n] are staged and the outputs computed into engine buffers from index 0 = off[0]
+    const long long base = space == PHMM_SPACE_HOST ? hoff[0] : 0;
+    const size_t B = (size_t)(hoff[n] - hoff[0]);
+    const int64_t* d_off;
+    const char* d_seq; const uint8_t* d_sub;
+    if ((rc = stage(e, e->h_off, off, (size_t)n + 1, space, &d_off))) return rc;
+    if ((rc = stage(e, e->h_seq, space == PHMM_SPACE_HOST ? seq + base : seq, B, space, &d_seq))) return rc;
+    if ((rc = stage(e, e->rs_sub, is_substitution && space == PHMM_SPACE_HOST ? is_substitution + base : is_substitution, B, space, &d_sub))) return rc;
+    char *mf = snv_mask_fwd, *mr = snv_mask_rev;
+    int8_t *pf = snv_prior_fwd, *pr = snv_prior_rev, *go = gap_open, *ge = gap_extend;
+    if (space == PHMM_SPACE_HOST) {
+        DBuf* bufs[6] = {&e->h_mf, &e->h_pf, &e->h_mr, &e->h_pr, &e->h_go, &e->h_ge};
+        for (DBuf* b : bufs) CU(b->ensure(std::max<size_t>(B, 1)));
+        mf = e->h_mf.as<char>(); pf = e->h_pf.as<int8_t>(); mr = e->h_mr.as<char>(); pr = e->h_pr.as<int8_t>(); go = e->h_go.as<int8_t>(); ge = e->h_ge.as<int8_t>();
+    }
+    // the model: fixed rows travel in the kernel argument, a custom model's motif tables in one device block
+    phmm_reset::Model dm = phmm_reset::model_of(m);
+    if (dm.custom) {
+        const phmm_reset::MotifTable* t[2] = {&dm.custom_open, &dm.custom_extend};
+        size_t bytes = 0, at[2][3];
+        for (int i = 0; i < 2; ++i) {
+            at[i][0] = bytes; bytes += ((size_t)t[i]->n * sizeof(uint64_t) + 7) & ~(size_t)7;
+            at[i][1] = bytes; bytes += (((size_t)t[i]->n + 1) * sizeof(uint32_t) + 7) & ~(size_t)7;
+            at[i][2] = bytes; bytes += ((t[i]->n > 0 ? (size_t)t[i]->row[t[i]->n] : 0) + 7) & ~(size_t)7;
+        }
+        std::vector<char> blob(std::max<size_t>(bytes, 8), 0);
+        CU(e->rs_model.ensure(blob.size()));
+        phmm_reset::MotifTable* dt[2] = {&dm.custom_open, &dm.custom_extend};
+        for (int i = 0; i < 2; ++i) {
+            const phmm_reset::MotifTable src = *t[i];
+            if (src.n > 0) {
+                std::memcpy(blob.data() + at[i][0], src.key, (size_t)src.n * sizeof(uint64_t));
+                std::memcpy(blob.data() + at[i][1], src.row, ((size_t)src.n + 1) * sizeof(uint32_t));
+                std::memcpy(blob.data() + at[i][2], src.data, src.row[src.n]);
+            }
+            dt[i]->key = (const uint64_t*)(e->rs_model.as<char>() + at[i][0]);
+            dt[i]->row = (const uint32_t*)(e->rs_model.as<char>() + at[i][1]);
+            dt[i]->data = (const int8_t*)(e->rs_model.as<char>() + at[i][2]);
+        }
+        CU(cudaMemcpyAsync(e->rs_model.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, e->stream));
+    }
+    // scratch slots sized for the longest haplotype
+    const uint32_t cap = phmm_reset::first_cap((uint32_t)L);
+    const size_t slot_words = phmm_reset::scratch_words((uint32_t)L, cap);
+    const size_t slot_bytes = slot_words * sizeof(uint32_t) + 2 * (size_t)cap * sizeof(phmm_reset::Run);
+    const int resident = std::max(1, e->sm_count) * 2048;
+    const long long wanted = std::max<long long>(1, std::min<long long>({(long long)n, (long long)(kResetScratchBudget / slot_bytes), (long long)resident}));
+    const int lanes = (int)std::min<long long>(32, (wanted + (long long)std::max(1, e->sm_count) * kResetWarpsPerSm - 1) / ((long long)std::max(1, e->sm_count) * kResetWarpsPerSm));
+    const long long warps = (wanted + lanes - 1) / lanes;
+    const int slots = (int)(warps * lanes);
+    CU(e->rs_words.ensure((size_t)slots * slot_words * sizeof(uint32_t)));
+    CU(e->rs_runs.ensure((size_t)slots * 2 * cap * sizeof(phmm_reset::Run)));
+    CU(e->rs_flags.ensure((size_t)n));
+    CU(cudaEventRecord(e->ev0, e->stream));
+    k_reset_haplotypes<<<(unsigned)((warps + 3) / 4), 128, 0, e->stream>>>(dm, n, (const long long*)d_off, base, (const unsigned char*)d_seq, d_sub,
+                                                                        mf, pf, mr, pr, go, ge, e->rs_words.as<uint32_t>(),
+                                                                        e->rs_runs.as<phmm_reset::Run>(), slot_words, cap, lanes, slots,
+                                                                        e->rs_flags.as<uint8_t>());
+    LAUNCHED();
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(e->ev1, e->stream));
+    std::vector<uint8_t> overflow((size_t)n);
+    CU(cudaMemcpyAsync(overflow.data(), e->rs_flags.p, (size_t)n, cudaMemcpyDeviceToHost, e->stream));
+    if (space == PHMM_SPACE_HOST && B > 0) {
+        CU(cudaMemcpyAsync(snv_mask_fwd + base, mf, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(snv_prior_fwd + base, pf, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(snv_mask_rev + base, mr, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(snv_prior_rev + base, pr, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(gap_open + base, go, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(gap_extend + base, ge, B, cudaMemcpyDeviceToHost, e->stream));
+    }
+    CU(cudaStreamSynchronize(e->stream));
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, e->ev0, e->ev1) == cudaSuccess) e->last_dp_ms = ms;
+    // haplotypes whose runs overflowed their slot: the host core with a growing capacity, the same arithmetic
+    phmm_reset::HostScratch scratch;
+    const phmm_reset::Model& hm = phmm_reset::model_of(m);
+    std::vector<unsigned char> s, sub;
+    std::vector<int8_t> out;
+    for (int h = 0; h < n; ++h) {
+        if (!overflow[h]) continue;
+        const long long o = hoff[h];
+        const uint32_t len = (uint32_t)(hoff[h + 1] - o);
+        if (space == PHMM_SPACE_HOST) {
+            phmm_reset::reset_haplotype_host(hm, (const unsigned char*)seq + o, len, is_substitution ? is_substitution + o : nullptr, snv_mask_fwd + o,
+                                             snv_prior_fwd + o, snv_mask_rev + o, snv_prior_rev + o, gap_open + o, gap_extend + o, scratch);
+            continue;
+        }
+        s.resize(len); sub.resize(len); out.resize(6 * (size_t)len);
+        CU(cudaMemcpy(s.data(), seq + o, len, cudaMemcpyDeviceToHost));
+        if (is_substitution) CU(cudaMemcpy(sub.data(), is_substitution + o, len, cudaMemcpyDeviceToHost));
+        int8_t* a = out.data();
+        phmm_reset::reset_haplotype_host(hm, s.data(), len, is_substitution ? sub.data() : nullptr, (char*)a, a + len, (char*)a + 2 * len, a + 3 * len,
+                                         a + 4 * len, a + 5 * len, scratch);
+        void* dst[6] = {snv_mask_fwd + o, snv_prior_fwd + o, snv_mask_rev + o, snv_prior_rev + o, gap_open + o, gap_extend + o};
+        for (int k = 0; k < 6; ++k) CU(cudaMemcpy(dst[k], a + (size_t)k * len, len, cudaMemcpyHostToDevice));
+    }
     return PHMM_OK;
 }
 

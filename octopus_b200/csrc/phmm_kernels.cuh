@@ -2,6 +2,7 @@
 #pragma once
 
 #include "phmm_device.cuh"
+#include "phmm_reset.cuh"
 
 namespace phmm {
 
@@ -1948,4 +1949,32 @@ __global__ void k_mutation_rescore(const int n, const int2* __restrict__ list, c
     status[i] = st;
 }
 
+// -------------------------------------------------------------------------------------------------------------
+// HaplotypeLikelihoodModel::reset (phmm_engine_reset_haplotypes): phmm_reset.cuh's core, one haplotype per thread. The first `lanes`
+// lanes of every warp work: the core branches on the sequence, so lanes of one warp serialise, and a call with few haplotypes runs
+// faster spread over more warps (down to one lane each) than packed into few. Working thread t owns scratch slot t (slot_words
+// words, 2 cap runs) and takes haplotypes t, t + slots, ... A haplotype whose runs overflow the slot is flagged in overflow[h]; the
+// host recomputes it.
+// -------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) k_reset_haplotypes(const phmm_reset::Model m, const int n, const long long* __restrict__ off,
+                                                          const long long base, const unsigned char* __restrict__ seq,
+                                                          const uint8_t* __restrict__ is_substitution, char* mask_f, int8_t* prior_f,
+                                                          char* mask_r, int8_t* prior_r, int8_t* gap_open, int8_t* gap_extend,
+                                                          uint32_t* words, phmm_reset::Run* runs, const size_t slot_words,
+                                                          const uint32_t cap, const int lanes, const int slots, uint8_t* overflow)
+{
+    const int lane = (int)(threadIdx.x & 31);
+    const int slot = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * lanes + lane;
+    if (lane >= lanes || slot >= slots) return;
+    const phmm_reset::Scratch sc {words + (size_t)slot * slot_words, runs + (size_t)slot * 2 * cap, runs + (size_t)slot * 2 * cap + cap, cap};
+    for (int h = slot; h < n; h += slots) {
+        const long long o = off[h] - base;
+        const uint32_t len = (uint32_t)(off[h + 1] - off[h]);
+        const int rc = phmm_reset::reset_haplotype(m, seq + o, len, is_substitution ? is_substitution + o : nullptr, mask_f + o, prior_f + o,
+                                                   mask_r + o, prior_r + o, gap_open + o, gap_extend + o, sc);
+        overflow[h] = rc != phmm_reset::kOk;
+    }
+}
+
 } // namespace phmm
+
