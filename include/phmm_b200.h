@@ -397,6 +397,47 @@ int  phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int
                                   const uint8_t* is_substitution, char* snv_mask_fwd, int8_t* snv_prior_fwd, char* snv_mask_rev,
                                   int8_t* snv_prior_rev, int8_t* gap_open, int8_t* gap_extend, int space);
 
+/* Populate from haplotype SEQUENCES, as HaplotypeLikelihoodArray::populate does (haplotype_likelihood_array.cpp:77-95 runs
+ * likelihood_model_.reset(haplotype) itself): the caller passes the sequences and an error model, the engine derives the six per-base
+ * arrays of phmm_haplotypes on the GPU (the kernel of phmm_engine_reset_haplotypes) and runs the populate kernel chain on them in the
+ * same call. Only one byte per haplotype base (two with is_substitution) travels to the device. */
+typedef struct {
+    int32_t        n;
+    const int64_t* off;              /* [n+1] */
+    const char*    seq;              /* Haplotype::sequence() */
+    const uint8_t* is_substitution;  /* per base or NULL: as in phmm_reset_haplotypes */
+    const int64_t* begin;            /* [n] mapped_begin(haplotype), or NULL (= 0) */
+} phmm_haplotype_sequences;
+
+/* The _reset twins of the populate entry points. Contract: the return code, out at every PHMM_STATUS_OK pair and status are bit for
+ * bit those of phmm_reset_haplotypes (same model, sequences and flags) followed by the plain twin on the same inputs, for host and
+ * device space (every pointer of seqs in `space`, as the plain twin's). PHMM_ERR_INVALID, with a message in phmm_last_error(e), for a
+ * null model or sequence pointer, bad offsets (off[0] < 0, decreasing), a haplotype longer than 65535 bases (the device reset's
+ * limit) or a bad space; these follow the region / template argument checks and precede the plain twin's other checks.
+ * seqs->n == 0 behaves as the plain twin does.
+ * phmm_last_dp_kernel_ms / phmm_last_dp_cells keep their populate meaning: the reset kernel is not counted in them. A host-space
+ * call that the plain populate would pipeline computes the arrays once and then runs that pipeline. */
+int phmm_populate_reset(phmm_engine* e, const phmm_config* cfg, const phmm_error_model* m, const phmm_haplotype_sequences* seqs,
+                        const phmm_reads* reads, const phmm_positions* positions, const phmm_flank_state* flank,
+                        double* out, int32_t* status, int space);
+int phmm_populate_regions_reset(phmm_engine* e, const phmm_config* cfg, const phmm_error_model* m, const phmm_haplotype_sequences* seqs,
+                                const phmm_reads* reads, const phmm_regions* regions, double* out, int32_t* status, int space);
+int phmm_populate_templates_reset(phmm_engine* e, const phmm_config* cfg, const phmm_error_model* m, const phmm_haplotype_sequences* seqs,
+                                  const phmm_reads* reads, const int64_t* template_off, int32_t n_templates,
+                                  const phmm_positions* positions, const phmm_flank_state* flank, double* out, int32_t* status, int space);
+
+/* The same through a shared engine (the batcher contract above; host memory). Concurrent requests merge when their configs are equal
+ * and their error models are equal BY CONTENT (separately created models of one label or one custom text merge); requests under
+ * different models, and plain and reset requests, never share a call. A batch is one phmm_populate_regions_reset call. Requests with
+ * explicit positions, of pipelined size, with more than 65535 haplotypes, or whose model has a penalty outside [0,127], run alone
+ * through phmm_populate_reset. Every request is checked on its own thread with phmm_populate_reset's checks and messages. */
+int phmm_batcher_populate_reset(phmm_batcher* b, const phmm_config* cfg, const phmm_error_model* m, const phmm_haplotype_sequences* seqs,
+                                const phmm_reads* reads, const phmm_positions* positions, const phmm_flank_state* flank,
+                                double* out, int32_t* status);
+int phmm_batcher_populate_templates_reset(phmm_batcher* b, const phmm_config* cfg, const phmm_error_model* m,
+                                          const phmm_haplotype_sequences* seqs, const phmm_reads* reads, const int64_t* template_off,
+                                          int32_t n_templates, const phmm_flank_state* flank, double* out, int32_t* status);
+
 /* tandem::extract_exact_tandem_repeats(seq, min_period, max_period) (lib/tandem/tandem.hpp:504-521): (pos, length, period) triples in
  * the library's output order. Returns the number of repeats (only the first cap are written), or a negative error code. */
 int  phmm_tandem_repeats(const char* seq, int32_t n, int32_t min_period, int32_t max_period, uint32_t* out_triples, int32_t cap);

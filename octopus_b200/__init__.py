@@ -7,6 +7,6 @@ There is no CPU fallback: importing works anywhere, computing requires an H100.
 """
 from .api import (ErrorModel, HaplotypeLikelihoodArray, HaplotypeLikelihoodModel, MutationModel, PairHMMEngine, PhmmError,  # noqa: F401
                   PopulateBatcher, ShortHaplotypeError)
-from .batch import HaplotypeBlock, ReadBlock, pack_haplotypes, pack_reads  # noqa: F401
+from .batch import HaplotypeBlock, HaplotypeSequences, ReadBlock, pack_haplotypes, pack_reads  # noqa: F401
 
 __version__ = "0.1.0"

@@ -17,7 +17,8 @@ EXPORTS = ["phmm_version", "phmm_default_config", "phmm_create", "phmm_destroy",
            "phmm_mutation_prime", "phmm_mutation_prime_sets", "phmm_batcher_mutation_prime", "phmm_wait_event", "phmm_engine_stream", "phmm_reserve_sms", "phmm_host_alloc", "phmm_host_free",
            "phmm_populate_ld", "phmm_device_alloc", "phmm_device_free", "phmm_ipc_export", "phmm_ipc_open", "phmm_ipc_close",
            "phmm_batcher_create", "phmm_batcher_destroy", "phmm_batcher_last_error", "phmm_batcher_populate",
-           "phmm_batcher_populate_templates", "phmm_batcher_stats_get"]
+           "phmm_batcher_populate_templates", "phmm_batcher_stats_get", "phmm_populate_reset", "phmm_populate_regions_reset",
+           "phmm_populate_templates_reset", "phmm_batcher_populate_reset", "phmm_batcher_populate_templates_reset"]
 
 
 class Config(C.Structure):
@@ -31,6 +32,10 @@ class Haplotypes(C.Structure):
     _fields_ = [("n", C.c_int32), ("off", C.c_void_p), ("seq", C.c_void_p), ("snv_mask_fwd", C.c_void_p),
                 ("snv_prior_fwd", C.c_void_p), ("snv_mask_rev", C.c_void_p), ("snv_prior_rev", C.c_void_p),
                 ("gap_open", C.c_void_p), ("gap_extend", C.c_void_p), ("begin", C.c_void_p)]
+
+
+class HaplotypeSequences(C.Structure):
+    _fields_ = [("n", C.c_int32), ("off", C.c_void_p), ("seq", C.c_void_p), ("is_substitution", C.c_void_p), ("begin", C.c_void_p)]
 
 
 class Reads(C.Structure):
@@ -120,6 +125,23 @@ def load():
     lib.phmm_populate_templates.restype = C.c_int
     lib.phmm_populate_templates.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p, C.c_int32,
                                             C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_int]
+    lib.phmm_populate_reset.restype = C.c_int
+    lib.phmm_populate_reset.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.POINTER(HaplotypeSequences), C.POINTER(Reads),
+                                        C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_int]
+    lib.phmm_populate_regions_reset.restype = C.c_int
+    lib.phmm_populate_regions_reset.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.POINTER(HaplotypeSequences), C.POINTER(Reads),
+                                                C.POINTER(Regions), C.c_void_p, C.c_void_p, C.c_int]
+    lib.phmm_populate_templates_reset.restype = C.c_int
+    lib.phmm_populate_templates_reset.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.POINTER(HaplotypeSequences), C.POINTER(Reads),
+                                                  C.c_void_p, C.c_int32, C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_void_p,
+                                                  C.c_int]
+    lib.phmm_batcher_populate_reset.restype = C.c_int
+    lib.phmm_batcher_populate_reset.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.POINTER(HaplotypeSequences), C.POINTER(Reads),
+                                                C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_void_p]
+    lib.phmm_batcher_populate_templates_reset.restype = C.c_int
+    lib.phmm_batcher_populate_templates_reset.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.POINTER(HaplotypeSequences),
+                                                          C.POINTER(Reads), C.c_void_p, C.c_int32, C.POINTER(FlankState), C.c_void_p,
+                                                          C.c_void_p]
     lib.phmm_batcher_create.restype = C.c_int
     lib.phmm_batcher_create.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(BatcherOptions)]
     lib.phmm_batcher_destroy.argtypes = [C.c_void_p]

@@ -14,7 +14,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .batch import HaplotypeBlock, ReadBlock, _ptr, _u8, concat_reads, pack_sequences
+from .batch import HaplotypeBlock, HaplotypeSequences, ReadBlock, _ptr, _u8, concat_reads, pack_sequences
 
 
 class PhmmError(RuntimeError):
@@ -123,6 +123,22 @@ def _regions(hap_first, read_first, flank_states=None):
     regs = _lib.Regions(G, hf.ctypes.data, rf.ctypes.data, C.addressof(fl) if fl is not None else None)
     regs.arrays = hf, rf, fl
     return regs, off
+
+
+def _haps(haps, error_model):
+    """(haplotype block argument, model arguments): the plain call's HaplotypeBlock and (), or with an error model the _reset twin's
+    HaplotypeSequences and (model handle,)."""
+    if error_model is None:
+        return C.byref(haps.c_struct()), ()
+    if not isinstance(haps, HaplotypeSequences):
+        raise TypeError("with error_model, haps must be a HaplotypeSequences block")
+    return C.byref(haps.c_struct()), (error_model._h,)
+
+
+def _call(lib, name, handle, config, haps, error_model, *rest):
+    """lib.<name>(handle, config, haps, ...) or, with an error model, lib.<name>_reset(handle, config, model, sequences, ...)."""
+    hs, model = _haps(haps, error_model)
+    return getattr(lib, name + ("_reset" if model else ""))(handle, _config(config), *model, hs, *rest)
 
 
 def _mutation_set(sequences):
@@ -365,30 +381,32 @@ class PairHMMEngine(_Handle):
         return out
 
     # -- batch boundary ----------------------------------------------------------------------------------------
-    def populate_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, flank_state=None):
+    def populate_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, flank_state=None, error_model=None):
         """HaplotypeLikelihoodArray::populate(TemplateMap): host blocks; template t = reads [template_off[t], template_off[t+1]).
-        Returns the (H, T) matrix: each entry the sum of the template's reads' ln-likelihoods."""
+        Returns the (H, T) matrix: each entry the sum of the template's reads' ln-likelihoods. With ``error_model`` (an ErrorModel),
+        haps is a HaplotypeSequences block whose penalty arrays the GPU derives in the same call (phmm_populate_templates_reset)."""
         assert not haps.on_device and not reads.on_device
         toff = np.ascontiguousarray(template_off, dtype=np.int64)
         T = len(toff) - 1
         out = np.empty((haps.n, T), dtype=np.float64)
-        self._check(self._lib.phmm_populate_templates(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()),
-                                                      toff.ctypes.data, T, None, _ref(_flank(flank_state)), out.ctypes.data, None,
-                                                      _lib.SPACE_HOST))
+        self._check(_call(self._lib, "phmm_populate_templates", self._h, config, haps, error_model, C.byref(reads.c_struct()),
+                          toff.ctypes.data, T, None, _ref(_flank(flank_state)), out.ctypes.data, None, _lib.SPACE_HOST))
         return out
 
-    def populate_regions(self, config, haps: HaplotypeBlock, reads: ReadBlock, hap_first, read_first, flank_states=None, out=None, want_status=False):
+    def populate_regions(self, config, haps: HaplotypeBlock, reads: ReadBlock, hap_first, read_first, flank_states=None, out=None, want_status=False,
+                         error_model=None):
         """Many regions in one call (phmm_populate_regions): region g owns haplotypes [hap_first[g], hap_first[g+1]) and reads
         [read_first[g], read_first[g+1]). Returns the flat result vector (the regions' [H_g, R_g] matrices back to back) and the
-        per-region offsets into it; ``split_regions`` cuts it into matrices. flank_states: None or a list of (lhs, rhs) / None."""
+        per-region offsets into it; ``split_regions`` cuts it into matrices. flank_states: None or a list of (lhs, rhs) / None.
+        With ``error_model``, haps is a HaplotypeSequences block (phmm_populate_regions_reset)."""
         sp = _Space.of(haps, reads)
         regs, off = _regions(hap_first, read_first, flank_states)
         total = int(off[-1])
         if out is None:
             out = sp.empty(total, np.float64)
         status = sp.empty(total, np.int32) if want_status else None
-        self._check(self._lib.phmm_populate_regions(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()),
-                                                    C.byref(regs), sp.ptr(out), sp.ptr(status), sp.flag), want_status)
+        self._check(_call(self._lib, "phmm_populate_regions", self._h, config, haps, error_model, C.byref(reads.c_struct()), C.byref(regs),
+                          sp.ptr(out), sp.ptr(status), sp.flag), want_status)
         return (out, off, status) if want_status else (out, off)
 
     def assign_reads(self, config, haps: HaplotypeBlock, reads: ReadBlock, hap_first, read_first, log_priors=None, want_likelihoods=False,
@@ -426,18 +444,26 @@ class PairHMMEngine(_Handle):
                 for g in range(len(off) - 1)]
 
     def populate(self, config, haps: HaplotypeBlock, reads: ReadBlock, positions=None, flank_state=None, out=None,
-                 want_status=False):
+                 want_status=False, error_model=None):
         """Returns the (H, R) matrix of ln-likelihoods (numpy float64, or a torch CUDA tensor for device-resident blocks).
-        positions: None or (off[H*R+1] int64, pos int32) CSR in [H][R] order. flank_state: None or (lhs_flank, rhs_flank)."""
+        positions: None or (off[H*R+1] int64, pos int32) CSR in [H][R] order. flank_state: None or (lhs_flank, rhs_flank).
+        With ``error_model`` (an ErrorModel), haps is a HaplotypeSequences block: the GPU runs the model's reset() for every
+        haplotype in the same call (phmm_populate_reset), with the result of error_model.reset + populate."""
         sp = _Space.of(haps, reads)
         H, R = haps.n, reads.n
-        args = (self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), _ref(_positions(sp, positions)),
-                _ref(_flank(flank_state)))
         if out is None:
             out = sp.empty((H, R), np.float64)
         status = sp.empty((H, R), np.int32) if want_status else None
         if sp.on_device and (tuple(out.shape) != (H, R) or out.dtype != sp.dtype(np.float64) or (R > 1 and out.stride(1) != 1)):
             raise ValueError("out must be a float64 [H, R] tensor with unit column stride")
+        if error_model is not None:
+            if sp.on_device and H > 1 and out.stride(0) != R:
+                raise ValueError("populate with an error model writes a dense [H, R] matrix")
+            self._check(_call(self._lib, "phmm_populate", self._h, config, haps, error_model, C.byref(reads.c_struct()),
+                              _ref(_positions(sp, positions)), _ref(_flank(flank_state)), sp.ptr(out), sp.ptr(status), sp.flag), want_status)
+            return (out, status) if want_status else out
+        args = (self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), _ref(_positions(sp, positions)),
+                _ref(_flank(flank_state)))
         if sp.on_device and H > 1 and out.stride(0) != R:
             # a column window of a wider matrix — possibly another GPU's (octopus_b200.peer): phmm_populate_ld
             rc = self._lib.phmm_populate_ld(*args, sp.ptr(out), int(out.stride(0)), sp.ptr(status))
@@ -471,27 +497,29 @@ class PopulateBatcher(_Handle):
             raise PhmmError(rc, "stats")
         return {f: int(getattr(s, f)) for f, _ in _lib.BatcherStats._fields_}
 
-    def populate(self, config, haps: HaplotypeBlock, reads: ReadBlock, positions=None, flank_state=None, want_status=False):
-        """As PairHMMEngine.populate for host blocks: the (H, R) matrix (and the status matrix with want_status)."""
+    def populate(self, config, haps: HaplotypeBlock, reads: ReadBlock, positions=None, flank_state=None, want_status=False, error_model=None):
+        """As PairHMMEngine.populate for host blocks: the (H, R) matrix (and the status matrix with want_status). With
+        ``error_model``, haps is a HaplotypeSequences block (phmm_batcher_populate_reset): concurrent requests under models equal by
+        content run as one call that derives their penalty arrays on the GPU."""
         assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
         H, R = haps.n, reads.n
         out = _HOST.empty((H, R), np.float64)
         status = _HOST.empty((H, R), np.int32) if want_status else None
-        self._check(self._lib.phmm_batcher_populate(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()),
-                                                    _ref(_positions(_HOST, positions)), _ref(_flank(flank_state)), _ptr(out), _ptr(status)),
-                    want_status)
+        self._check(_call(self._lib, "phmm_batcher_populate", self._h, config, haps, error_model, C.byref(reads.c_struct()),
+                          _ref(_positions(_HOST, positions)), _ref(_flank(flank_state)), _ptr(out), _ptr(status)), want_status)
         return (out, status) if want_status else out
 
-    def populate_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, flank_state=None, want_status=False):
-        """As PairHMMEngine.populate_templates: the (H, T) matrix (and the per-read (H, R) status matrix with want_status)."""
+    def populate_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, flank_state=None, want_status=False,
+                           error_model=None):
+        """As PairHMMEngine.populate_templates: the (H, T) matrix (and the per-read (H, R) status matrix with want_status). With
+        ``error_model``, haps is a HaplotypeSequences block (phmm_batcher_populate_templates_reset)."""
         assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
         toff = np.ascontiguousarray(template_off, dtype=np.int64)
         T = len(toff) - 1
         out = _HOST.empty((haps.n, T), np.float64)
         status = _HOST.empty((haps.n, reads.n), np.int32) if want_status else None
-        self._check(self._lib.phmm_batcher_populate_templates(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()),
-                                                              toff.ctypes.data, T, _ref(_flank(flank_state)), _ptr(out), _ptr(status)),
-                    want_status)
+        self._check(_call(self._lib, "phmm_batcher_populate_templates", self._h, config, haps, error_model, C.byref(reads.c_struct()),
+                          toff.ctypes.data, T, _ref(_flank(flank_state)), _ptr(out), _ptr(status)), want_status)
         return (out, status) if want_status else out
 
     def mutation_prime(self, model, sequences):
@@ -649,9 +677,10 @@ class HaplotypeLikelihoodArray:
     mapperKmerSize = 6          # haplotype_likelihood_array.hpp:103
     maxMappingPositions = 10    # :104
 
-    def __init__(self, likelihood_model=None, engine=None):
+    def __init__(self, likelihood_model=None, engine=None, error_model=None):
         self.likelihood_model = likelihood_model or HaplotypeLikelihoodModel()
         self._engine = engine
+        self.error_model = error_model    # an ErrorModel: populate takes HaplotypeSequences and runs reset() on the GPU
         self.likelihoods = None     # [H, sum of the samples' widths]
         self._samples = []
         self._off = [0]
@@ -662,6 +691,9 @@ class HaplotypeLikelihoodArray:
         if self._engine is None:
             self._engine = PairHMMEngine()
         return self._engine
+
+    def _with_model(self):
+        return {} if self.error_model is None else {"error_model": self.error_model}
 
     def _set_samples(self, names, widths):
         self._samples = list(names)
@@ -675,13 +707,15 @@ class HaplotypeLikelihoodArray:
         {sample: ReadBlock} in sample order, or one ReadBlock (a single unnamed sample, left primed)."""
         if isinstance(reads, ReadBlock):
             self._set_samples([""], [reads.n])
-            self.likelihoods = self.engine.populate(self.likelihood_model.config, haplotypes, reads, positions, flank_state)
+            self.likelihoods = self.engine.populate(self.likelihood_model.config, haplotypes, reads, positions, flank_state,
+                                                    **self._with_model())
             self._primed = 0
             return self
         names = list(reads.keys())
         blocks = [reads[k] for k in names]
         self._set_samples(names, [b.n for b in blocks])
-        self.likelihoods = self.engine.populate(self.likelihood_model.config, haplotypes, concat_reads(blocks), positions, flank_state)
+        self.likelihoods = self.engine.populate(self.likelihood_model.config, haplotypes, concat_reads(blocks), positions, flank_state,
+                                                **self._with_model())
         return self
 
     def populate_templates(self, templates, haplotypes: HaplotypeBlock, flank_state=None):
@@ -698,7 +732,7 @@ class HaplotypeLikelihoodArray:
             base += rb.n
         self._set_samples(names, [len(templates[k][1]) - 1 for k in names])
         self.likelihoods = self.engine.populate_templates(self.likelihood_model.config, haplotypes, concat_reads(blocks),
-                                                          np.concatenate(toff), flank_state)
+                                                          np.concatenate(toff), flank_state, **self._with_model())
         return self
 
     # -- accessors (haplotype_likelihood_array.cpp:200-291) ----------------------------------------------------
@@ -762,7 +796,7 @@ class HaplotypeLikelihoodArray:
         """merge_samples (:362-409): a one-sample array holding the chosen samples' likelihoods back to back; primed."""
         samples = self.samples() if samples is None else list(samples)
         idx = [self._sample_index(s) for s in samples]
-        out = HaplotypeLikelihoodArray(self.likelihood_model, self._engine)
+        out = HaplotypeLikelihoodArray(self.likelihood_model, self._engine, self.error_model)
         parts = [self.likelihoods[:, self._off[s]:self._off[s + 1]] for s in idx]
         if isinstance(self.likelihoods, np.ndarray):
             out.likelihoods = np.concatenate(parts, axis=1)

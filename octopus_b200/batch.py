@@ -123,6 +123,39 @@ class HaplotypeBlock(_Block):
         return {f: getattr(self, f)[a:b] for f in self._fields[1:8]}
 
 
+class HaplotypeSequences(_Block):
+    """H haplotypes as sequences only (phmm_haplotype_sequences): the populate calls with an error model derive the penalty arrays
+    of a HaplotypeBlock from them on the GPU. ``is_substitution``: per-base flags (bases that are substitutions in
+    Haplotype::cigar()) or None; ``begin``: mapped_begin per haplotype or None. Numpy arrays, or torch CUDA tensors."""
+    _fields = ("off", "seq", "is_substitution", "begin")
+
+    def __init__(self, off, seq, begin=None, is_substitution=None):
+        self.n = len(off) - 1
+        self.on_device = hasattr(seq, "data_ptr") and seq.is_cuda
+        if self.on_device:
+            self.off, self.seq, self.is_substitution, self.begin = off, seq, is_substitution, begin
+            return
+        self.off = np.ascontiguousarray(off, dtype=np.int64)
+        self.seq = np.ascontiguousarray(seq, dtype=np.uint8)
+        self.is_substitution = None if is_substitution is None else np.ascontiguousarray(is_substitution, dtype=np.uint8)
+        self.begin = None if begin is None else np.ascontiguousarray(begin, dtype=np.int64)
+        assert self.is_substitution is None or len(self.is_substitution) == int(self.off[-1])
+
+    @classmethod
+    def pack(cls, sequences, begin=None, is_substitution=None):
+        """sequences (list of str / bytes / uint8 arrays), optional per-haplotype begins and per-haplotype flag arrays → block."""
+        off, seq = pack_sequences(sequences)
+        sub = None if is_substitution is None else pack_sequences([np.asarray(x, dtype=np.uint8) for x in is_substitution])[1]
+        return cls(off, seq, begin, sub)
+
+    def c_struct(self):
+        s = _lib.HaplotypeSequences()
+        s.n = self.n
+        for f in self._fields:
+            setattr(s, f, _ptr(getattr(self, f)))
+        return s
+
+
 class ReadBlock(_Block):
     """R reads: the AlignedRead fields the path consumes (basics/aligned_read.hpp:36-39,120-146)."""
     _fields = ("off", "bases", "quals", "mapq", "reverse", "begin")
@@ -195,6 +228,16 @@ def _cat_off(blocks):
 
 def _cat(blocks, f):
     return np.concatenate([getattr(b, f) for b in blocks])
+
+
+def concat_sequences(blocks):
+    """Host HaplotypeSequences back to back as one block (flags zero-filled where a block has none, begins 0 where it has none)."""
+    total = [int(b.off[-1]) for b in blocks]
+    sub = None
+    if any(b.is_substitution is not None for b in blocks):
+        sub = np.concatenate([b.is_substitution if b.is_substitution is not None else np.zeros(t, dtype=np.uint8) for b, t in zip(blocks, total)])
+    begin = np.concatenate([b.begin if b.begin is not None else np.zeros(b.n, dtype=np.int64) for b in blocks])
+    return HaplotypeSequences(_cat_off(blocks), _cat(blocks, "seq"), begin, sub)
 
 
 def concat_reads(blocks):

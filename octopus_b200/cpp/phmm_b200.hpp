@@ -438,6 +438,12 @@ struct HaplotypeBlock   // what HaplotypeLikelihoodModel::reset derives per hapl
         off.push_back(static_cast<std::int64_t>(seq.size()));
     }
     std::size_t size() const noexcept { return off.size() - 1; }
+    // The sequences side only: what a populate with an error model reads (seq, off, begin and the substitution flags of add()).
+    phmm_haplotype_sequences sequences_view() const noexcept
+    {
+        return phmm_haplotype_sequences {static_cast<std::int32_t>(size()), off.data(), seq.data(),
+                                         is_substitution.size() == seq.size() ? is_substitution.data() : nullptr, begin.data()};
+    }
     phmm_haplotypes view() const noexcept
     {
         return phmm_haplotypes {static_cast<std::int32_t>(size()), off.data(), seq.data(), snv_mask_fwd.data(), snv_prior_fwd.data(),
@@ -747,6 +753,13 @@ public:
     explicit HaplotypeLikelihoodArray(phmm_config config, Engine engine = Engine {}) : engine_ {std::move(engine)}, config_ {checked(config)} {}
     // populate() goes through a process-wide SharedEngine: any number of threads, each with its own array, share one GPU engine
     HaplotypeLikelihoodArray(phmm_config config, SharedEngine shared) : engine_ {nullptr}, shared_ {std::move(shared)}, config_ {checked(config)} {}
+    // With an error model, populate() runs likelihood_model_.reset(haplotype) itself, as the reference's populate does
+    // (haplotype_likelihood_array.cpp:77-95): it reads only the HaplotypeBlock's sequences (add(sequence, begin, substitutions)) and
+    // the GPU derives the penalty arrays in the same call (phmm_populate*_reset), with the values of HaplotypeBlock::reset(model).
+    HaplotypeLikelihoodArray(phmm_config config, ErrorModel model, Engine engine = Engine {})
+        : engine_ {std::move(engine)}, model_ {std::make_shared<const ErrorModel>(std::move(model))}, config_ {checked(config)} {}
+    HaplotypeLikelihoodArray(phmm_config config, ErrorModel model, SharedEngine shared)
+        : engine_ {nullptr}, shared_ {std::move(shared)}, model_ {std::make_shared<const ErrorModel>(std::move(model))}, config_ {checked(config)} {}
     static phmm_config default_config() noexcept { phmm_config c; phmm_default_config(&c); return c; }
 
     // populate(const ReadMap&, haplotypes, flank_state) — haplotype_likelihood_array.cpp:51-103.
@@ -824,6 +837,7 @@ public:
         SampleName name;
         if (new_sample) name = *new_sample; else for (const auto& s : samples) name += s;
         HaplotypeLikelihoodArray result = shared_.get() ? HaplotypeLikelihoodArray {config_, shared_} : HaplotypeLikelihoodArray {config_, engine_};
+        result.model_ = model_;
         std::vector<std::size_t> idx;
         std::size_t total = 0;
         for (const auto& s : samples) { idx.push_back(sample_index(s)); total += width(idx.back()); }
@@ -845,6 +859,7 @@ public:
 private:
     Engine engine_;
     SharedEngine shared_ {nullptr};   // set: populate() goes through the batcher instead of engine_
+    std::shared_ptr<const ErrorModel> model_;   // set: populate() takes sequences and runs the model's reset() on the GPU
     phmm_config config_;
     pinned_vector<double> likelihoods_;
     pinned_vector<std::int32_t> status_;
@@ -880,7 +895,7 @@ private:
     void run(const ReadBlock& reads, const pinned_vector<std::int64_t>* template_off, const HaplotypeBlock& haplotypes,
              const FlankState* flank_state, const phmm_positions* positions)
     {
-        const auto hv = haplotypes.view();
+        const auto hv = haplotypes.view();         // unused with an error model
         const auto rv = reads.view();
         num_haplotypes_ = haplotypes.size();
         likelihoods_.resize(num_haplotypes_ * total_width());        // every element is written by the call (no zero fill; the storage is page-locked and kept)
@@ -890,7 +905,21 @@ private:
         phmm_flank_state fs = detail::flank_state(flank_state);
         const auto n_templates = template_off ? static_cast<std::int32_t>(template_off->size() - 1) : 0;
         int rc;
-        if (shared_.get()) {
+        if (model_) {
+            const auto sv = haplotypes.sequences_view();
+            const phmm_error_model* m = model_->get();
+            if (shared_.get()) {
+                rc = template_off
+                    ? phmm_batcher_populate_templates_reset(shared_.get(), &config_, m, &sv, &rv, template_off->data(), n_templates, &fs,
+                                                            likelihoods_.data(), status.data())
+                    : phmm_batcher_populate_reset(shared_.get(), &config_, m, &sv, &rv, positions, &fs, likelihoods_.data(), status.data());
+            } else {
+                rc = template_off
+                    ? phmm_populate_templates_reset(engine_.get(), &config_, m, &sv, &rv, template_off->data(), n_templates, positions, &fs,
+                                                    likelihoods_.data(), status.data(), PHMM_SPACE_HOST)
+                    : phmm_populate_reset(engine_.get(), &config_, m, &sv, &rv, positions, &fs, likelihoods_.data(), status.data(), PHMM_SPACE_HOST);
+            }
+        } else if (shared_.get()) {
             rc = template_off
                 ? phmm_batcher_populate_templates(shared_.get(), &config_, &hv, &rv, template_off->data(), n_templates, &fs, likelihoods_.data(), status.data())
                 : phmm_batcher_populate(shared_.get(), &config_, &hv, &rv, positions, &fs, likelihoods_.data(), status.data());

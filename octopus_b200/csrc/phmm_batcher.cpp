@@ -3,6 +3,7 @@
 // call. Host C++ over the public C ABI; a batch runs the engine's existing multi-region / multi-set kernel chain. No thread of its
 // own: the first member of a batch (its leader) makes the call.
 #include "../../include/phmm_b200.h"
+#include "phmm_batcher_seam.h"
 #include "phmm_checks.h"
 #include "phmm_mutation.h"
 
@@ -63,14 +64,104 @@ struct Pinned {
     }
 };
 
-// The two request kinds. Each supplies what differs between them: its counts, its staging, its merge key and limits, its
-// per-member bookkeeping (a Kind object lives in each batch), the copy in, the merged engine call and the copy out.
+// The request kinds. Each supplies what differs between them: its counts, its staging, its merge key and limits, its per-member
+// bookkeeping (a Kind object lives in each batch), the copy in, the merged engine call and the copy out.
 
-// Populate requests: a batch is one phmm_populate_regions call and each member one of its regions; equal configs merge.
-struct Populate {
+// What the two populate kinds share: their counts, the read side of their staging, a batch's regions (one per member; the batch is
+// one multi-region call) and the copy out.
+struct PopulateBase {
     enum { HAPS, HAP_BASES, READS, READ_BASES, PAIRS, N_COUNTS };
     using Sizes = Counts<N_COUNTS>;
 
+    // One batch's page-locked copy of its members' reads and its results.
+    struct ReadStaging {
+        Pinned<int64_t> read_off, read_begin;
+        Pinned<char> bases;
+        Pinned<uint8_t> quals, mapq, reverse;
+        Pinned<double> out;
+        Pinned<int32_t> status;
+        Sizes cap;
+        bool busy = false;
+
+        bool grow_reads(const Sizes& s)
+        {
+            const bool ok = read_off.ensure(s[READS] + 1) && read_begin.ensure(s[READS]) && bases.ensure(s[READ_BASES]) && quals.ensure(s[READ_BASES]) &&
+                            mapq.ensure(s[READS]) && reverse.ensure(s[READS]) && out.ensure(s[PAIRS]) && status.ensure(s[PAIRS]);
+            if (!ok) return false;
+            cap[READS] = std::min({read_off.cap - 1, read_begin.cap, mapq.cap, reverse.cap});
+            cap[READ_BASES] = std::min(bases.cap, quals.cap);
+            cap[PAIRS] = std::min(out.cap, status.cap);
+            return true;
+        }
+
+        void copy_in_reads(const Sizes& at, const phmm_reads* reads)
+        {
+            const int R = reads->n;
+            const long long rb = reads->off[R];
+            if (at[READS] == 0) read_off.p[0] = 0;
+            for (int r = 0; r < R; ++r) read_off.p[at[READS] + r + 1] = at[READ_BASES] + reads->off[r + 1];
+            if (reads->begin) std::memcpy(read_begin.p + at[READS], reads->begin, (size_t)R * sizeof(int64_t));
+            else std::memset(read_begin.p + at[READS], 0, (size_t)R * sizeof(int64_t));
+            std::memcpy(bases.p + at[READ_BASES], reads->bases, (size_t)rb);
+            std::memcpy(quals.p + at[READ_BASES], reads->quals, (size_t)rb);
+            std::memcpy(mapq.p + at[READS], reads->mapq, (size_t)R);
+            std::memcpy(reverse.p + at[READS], reads->reverse, (size_t)R);
+        }
+
+        phmm_reads reads(const Sizes& used) const { return {(int32_t)used[READS], read_off.p, bases.p, quals.p, mapq.p, reverse.p, read_begin.p}; }
+    };
+
+    // first staging size: some tens of regions of a few hundred reads; it grows to what merged batches ask for
+    static Sizes initial_staging() { return {{4096, 1LL << 20, 1LL << 16, 8LL << 20, 1LL << 20}}; }
+    static bool within_limits(const Sizes& s) { return s[HAPS] <= kMaxBatchHaps && s[PAIRS] <= kMaxBatchPairs; }
+
+    phmm_config cfg;
+    std::vector<int32_t> hap_first {0}, read_first {0};
+    std::vector<phmm_flank_state> flanks;
+
+    explicit PopulateBase(const phmm_config* c) : cfg(*c) {}
+
+    // a new member's region, ending at the batch's counts `used`
+    template <typename Request>
+    void add(const Request& q, const Sizes& used)
+    {
+        hap_first.push_back((int32_t)used[HAPS]);
+        read_first.push_back((int32_t)used[READS]);
+        flanks.push_back(q.flank ? *q.flank : phmm_flank_state {0, 0, 0});
+    }
+
+    phmm_regions regions() const { return {(int32_t)flanks.size(), hap_first.data(), read_first.data(), flanks.data()}; }
+
+    // this member's slice of the call's result, [H][R] at the pair offset of its region
+    template <typename Request>
+    static int copy_out(const ReadStaging& st, const Sizes& at, const Request& q, int rc, const std::string& err)
+    {
+        if (rc != PHMM_OK && rc != PHMM_ERR_SHORT_HAPLOTYPE) { t_error = err; return rc; }
+        const long long H = q.need[HAPS], R = q.need[READS];
+        const double* res = st.out.p + at[PAIRS];
+        const int32_t* res_status = st.status.p + at[PAIRS];
+        rc = PHMM_OK;
+        for (long long i = 0; i < q.need[PAIRS]; ++i) if ((res_status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) { rc = PHMM_ERR_SHORT_HAPLOTYPE; break; }
+        t_error = rc == PHMM_OK ? std::string() : std::string("Haplotype is too short for alignment");
+        if (q.status) std::memcpy(q.status, res_status, (size_t)q.need[PAIRS] * sizeof(int32_t));
+        if (q.template_off) {
+            // k_template_sum's order: each template's reads left to right from 0.0
+            for (long long h = 0; h < H; ++h) {
+                for (int t = 0; t < q.n_templates; ++t) {
+                    double acc = 0.0;
+                    for (long long r = q.template_off[t]; r < q.template_off[t + 1]; ++r) acc += res[(size_t)h * R + r];
+                    q.out[(size_t)h * q.n_templates + t] = acc;
+                }
+            }
+        } else {
+            std::memcpy(q.out, res, (size_t)q.need[PAIRS] * sizeof(double));
+        }
+        return rc;
+    }
+};
+
+// Populate requests: a batch is one phmm_populate_regions call and each member one of its regions; equal configs merge.
+struct Populate : PopulateBase {
     struct Request {
         const phmm_config* cfg; const phmm_haplotypes* haps; const phmm_reads* reads;
         const int64_t* template_off; int32_t n_templates;     // template_off NULL: a read request
@@ -79,59 +170,33 @@ struct Populate {
     };
 
     // One batch's page-locked copy of its members' blocks and its results.
-    struct Staging {
-        Pinned<int64_t> hap_off, hap_begin, read_off, read_begin;
-        Pinned<char> seq, mask_f, mask_r, bases;
+    struct Staging : ReadStaging {
+        Pinned<int64_t> hap_off, hap_begin;
+        Pinned<char> seq, mask_f, mask_r;
         Pinned<int8_t> prior_f, prior_r, gap_open, gap_extend;
-        Pinned<uint8_t> quals, mapq, reverse;
-        Pinned<double> out;
-        Pinned<int32_t> status;
-        Sizes cap;
-        bool busy = false;
 
         bool grow(const Sizes& s)
         {
-            const bool ok = hap_off.ensure(s[HAPS] + 1) && hap_begin.ensure(s[HAPS]) && read_off.ensure(s[READS] + 1) && read_begin.ensure(s[READS]) &&
-                            seq.ensure(s[HAP_BASES]) && mask_f.ensure(s[HAP_BASES]) && mask_r.ensure(s[HAP_BASES]) && prior_f.ensure(s[HAP_BASES]) &&
-                            prior_r.ensure(s[HAP_BASES]) && gap_open.ensure(s[HAP_BASES]) && gap_extend.ensure(s[HAP_BASES]) &&
-                            bases.ensure(s[READ_BASES]) && quals.ensure(s[READ_BASES]) && mapq.ensure(s[READS]) && reverse.ensure(s[READS]) &&
-                            out.ensure(s[PAIRS]) && status.ensure(s[PAIRS]);
+            const bool ok = hap_off.ensure(s[HAPS] + 1) && hap_begin.ensure(s[HAPS]) && seq.ensure(s[HAP_BASES]) && mask_f.ensure(s[HAP_BASES]) &&
+                            mask_r.ensure(s[HAP_BASES]) && prior_f.ensure(s[HAP_BASES]) && prior_r.ensure(s[HAP_BASES]) &&
+                            gap_open.ensure(s[HAP_BASES]) && gap_extend.ensure(s[HAP_BASES]) && grow_reads(s);
             if (!ok) return false;
             cap[HAPS] = std::min(hap_off.cap - 1, hap_begin.cap);
-            cap[READS] = std::min({read_off.cap - 1, read_begin.cap, mapq.cap, reverse.cap});
             cap[HAP_BASES] = std::min({seq.cap, mask_f.cap, mask_r.cap, prior_f.cap, prior_r.cap, gap_open.cap, gap_extend.cap});
-            cap[READ_BASES] = std::min(bases.cap, quals.cap);
-            cap[PAIRS] = std::min(out.cap, status.cap);
             return true;
         }
     };
 
-    // first staging size: some tens of regions of a few hundred reads; it grows to what merged batches ask for
-    static Sizes initial_staging() { return {{4096, 1LL << 20, 1LL << 16, 8LL << 20, 1LL << 20}}; }
-    static bool within_limits(const Sizes& s) { return s[HAPS] <= kMaxBatchHaps && s[PAIRS] <= kMaxBatchPairs; }
     static std::string key(const Request& q) { return std::string(reinterpret_cast<const char*>(q.cfg), sizeof(phmm_config)); }
 
-    phmm_config cfg;
-    std::vector<int32_t> hap_first {0}, read_first {0};
-    std::vector<phmm_flank_state> flanks;
-
-    explicit Populate(const Request& q) : cfg(*q.cfg) {}
-
-    // a new member's region, ending at the batch's counts `used`
-    void add(const Request& q, const Sizes& used)
-    {
-        hap_first.push_back((int32_t)used[HAPS]);
-        read_first.push_back((int32_t)used[READS]);
-        flanks.push_back(q.flank ? *q.flank : phmm_flank_state {0, 0, 0});
-    }
+    explicit Populate(const Request& q) : PopulateBase(q.cfg) {}
 
     // the request into its slot at `at` (outside the lock: each member writes its own ranges only)
     static void copy_in(Staging& st, const Sizes& at, const Request& q)
     {
         const phmm_haplotypes* haps = q.haps;
-        const phmm_reads* reads = q.reads;
-        const int H = haps->n, R = reads->n;
-        const long long hb = haps->off[H], rb = reads->off[R];
+        const int H = haps->n;
+        const long long hb = haps->off[H];
         if (at[HAPS] == 0) st.hap_off.p[0] = 0;
         for (int h = 0; h < H; ++h) st.hap_off.p[at[HAPS] + h + 1] = at[HAP_BASES] + haps->off[h + 1];
         if (haps->begin) std::memcpy(st.hap_begin.p + at[HAPS], haps->begin, (size_t)H * sizeof(int64_t));
@@ -143,14 +208,7 @@ struct Populate {
         std::memcpy(st.prior_r.p + at[HAP_BASES], haps->snv_prior_rev, (size_t)hb);
         std::memcpy(st.gap_open.p + at[HAP_BASES], haps->gap_open, (size_t)hb);
         std::memcpy(st.gap_extend.p + at[HAP_BASES], haps->gap_extend, (size_t)hb);
-        if (at[READS] == 0) st.read_off.p[0] = 0;
-        for (int r = 0; r < R; ++r) st.read_off.p[at[READS] + r + 1] = at[READ_BASES] + reads->off[r + 1];
-        if (reads->begin) std::memcpy(st.read_begin.p + at[READS], reads->begin, (size_t)R * sizeof(int64_t));
-        else std::memset(st.read_begin.p + at[READS], 0, (size_t)R * sizeof(int64_t));
-        std::memcpy(st.bases.p + at[READ_BASES], reads->bases, (size_t)rb);
-        std::memcpy(st.quals.p + at[READ_BASES], reads->quals, (size_t)rb);
-        std::memcpy(st.mapq.p + at[READS], reads->mapq, (size_t)R);
-        std::memcpy(st.reverse.p + at[READS], reads->reverse, (size_t)R);
+        st.copy_in_reads(at, q.reads);
     }
 
     // the leader's call: the batch's members as the regions of one phmm_populate_regions call
@@ -158,35 +216,67 @@ struct Populate {
     {
         const phmm_haplotypes hv {(int32_t)used[HAPS], st.hap_off.p, st.seq.p, st.mask_f.p, st.prior_f.p, st.mask_r.p, st.prior_r.p,
                                   st.gap_open.p, st.gap_extend.p, st.hap_begin.p};
-        const phmm_reads rv {(int32_t)used[READS], st.read_off.p, st.bases.p, st.quals.p, st.mapq.p, st.reverse.p, st.read_begin.p};
-        const phmm_regions regions {(int32_t)flanks.size(), hap_first.data(), read_first.data(), flanks.data()};
-        return phmm_populate_regions(e, &cfg, &hv, &rv, &regions, st.out.p, st.status.p, PHMM_SPACE_HOST);
+        const phmm_reads rv = st.reads(used);
+        const phmm_regions rg = regions();
+        return phmm_populate_regions(e, &cfg, &hv, &rv, &rg, st.out.p, st.status.p, PHMM_SPACE_HOST);
+    }
+};
+
+// Populate requests with an error model: a batch is one phmm_populate_regions_reset call. Equal configs under models equal by
+// content merge; the staging holds the sequences and their substitution flags instead of the six penalty arrays.
+struct PopulateReset : PopulateBase {
+    struct Request {
+        const phmm_batcher_seam::ResetRequest* r;
+        const phmm_config* cfg; const phmm_haplotype_sequences* seqs; const phmm_reads* reads;
+        const int64_t* template_off; int32_t n_templates; const phmm_flank_state* flank; double* out; int32_t* status;
+        Sizes need;
+    };
+
+    struct Staging : ReadStaging {
+        Pinned<int64_t> hap_off, hap_begin;
+        Pinned<char> seq;
+        Pinned<uint8_t> is_substitution;
+
+        bool grow(const Sizes& s)
+        {
+            if (!(hap_off.ensure(s[HAPS] + 1) && hap_begin.ensure(s[HAPS]) && seq.ensure(s[HAP_BASES]) && is_substitution.ensure(s[HAP_BASES]) &&
+                  grow_reads(s)))
+                return false;
+            cap[HAPS] = std::min(hap_off.cap - 1, hap_begin.cap);
+            cap[HAP_BASES] = std::min(seq.cap, is_substitution.cap);
+            return true;
+        }
+    };
+
+    static std::string key(const Request& q) { return std::string(reinterpret_cast<const char*>(q.cfg), sizeof(phmm_config)) + q.r->model_key; }
+
+    const phmm_error_model* model;                       // the leader's model (the members' are equal by content)
+    const phmm_batcher_seam::ResetCalls* calls;
+
+    explicit PopulateReset(const Request& q) : PopulateBase(q.cfg), model(q.r->m), calls(q.r->calls) {}
+
+    static void copy_in(Staging& st, const Sizes& at, const Request& q)
+    {
+        const phmm_haplotype_sequences* seqs = q.seqs;
+        const int H = seqs->n;
+        const long long hb = seqs->off[H];
+        if (at[HAPS] == 0) st.hap_off.p[0] = 0;
+        for (int h = 0; h < H; ++h) st.hap_off.p[at[HAPS] + h + 1] = at[HAP_BASES] + seqs->off[h + 1];
+        if (seqs->begin) std::memcpy(st.hap_begin.p + at[HAPS], seqs->begin, (size_t)H * sizeof(int64_t));
+        else std::memset(st.hap_begin.p + at[HAPS], 0, (size_t)H * sizeof(int64_t));
+        std::memcpy(st.seq.p + at[HAP_BASES], seqs->seq, (size_t)hb);
+        // no flags and all-zero flags give the same arrays
+        if (seqs->is_substitution) std::memcpy(st.is_substitution.p + at[HAP_BASES], seqs->is_substitution, (size_t)hb);
+        else std::memset(st.is_substitution.p + at[HAP_BASES], 0, (size_t)hb);
+        st.copy_in_reads(at, q.reads);
     }
 
-    // this member's slice of the call's result, [H][R] at the pair offset of its region
-    static int copy_out(const Staging& st, const Sizes& at, const Request& q, int rc, const std::string& err)
+    int run(phmm_engine* e, Staging& st, const Sizes& used) const
     {
-        if (rc != PHMM_OK && rc != PHMM_ERR_SHORT_HAPLOTYPE) { t_error = err; return rc; }
-        const int H = q.haps->n, R = q.reads->n;
-        const double* res = st.out.p + at[PAIRS];
-        const int32_t* res_status = st.status.p + at[PAIRS];
-        rc = PHMM_OK;
-        for (long long i = 0; i < q.need[PAIRS]; ++i) if ((res_status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) { rc = PHMM_ERR_SHORT_HAPLOTYPE; break; }
-        t_error = rc == PHMM_OK ? std::string() : std::string("Haplotype is too short for alignment");
-        if (q.status) std::memcpy(q.status, res_status, (size_t)q.need[PAIRS] * sizeof(int32_t));
-        if (q.template_off) {
-            // k_template_sum's order: each template's reads left to right from 0.0
-            for (int h = 0; h < H; ++h) {
-                for (int t = 0; t < q.n_templates; ++t) {
-                    double acc = 0.0;
-                    for (long long r = q.template_off[t]; r < q.template_off[t + 1]; ++r) acc += res[(size_t)h * R + r];
-                    q.out[(size_t)h * q.n_templates + t] = acc;
-                }
-            }
-        } else {
-            std::memcpy(q.out, res, (size_t)q.need[PAIRS] * sizeof(double));
-        }
-        return rc;
+        const phmm_haplotype_sequences sv {(int32_t)used[HAPS], st.hap_off.p, st.seq.p, st.is_substitution.p, st.hap_begin.p};
+        const phmm_reads rv = st.reads(used);
+        const phmm_regions rg = regions();
+        return calls->populate_regions(e, &cfg, model, &sv, &rv, &rg, st.out.p, st.status.p, PHMM_SPACE_HOST);
     }
 };
 
@@ -290,6 +380,7 @@ struct phmm_batcher {
     mutable std::mutex m;
     std::condition_variable cv;
     Lane<Populate> populate;
+    Lane<PopulateReset> populate_reset;
     Lane<MutationPrime> mutation;
     bool engine_busy = false;
     int waiting = 0;                                  // requests in batches not yet sent + requests running alone
@@ -308,9 +399,9 @@ void count_call(phmm_batcher* b, int requests)
     b->stats.dp_cells += phmm_last_dp_cells(b->engine);
 }
 
-// A request phmm_populate_regions cannot merge: one engine call of its own, in turn with the batches.
-int run_alone(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_positions* positions,
-              const int64_t* template_off, int32_t n_templates, const phmm_flank_state* flank, double* out, int32_t* status)
+// A request a multi-region call cannot merge: one engine call of its own, call(engine), in turn with the batches.
+template <typename Call>
+int run_alone(phmm_batcher* b, Call&& call)
 {
     std::unique_lock<std::mutex> lk(b->m);
     ++b->waiting;
@@ -318,8 +409,7 @@ int run_alone(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* ha
     b->cv.wait(lk, [&] { return !b->engine_busy; });
     b->engine_busy = true;
     lk.unlock();
-    const int rc = template_off ? phmm_populate_templates(b->engine, cfg, haps, reads, template_off, n_templates, positions, flank, out, status, PHMM_SPACE_HOST)
-                                : phmm_populate(b->engine, cfg, haps, reads, positions, flank, out, status, PHMM_SPACE_HOST);
+    const int rc = call(b->engine);
     t_error = rc == PHMM_OK ? std::string() : std::string(phmm_last_error(b->engine));
     lk.lock();
     count_call(b, 1);
@@ -445,12 +535,13 @@ int take_part(phmm_batcher* b, Lane<Kind>& lane, const typename Kind::Request& q
 
 // The host-side checks of phmm_populate, in its order, for a request without position lists. Sets *alone when the request has to
 // run on its own (pipelined size, too many haplotypes, a haplotype too long for the task word); the remaining checks are then
-// phmm_populate's own.
-int check_request(const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads, const double* out, bool* alone, Populate::Sizes* need)
+// phmm_populate's own. `derived`: a request with an error model, whose penalty arrays the engine derives (haps holds n / off / seq).
+int check_request(const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads, const double* out, bool* alone, Populate::Sizes* need,
+                  bool derived = false)
 {
     int rc;
     if ((rc = phmm_checks::config_and_output(cfg, out, reads, t_error)) != PHMM_OK) return rc;
-    if ((rc = phmm_checks::blocks(haps, reads, t_error)) != PHMM_OK) return rc;
+    if ((rc = phmm_checks::blocks(haps, reads, t_error, derived)) != PHMM_OK) return rc;
     const long long pairs = (long long)haps->n * reads->n;
     if (pairs >= 2 * phmm_checks::populate_chunk_pairs(pairs) || haps->n > kMaxBatchHaps) { *alone = true; return PHMM_OK; }
     long long len_min, len_max;
@@ -461,7 +552,7 @@ int check_request(const phmm_config* cfg, const phmm_haplotypes* haps, const phm
     for (int h = 0; h < haps->n; ++h) max_hap = std::max<long long>(max_hap, haps->off[h + 1] - haps->off[h]);
     if (cfg->map_positions && (rc = phmm_checks::mapper_haplotypes(max_hap, hap_bases, t_error)) != PHMM_OK) return rc;
     if (max_hap > 65535) { *alone = true; return PHMM_OK; }
-    if ((rc = phmm_checks::penalties(haps, hap_bases, t_error)) != PHMM_OK) return rc;
+    if (!derived && (rc = phmm_checks::penalties(haps, hap_bases, t_error)) != PHMM_OK) return rc;
     *need = {{haps->n, hap_bases, reads->n, read_bases, pairs}};
     return PHMM_OK;
 }
@@ -475,7 +566,12 @@ int submit(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps,
         const int rc = check_request(cfg, haps, reads, out, &alone, &q.need);
         if (rc != PHMM_OK) return rc;
     }
-    if (alone) return run_alone(b, cfg, haps, reads, positions, template_off, n_templates, flank, out, status);
+    if (alone) {
+        return run_alone(b, [&](phmm_engine* e) {
+            return template_off ? phmm_populate_templates(e, cfg, haps, reads, template_off, n_templates, positions, flank, out, status, PHMM_SPACE_HOST)
+                                : phmm_populate(e, cfg, haps, reads, positions, flank, out, status, PHMM_SPACE_HOST);
+        });
+    }
     return take_part(b, b->populate, q);
 }
 
@@ -487,6 +583,29 @@ struct InFlight {
 };
 
 } // namespace
+
+int phmm_batcher_seam::submit_reset(phmm_batcher* b, const ResetRequest& r)
+{
+    if (!b) { t_error = "null batcher"; return PHMM_ERR_INVALID; }
+    // phmm_populate(_templates)_reset's checks in their order: the sequences block, the template offsets, the reset, the populate
+    if (!r.seqs) { t_error = "null argument"; return PHMM_ERR_INVALID; }
+    int rc;
+    if (r.template_off && (rc = phmm_checks::template_offsets(r.template_off, r.n_templates, r.reads, true, t_error)) != PHMM_OK) return rc;
+    if ((rc = phmm_checks::reset_sequences(r.m, r.seqs, t_error)) != PHMM_OK) return rc;
+    InFlight guard(b);
+    const phmm_haplotypes shell {r.seqs->n, r.seqs->off, r.seqs->seq, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, r.seqs->begin};
+    bool alone = (r.positions && r.positions->off && r.positions->pos) || r.model_key.empty();
+    PopulateReset::Request q {&r, r.cfg, r.seqs, r.reads, r.template_off, r.n_templates, r.flank, r.out, r.status, {}};
+    if (!alone && (rc = check_request(r.cfg, &shell, r.reads, r.out, &alone, &q.need, true)) != PHMM_OK) return rc;
+    if (alone) {
+        return run_alone(b, [&](phmm_engine* e) {
+            return r.template_off ? r.calls->populate_templates(e, r.cfg, r.m, r.seqs, r.reads, r.template_off, r.n_templates, r.positions, r.flank,
+                                                                r.out, r.status, PHMM_SPACE_HOST)
+                                  : r.calls->populate(e, r.cfg, r.m, r.seqs, r.reads, r.positions, r.flank, r.out, r.status, PHMM_SPACE_HOST);
+        });
+    }
+    return take_part(b, b->populate_reset, q);
+}
 
 extern "C" {
 

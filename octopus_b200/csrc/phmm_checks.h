@@ -21,15 +21,16 @@ inline int config_and_output(const phmm_config* cfg, const void* out, const phmm
     return PHMM_OK;
 }
 
-// non-empty blocks with every per-base array present
-inline int blocks(const phmm_haplotypes* haps, const phmm_reads* reads, std::string& err)
+// non-empty blocks with every per-base array present; `derived`: the six penalty arrays are yet to be derived from the sequences
+// (a populate call with an error model)
+inline int blocks(const phmm_haplotypes* haps, const phmm_reads* reads, std::string& err, bool derived = false)
 {
     if (!haps || !reads || haps->n <= 0 || reads->n <= 0 || !haps->off || !reads->off) {
         err = "empty or null haplotype / read block";
         return PHMM_ERR_INVALID;
     }
-    if (!haps->seq || !haps->snv_mask_fwd || !haps->snv_prior_fwd || !haps->snv_mask_rev || !haps->snv_prior_rev ||
-        !haps->gap_open || !haps->gap_extend || !reads->bases || !reads->quals) {
+    if (!haps->seq || (!derived && (!haps->snv_mask_fwd || !haps->snv_prior_fwd || !haps->snv_mask_rev || !haps->snv_prior_rev ||
+        !haps->gap_open || !haps->gap_extend)) || !reads->bases || !reads->quals) {
         err = "null per-base array";
         return PHMM_ERR_INVALID;
     }
@@ -74,6 +75,20 @@ inline int penalties(const phmm_haplotypes* haps, long long hap_bases, std::stri
             if (a[i] < 0) { err = "snv prior / gap penalty outside [0,127]"; return PHMM_ERR_INVALID; }
         }
     }
+    return PHMM_OK;
+}
+
+// the error-model reset of a populate call with an error model, for host-resident sequences (phmm_engine_reset_haplotypes' checks)
+inline int reset_sequences(const void* model, const phmm_haplotype_sequences* seqs, std::string& err)
+{
+    if (!model || !seqs || seqs->n < 0 || (seqs->n > 0 && (!seqs->off || !seqs->seq))) { err = "null argument"; return PHMM_ERR_INVALID; }
+    if (seqs->n > 0 && seqs->off[0] < 0) { err = "bad haplotype offsets"; return PHMM_ERR_INVALID; }
+    long long longest = 0;
+    for (int32_t h = 0; h < seqs->n; ++h) {
+        if (seqs->off[h + 1] < seqs->off[h]) { err = "bad haplotype offsets"; return PHMM_ERR_INVALID; }
+        longest = std::max<long long>(longest, seqs->off[h + 1] - seqs->off[h]);
+    }
+    if (longest > 65535) { err = "haplotype longer than 65535 bases"; return PHMM_ERR_INVALID; }
     return PHMM_OK;
 }
 

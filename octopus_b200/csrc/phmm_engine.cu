@@ -171,13 +171,17 @@ int fetch_offsets(phmm_engine* e, const int64_t* off, int n, int space, std::vec
     return PHMM_OK;
 }
 
-// Upload (or alias) the batch and run the preparation kernels: column tables, row half-words, read info.
+// Upload (or alias) the batch and run the preparation kernels: column tables, row half-words, read info. The haplotypes live in
+// hap_space (< 0: `space`, the reads'): a populate call with an error model hands over the arrays it derived on the device, and
+// the haplotype offsets it already holds on the host (hap_off_host, else they are fetched).
 int stage_batch(phmm_engine* e, const phmm_haplotypes* haps, const phmm_reads* reads, int space, Staged& s, bool need_info_host = true,
-                bool defer_flag_check = false)
+                bool defer_flag_check = false, int hap_space = -1, const std::vector<long long>* hap_off_host = nullptr)
 {
     int rc;
+    if (hap_space < 0) hap_space = space;
     if ((rc = phmm_checks::blocks(haps, reads, e->err)) != PHMM_OK) return rc;
-    if ((rc = fetch_offsets(e, haps->off, haps->n, space, s.hap_off_host)) != PHMM_OK) return rc;
+    if (hap_off_host) s.hap_off_host = *hap_off_host;
+    else if ((rc = fetch_offsets(e, haps->off, haps->n, hap_space, s.hap_off_host)) != PHMM_OK) return rc;
     for (int h = 0; h < haps->n; ++h) s.max_hap_len = std::max(s.max_hap_len, s.hap_off_host[h + 1] - s.hap_off_host[h]);
     OffsetSummary rs {};
     if (space == PHMM_SPACE_HOST) {
@@ -204,15 +208,15 @@ int stage_batch(phmm_engine* e, const phmm_haplotypes* haps, const phmm_reads* r
     DevReads& rd = s.rd;
     hp.n = haps->n; rd.n = reads->n;
     const long long* tmp_ll;
-    if ((rc = stage(e, e->h_off, (const long long*)haps->off, (size_t)haps->n + 1, space, &tmp_ll))) return rc; hp.off = tmp_ll;
-    if ((rc = stage(e, e->h_seq, haps->seq, s.hap_bases, space, &hp.seq))) return rc;
-    if ((rc = stage(e, e->h_mf, haps->snv_mask_fwd, s.hap_bases, space, &hp.mask_f))) return rc;
-    if ((rc = stage(e, e->h_pf, haps->snv_prior_fwd, s.hap_bases, space, &hp.prior_f))) return rc;
-    if ((rc = stage(e, e->h_mr, haps->snv_mask_rev, s.hap_bases, space, &hp.mask_r))) return rc;
-    if ((rc = stage(e, e->h_pr, haps->snv_prior_rev, s.hap_bases, space, &hp.prior_r))) return rc;
-    if ((rc = stage(e, e->h_go, haps->gap_open, s.hap_bases, space, &hp.gap_open))) return rc;
-    if ((rc = stage(e, e->h_ge, haps->gap_extend, s.hap_bases, space, &hp.gap_extend))) return rc;
-    if ((rc = stage(e, e->h_begin, (const long long*)haps->begin, haps->n, space, &tmp_ll))) return rc; hp.begin = tmp_ll;
+    if ((rc = stage(e, e->h_off, (const long long*)haps->off, (size_t)haps->n + 1, hap_space, &tmp_ll))) return rc; hp.off = tmp_ll;
+    if ((rc = stage(e, e->h_seq, haps->seq, s.hap_bases, hap_space, &hp.seq))) return rc;
+    if ((rc = stage(e, e->h_mf, haps->snv_mask_fwd, s.hap_bases, hap_space, &hp.mask_f))) return rc;
+    if ((rc = stage(e, e->h_pf, haps->snv_prior_fwd, s.hap_bases, hap_space, &hp.prior_f))) return rc;
+    if ((rc = stage(e, e->h_mr, haps->snv_mask_rev, s.hap_bases, hap_space, &hp.mask_r))) return rc;
+    if ((rc = stage(e, e->h_pr, haps->snv_prior_rev, s.hap_bases, hap_space, &hp.prior_r))) return rc;
+    if ((rc = stage(e, e->h_go, haps->gap_open, s.hap_bases, hap_space, &hp.gap_open))) return rc;
+    if ((rc = stage(e, e->h_ge, haps->gap_extend, s.hap_bases, hap_space, &hp.gap_extend))) return rc;
+    if ((rc = stage(e, e->h_begin, (const long long*)haps->begin, haps->n, hap_space, &tmp_ll))) return rc; hp.begin = tmp_ll;
     if ((rc = stage(e, e->r_off, (const long long*)reads->off, (size_t)reads->n + 1, space, &tmp_ll))) return rc; rd.off = tmp_ll;
     if ((rc = stage(e, e->r_bases, reads->bases, s.read_bases, space, &rd.bases))) return rc;
     if ((rc = stage(e, e->r_quals, reads->quals, s.read_bases, space, &rd.quals))) return rc;
@@ -734,15 +738,37 @@ int phmm_genotype_likelihoods(phmm_engine* e, const double* lnl, int32_t H, int3
 static constexpr size_t kResetScratchBudget = (size_t)1 << 30;
 static constexpr int kResetWarpsPerSm = 16;
 
-int phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int32_t n, const int64_t* off, const char* seq,
-                                 const uint8_t* is_substitution, char* snv_mask_fwd, int8_t* snv_prior_fwd, char* snv_mask_rev,
-                                 int8_t* snv_prior_rev, int8_t* gap_open, int8_t* gap_extend, int space)
+} // extern "C"
+
+// The six per-base arrays of phmm_haplotypes that reset() fills.
+struct ResetArrays {
+    char* mask_f; int8_t* prior_f; char* mask_r; int8_t* prior_r; int8_t* gap_open; int8_t* gap_extend;
+};
+
+// What phmm_engine_reset_haplotypes and the populate calls with an error model share: the checks, the staging of off / seq /
+// is_substitution, the model's upload, the scratch slots, k_reset_haplotypes and the host recompute of the haplotypes whose runs
+// overflow their slot, after the call's one synchronisation. Inputs in `space`. The arrays are written to `dev` (device memory) or,
+// with dev null, to the engine's h_mf .. h_ge; there haplotype h starts at off[h] - base, base = off[0] for host space and 0 for device
+// space. With `host` they are then copied to those host arrays (h at off[h]). *staged (optional) receives the device copies of off and
+// seq, the device arrays and the offsets on the host. n == 0 returns PHMM_OK without touching the GPU.
+struct ResetStaged { const int64_t* off = nullptr; const char* seq = nullptr; ResetArrays a {}; std::vector<long long> hoff; };
+
+// Run capacity of a haplotype's first attempt on the device. The haplotype's runs never come near phmm_reset::first_cap, so
+// PHMM_RESET_CAP (read once per process) can force a smaller one: a test hook that makes the host recompute of overflowed
+// haplotypes run. PHMM_TRACE reports how many haplotypes that recompute took.
+static uint32_t reset_first_cap(uint32_t longest)
 {
-    if (!e) return PHMM_ERR_INVALID;
-    e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
-    if (!m || n < 0 || (n > 0 && (!off || !seq || !snv_mask_fwd || !snv_prior_fwd || !snv_mask_rev || !snv_prior_rev || !gap_open || !gap_extend))) {
-        e->err = "null argument"; return PHMM_ERR_INVALID;
-    }
+    static const long long forced = [] {
+        const char* v = std::getenv("PHMM_RESET_CAP");
+        return v ? std::atoll(v) : 0LL;
+    }();
+    return forced > 0 ? (uint32_t)forced : phmm_reset::first_cap(longest);
+}
+
+static int reset_arrays(phmm_engine* e, const phmm_error_model* m, int32_t n, const int64_t* off, const char* seq, const uint8_t* is_substitution,
+                        int space, const ResetArrays* dev, const ResetArrays* host, ResetStaged* staged)
+{
+    if (!m || n < 0 || (n > 0 && (!off || !seq))) { e->err = "null argument"; return PHMM_ERR_INVALID; }
     if (space != PHMM_SPACE_HOST && space != PHMM_SPACE_DEVICE) { e->err = "bad memory space"; return PHMM_ERR_INVALID; }
     if (n == 0) return PHMM_OK;
     if (int rc0 = begin_call(e)) return rc0;
@@ -756,21 +782,22 @@ int phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int3
         L = std::max(L, hoff[h + 1] - hoff[h]);
     }
     if (L > 65535) { e->err = "haplotype longer than 65535 bases"; return PHMM_ERR_INVALID; }
-    // host space: the bases off[0] .. off[n] are staged and the outputs computed into engine buffers from index 0 = off[0]
+    // host space: the bases off[0] .. off[n] are staged and the outputs computed from index 0 = off[0]
     const long long base = space == PHMM_SPACE_HOST ? hoff[0] : 0;
-    const size_t B = (size_t)(hoff[n] - hoff[0]);
+    const size_t B = (size_t)(hoff[n] - base);
     const int64_t* d_off;
     const char* d_seq; const uint8_t* d_sub;
     if ((rc = stage(e, e->h_off, off, (size_t)n + 1, space, &d_off))) return rc;
     if ((rc = stage(e, e->h_seq, space == PHMM_SPACE_HOST ? seq + base : seq, B, space, &d_seq))) return rc;
     if ((rc = stage(e, e->rs_sub, is_substitution && space == PHMM_SPACE_HOST ? is_substitution + base : is_substitution, B, space, &d_sub))) return rc;
-    char *mf = snv_mask_fwd, *mr = snv_mask_rev;
-    int8_t *pf = snv_prior_fwd, *pr = snv_prior_rev, *go = gap_open, *ge = gap_extend;
-    if (space == PHMM_SPACE_HOST) {
+    ResetArrays d {};
+    if (dev) d = *dev;
+    else {
         DBuf* bufs[6] = {&e->h_mf, &e->h_pf, &e->h_mr, &e->h_pr, &e->h_go, &e->h_ge};
         for (DBuf* b : bufs) CU(b->ensure(std::max<size_t>(B, 1)));
-        mf = e->h_mf.as<char>(); pf = e->h_pf.as<int8_t>(); mr = e->h_mr.as<char>(); pr = e->h_pr.as<int8_t>(); go = e->h_go.as<int8_t>(); ge = e->h_ge.as<int8_t>();
+        d = {e->h_mf.as<char>(), e->h_pf.as<int8_t>(), e->h_mr.as<char>(), e->h_pr.as<int8_t>(), e->h_go.as<int8_t>(), e->h_ge.as<int8_t>()};
     }
+    if (staged) { staged->off = d_off; staged->seq = d_seq; staged->a = d; }
     // the model: fixed rows travel in the kernel argument, a custom model's motif tables in one device block
     phmm_reset::Model dm = phmm_reset::model_of(m);
     if (dm.custom) {
@@ -798,7 +825,7 @@ int phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int3
         CU(cudaMemcpyAsync(e->rs_model.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, e->stream));
     }
     // scratch slots sized for the longest haplotype
-    const uint32_t cap = phmm_reset::first_cap((uint32_t)L);
+    const uint32_t cap = reset_first_cap((uint32_t)L);
     const size_t slot_words = phmm_reset::scratch_words((uint32_t)L, cap);
     const size_t slot_bytes = slot_words * sizeof(uint32_t) + 2 * (size_t)cap * sizeof(phmm_reset::Run);
     const int resident = std::max(1, e->sm_count) * 2048;
@@ -811,21 +838,21 @@ int phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int3
     CU(e->rs_flags.ensure((size_t)n));
     CU(cudaEventRecord(e->ev0, e->stream));
     k_reset_haplotypes<<<(unsigned)((warps + 3) / 4), 128, 0, e->stream>>>(dm, n, (const long long*)d_off, base, (const unsigned char*)d_seq, d_sub,
-                                                                        mf, pf, mr, pr, go, ge, e->rs_words.as<uint32_t>(),
-                                                                        e->rs_runs.as<phmm_reset::Run>(), slot_words, cap, lanes, slots,
-                                                                        e->rs_flags.as<uint8_t>());
+                                                                        d.mask_f, d.prior_f, d.mask_r, d.prior_r, d.gap_open, d.gap_extend,
+                                                                        e->rs_words.as<uint32_t>(), e->rs_runs.as<phmm_reset::Run>(), slot_words,
+                                                                        cap, lanes, slots, e->rs_flags.as<uint8_t>());
     LAUNCHED();
     CU(cudaGetLastError());
     CU(cudaEventRecord(e->ev1, e->stream));
     std::vector<uint8_t> overflow((size_t)n);
     CU(cudaMemcpyAsync(overflow.data(), e->rs_flags.p, (size_t)n, cudaMemcpyDeviceToHost, e->stream));
-    if (space == PHMM_SPACE_HOST && B > 0) {
-        CU(cudaMemcpyAsync(snv_mask_fwd + base, mf, B, cudaMemcpyDeviceToHost, e->stream));
-        CU(cudaMemcpyAsync(snv_prior_fwd + base, pf, B, cudaMemcpyDeviceToHost, e->stream));
-        CU(cudaMemcpyAsync(snv_mask_rev + base, mr, B, cudaMemcpyDeviceToHost, e->stream));
-        CU(cudaMemcpyAsync(snv_prior_rev + base, pr, B, cudaMemcpyDeviceToHost, e->stream));
-        CU(cudaMemcpyAsync(gap_open + base, go, B, cudaMemcpyDeviceToHost, e->stream));
-        CU(cudaMemcpyAsync(gap_extend + base, ge, B, cudaMemcpyDeviceToHost, e->stream));
+    if (host && B > 0) {
+        CU(cudaMemcpyAsync(host->mask_f + base, d.mask_f, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(host->prior_f + base, d.prior_f, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(host->mask_r + base, d.mask_r, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(host->prior_r + base, d.prior_r, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(host->gap_open + base, d.gap_open, B, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(host->gap_extend + base, d.gap_extend, B, cudaMemcpyDeviceToHost, e->stream));
     }
     CU(cudaStreamSynchronize(e->stream));
     float ms = 0.f;
@@ -835,25 +862,52 @@ int phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int3
     const phmm_reset::Model& hm = phmm_reset::model_of(m);
     std::vector<unsigned char> s, sub;
     std::vector<int8_t> out;
+    if (std::getenv("PHMM_TRACE"))
+        std::fprintf(stderr, "[phmm %p] reset: %lld of %d haplotypes recomputed on the host\n", (void*)e,
+                     (long long)std::count(overflow.begin(), overflow.end(), (uint8_t)1), n);
     for (int h = 0; h < n; ++h) {
         if (!overflow[h]) continue;
         const long long o = hoff[h];
         const uint32_t len = (uint32_t)(hoff[h + 1] - o);
-        if (space == PHMM_SPACE_HOST) {
-            phmm_reset::reset_haplotype_host(hm, (const unsigned char*)seq + o, len, is_substitution ? is_substitution + o : nullptr, snv_mask_fwd + o,
-                                             snv_prior_fwd + o, snv_mask_rev + o, snv_prior_rev + o, gap_open + o, gap_extend + o, scratch);
+        const unsigned char* s_in = (const unsigned char*)seq + o;
+        const uint8_t* sub_in = is_substitution ? is_substitution + o : nullptr;
+        if (space == PHMM_SPACE_DEVICE) {
+            s.resize(len); sub.resize(len);
+            CU(cudaMemcpyAsync(s.data(), seq + o, len, cudaMemcpyDeviceToHost, e->stream));
+            if (is_substitution) CU(cudaMemcpyAsync(sub.data(), is_substitution + o, len, cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaStreamSynchronize(e->stream));
+            s_in = s.data(); sub_in = is_substitution ? sub.data() : nullptr;
+        }
+        if (host) {
+            phmm_reset::reset_haplotype_host(hm, s_in, len, sub_in, host->mask_f + o, host->prior_f + o, host->mask_r + o, host->prior_r + o,
+                                             host->gap_open + o, host->gap_extend + o, scratch);
             continue;
         }
-        s.resize(len); sub.resize(len); out.resize(6 * (size_t)len);
-        CU(cudaMemcpy(s.data(), seq + o, len, cudaMemcpyDeviceToHost));
-        if (is_substitution) CU(cudaMemcpy(sub.data(), is_substitution + o, len, cudaMemcpyDeviceToHost));
+        out.resize(6 * (size_t)len);
         int8_t* a = out.data();
-        phmm_reset::reset_haplotype_host(hm, s.data(), len, is_substitution ? sub.data() : nullptr, (char*)a, a + len, (char*)a + 2 * len, a + 3 * len,
-                                         a + 4 * len, a + 5 * len, scratch);
-        void* dst[6] = {snv_mask_fwd + o, snv_prior_fwd + o, snv_mask_rev + o, snv_prior_rev + o, gap_open + o, gap_extend + o};
-        for (int k = 0; k < 6; ++k) CU(cudaMemcpy(dst[k], a + (size_t)k * len, len, cudaMemcpyHostToDevice));
+        phmm_reset::reset_haplotype_host(hm, s_in, len, sub_in, (char*)a, a + len, (char*)a + 2 * len, a + 3 * len, a + 4 * len, a + 5 * len, scratch);
+        const long long at = o - base;
+        void* dst[6] = {d.mask_f + at, d.prior_f + at, d.mask_r + at, d.prior_r + at, d.gap_open + at, d.gap_extend + at};
+        for (int k = 0; k < 6; ++k) CU(cudaMemcpyAsync(dst[k], a + (size_t)k * len, len, cudaMemcpyHostToDevice, e->stream));
+        CU(cudaStreamSynchronize(e->stream));
     }
+    if (staged) staged->hoff = std::move(hoff);
     return PHMM_OK;
+}
+
+extern "C" {
+
+int phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int32_t n, const int64_t* off, const char* seq,
+                                 const uint8_t* is_substitution, char* snv_mask_fwd, int8_t* snv_prior_fwd, char* snv_mask_rev,
+                                 int8_t* snv_prior_rev, int8_t* gap_open, int8_t* gap_extend, int space)
+{
+    if (!e) return PHMM_ERR_INVALID;
+    e->err.clear(); e->launches_last = 0; e->last_dp_ms = 0.0; e->last_dp_cells = 0;
+    if (n > 0 && (!snv_mask_fwd || !snv_prior_fwd || !snv_mask_rev || !snv_prior_rev || !gap_open || !gap_extend)) { e->err = "null argument"; return PHMM_ERR_INVALID; }
+    const ResetArrays out {snv_mask_fwd, snv_prior_fwd, snv_mask_rev, snv_prior_rev, gap_open, gap_extend};
+    // device space: the kernel writes the caller's arrays; host space: the engine's buffers, copied back
+    return reset_arrays(e, m, n, off, seq, is_substitution, space, space == PHMM_SPACE_DEVICE ? &out : nullptr,
+                        space == PHMM_SPACE_HOST ? &out : nullptr, nullptr);
 }
 
 // -------------------------------------------------------------------------------------------------------------
@@ -1314,6 +1368,11 @@ struct PopulateCall {
     long long n_mapped = 0;
     const double* log_priors = nullptr;
     uint64_t* top = nullptr;
+    // the _reset entry points: `haps` holds the sequences block's n / off / seq / begin only; pop_reset derives the six arrays from
+    // the sequences under `model` on the device, and the call populates from those
+    bool reset = false;
+    const phmm_error_model* model = nullptr;
+    const uint8_t* is_substitution = nullptr;
 
     bool listed() const { return positions && positions->off && positions->pos; }
     bool assign() const { return staged != nullptr; }
@@ -1332,6 +1391,8 @@ static PopulateCall one_region_call(const phmm_config* cfg, const phmm_haplotype
 
 // What the phases of populate_impl share: the kernels' parameter block and the host-side sizes and decisions behind it.
 struct PopState {
+    phmm_haplotypes reset_haps {};              // pop_reset: the derived block, device-resident, and its offsets on the host
+    std::vector<long long> reset_off_host;
     Staged s;
     PopParams p {};
     int band = 0, G = 0, R = 0;
@@ -1370,6 +1431,22 @@ struct PopState {
     }
 };
 
+// Phase 0, calls with an error model only: reset() for every haplotype on the device (reset_arrays, one synchronisation) into the
+// engine's buffers, and the device-resident haplotype block over them that the rest of the call stages.
+static int pop_reset(phmm_engine* e, const PopulateCall& c, PopState& st)
+{
+    const phmm_haplotypes* h = c.haps;
+    ResetStaged r;
+    int rc = reset_arrays(e, c.model, h->n, h->off, h->seq, c.is_substitution, c.space, nullptr, nullptr, &r);
+    if (rc != PHMM_OK) return rc;
+    e->last_dp_ms = 0.0;                        // the call's DP kernel time is populate's alone
+    const long long* d_begin = nullptr;
+    if (h->n > 0 && (rc = stage(e, e->h_begin, (const long long*)h->begin, (size_t)h->n, c.space, &d_begin))) return rc;
+    st.reset_haps = {h->n, r.off, r.seq, r.a.mask_f, r.a.prior_f, r.a.mask_r, r.a.prior_r, r.a.gap_open, r.a.gap_extend, (const int64_t*)d_begin};
+    st.reset_off_host = std::move(r.hoff);
+    return PHMM_OK;
+}
+
 // Phase 1: the checks a call can fail before any device work, then the batch, the regions and the per-read region / result slot
 // on the device.
 static int pop_stage(phmm_engine* e, const PopulateCall& c, PopState& st)
@@ -1381,6 +1458,7 @@ static int pop_stage(phmm_engine* e, const PopulateCall& c, PopState& st)
     if (c.template_off && several) { e->err = "templates are not supported with several regions"; return PHMM_ERR_INVALID; }
     Staged& s = st.s;
     if (c.assign()) s = *c.staged;
+    else if (c.reset) rc = stage_batch(e, &st.reset_haps, c.reads, c.space, s, false, true, PHMM_SPACE_DEVICE, &st.reset_off_host);
     else rc = stage_batch(e, c.haps, c.reads, c.space, s, false, true);
     if (rc != PHMM_OK) return rc;
     const int band = st.band = round_band(std::max(1, c.cfg->max_indel_error));
@@ -1973,6 +2051,7 @@ static int populate_impl(phmm_engine* e, const PopulateCall& c)
 {
     PopState st;
     int rc;
+    if (c.reset && (rc = pop_reset(e, c, st))) return rc;
     if ((rc = pop_stage(e, c, st))) return rc;
     st.lap(e, "staged");
     if ((rc = pop_candidates(e, c, st))) return rc;
@@ -2123,20 +2202,40 @@ int phmm_populate_templates(phmm_engine* e, const phmm_config* cfg,
     return populate_impl(e, c);
 }
 
+} // extern "C"
+
+// Whether phmm_populate runs a call as its pipeline: a host-resident batch, no caller-supplied position lists (a [H][R] CSR cannot be
+// sliced by columns without a pass over it), enough pairs to amortise the per-chunk overheads.
+static bool pipelined(const phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                      const phmm_positions* positions, const double* out, int space)
+{
+    const long long all_pairs = (haps && reads) ? (long long)haps->n * reads->n : 0;
+    return !e->is_sub && space == PHMM_SPACE_HOST && haps && reads && cfg && out && haps->n > 0 && reads->n > 1 && reads->off && reads->mapq &&
+           reads->reverse && !(positions && positions->off && positions->pos) && all_pairs >= 2 * phmm_checks::populate_chunk_pairs(all_pairs);
+}
+
+// A sequences block as the haplotype block of a _reset call before pop_reset has derived its arrays.
+static phmm_haplotypes sequences_block(const phmm_haplotype_sequences* seqs)
+{
+    return phmm_haplotypes {seqs->n, seqs->off, seqs->seq, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, seqs->begin};
+}
+
+static PopulateCall& with_model(PopulateCall& c, const phmm_error_model* m, const phmm_haplotype_sequences* seqs)
+{
+    c.reset = true; c.model = m; c.is_substitution = seqs->is_substitution;
+    return c;
+}
+
+extern "C" {
+
 int phmm_populate(phmm_engine* e, const phmm_config* cfg,
                   const phmm_haplotypes* haps, const phmm_reads* reads,
                   const phmm_positions* positions, const phmm_flank_state* flank,
                   double* out, int32_t* status, int space)
 {
     if (int rc = begin_call(e)) return rc;
-    // Pipelined path: host-resident batch, no caller-supplied position lists (a [H][R] CSR cannot be sliced by columns
-    // without a pass over it), enough pairs to amortise the per-chunk overheads.
-    const long long all_pairs = (haps && reads) ? (long long)haps->n * reads->n : 0;
-    const long long kChunkPairs = phmm_checks::populate_chunk_pairs(all_pairs);
-    const bool can_chunk = !e->is_sub && space == PHMM_SPACE_HOST && haps && reads && cfg && out && haps->n > 0 && reads->n > 1 &&
-                           reads->off && reads->mapq && reads->reverse && !(positions && positions->off && positions->pos) &&
-                           all_pairs >= 2 * kChunkPairs;
-    if (!can_chunk) return populate_impl(e, one_region_call(cfg, haps, reads, positions, flank, out, status, space));
+    if (!pipelined(e, cfg, haps, reads, positions, out, space)) return populate_impl(e, one_region_call(cfg, haps, reads, positions, flank, out, status, space));
+    const long long kChunkPairs = phmm_checks::populate_chunk_pairs((long long)haps->n * reads->n);
     for (phmm_engine*& sub : e->sub) {
         if (!sub) {
             const int rc = phmm_create(&sub, e->device);
@@ -2195,6 +2294,57 @@ int phmm_populate(phmm_engine* e, const phmm_config* cfg,
     for (int k = 0; k < 2; ++k) if (rcs[k] != PHMM_OK && rcs[k] != PHMM_ERR_SHORT_HAPLOTYPE) { e->err = errs[k]; return rcs[k]; }
     for (int k = 0; k < 2; ++k) if (rcs[k] == PHMM_ERR_SHORT_HAPLOTYPE) { e->err = errs[k]; return rcs[k]; }
     return PHMM_OK;
+}
+
+int phmm_populate_reset(phmm_engine* e, const phmm_config* cfg, const phmm_error_model* m, const phmm_haplotype_sequences* seqs,
+                        const phmm_reads* reads, const phmm_positions* positions, const phmm_flank_state* flank,
+                        double* out, int32_t* status, int space)
+{
+    if (int rc = begin_call(e)) return rc;
+    if (!seqs) { e->err = "null argument"; return PHMM_ERR_INVALID; }
+    const phmm_haplotypes shell = sequences_block(seqs);
+    if (!pipelined(e, cfg, &shell, reads, positions, out, space)) {
+        PopulateCall c = one_region_call(cfg, &shell, reads, positions, flank, out, status, space);
+        return populate_impl(e, with_model(c, m, seqs));
+    }
+    // the pipeline takes a host block: the arrays once, on the device, then phmm_populate's pipeline
+    const size_t B = seqs->off ? (size_t)std::max<int64_t>(seqs->off[seqs->n], 0) : 0;
+    std::vector<int8_t> arrays(6 * std::max<size_t>(B, 1));
+    int8_t* a = arrays.data();
+    const size_t k = std::max<size_t>(B, 1);
+    const ResetArrays host {(char*)a, a + k, (char*)a + 2 * k, a + 3 * k, a + 4 * k, a + 5 * k};
+    const int rc = reset_arrays(e, m, seqs->n, seqs->off, seqs->seq, seqs->is_substitution, space, nullptr, &host, nullptr);
+    if (rc != PHMM_OK) return rc;
+    const phmm_haplotypes haps {seqs->n, seqs->off, seqs->seq, host.mask_f, host.prior_f, host.mask_r, host.prior_r, host.gap_open, host.gap_extend, seqs->begin};
+    return phmm_populate(e, cfg, &haps, reads, positions, flank, out, status, space);
+}
+
+int phmm_populate_regions_reset(phmm_engine* e, const phmm_config* cfg, const phmm_error_model* m, const phmm_haplotype_sequences* seqs,
+                                const phmm_reads* reads, const phmm_regions* regions, double* out, int32_t* status, int space)
+{
+    int rc;
+    if ((rc = begin_call(e))) return rc;
+    if (!seqs) { e->err = "null argument"; return PHMM_ERR_INVALID; }
+    const phmm_haplotypes shell = sequences_block(seqs);
+    PopulateCall c;
+    c.cfg = cfg; c.haps = &shell; c.reads = reads; c.space = space;
+    c.out = out; c.status = status;
+    if ((rc = region_setup(e, cfg, &shell, reads, regions, c.regions)) != PHMM_OK) return rc;
+    return populate_impl(e, with_model(c, m, seqs));
+}
+
+int phmm_populate_templates_reset(phmm_engine* e, const phmm_config* cfg, const phmm_error_model* m, const phmm_haplotype_sequences* seqs,
+                                  const phmm_reads* reads, const int64_t* template_off, int32_t n_templates,
+                                  const phmm_positions* positions, const phmm_flank_state* flank, double* out, int32_t* status, int space)
+{
+    int rc;
+    if ((rc = begin_call(e))) return rc;
+    if (!seqs) { e->err = "null argument"; return PHMM_ERR_INVALID; }
+    if ((rc = phmm_checks::template_offsets(template_off, n_templates, reads, space == PHMM_SPACE_HOST, e->err)) != PHMM_OK) return rc;
+    const phmm_haplotypes shell = sequences_block(seqs);
+    PopulateCall c = one_region_call(cfg, &shell, reads, positions, flank, out, status, space);
+    c.template_off = template_off; c.n_templates = n_templates;
+    return populate_impl(e, with_model(c, m, seqs));
 }
 
 } // extern "C"

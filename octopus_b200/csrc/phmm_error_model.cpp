@@ -71,9 +71,41 @@ struct phmm_error_model {
     phmm_reset::Model core;                      // what the shared core reads; the custom tables point into the vectors below
     MotifMap custom_open, custom_extend;         // a custom model as parsed (their iteration order picks the defaults)
     FlatMotifs flat_open, flat_extend;
+    std::string key;                             // phmm_reset::model_key
 };
 
 const phmm_reset::Model& phmm_reset::model_of(const phmm_error_model* m) { return m->core; }
+const std::string& phmm_reset::model_key(const phmm_error_model* m) { return m->key; }
+
+namespace {
+
+// Everything the core reads, as bytes: the flags, the fixed rows, the defaults and a custom model's flattened motif tables. A model
+// that holds a penalty outside [0,127] gets the empty key.
+void set_key(phmm_error_model& m)
+{
+    const phmm_reset::Model& c = m.core;
+    std::string& k = m.key;
+    k.clear();
+    bool in_range = c.default_open >= 0 && c.default_extend >= 0;
+    auto bytes = [&](const void* p, std::size_t n) { k.append(static_cast<const char*>(p), n); };
+    auto penalties = [&](const Penalty* p, std::size_t n) { for (std::size_t i = 0; i < n; ++i) in_range = in_range && p[i] >= 0; bytes(p, n); };
+    const char flags[3] = {(char)c.custom, (char)c.custom_has_extend, (char)c.has_snv};
+    bytes(flags, sizeof(flags));
+    for (const phmm_reset::PaddedRow<50>* r : {&c.open_at, &c.open_cg, &c.open_di, &c.open_tri, &c.ext_homo, &c.ext_di, &c.ext_tri}) penalties(r->v, 50);
+    for (const phmm_reset::PaddedRow<51>& r : c.caps) penalties(r.v, 51);
+    penalties(&c.default_open, 1);
+    penalties(&c.default_extend, 1);
+    for (const FlatMotifs* f : {&m.flat_open, &m.flat_extend}) {
+        const std::uint64_t n = f->key.size();
+        bytes(&n, sizeof(n));
+        bytes(f->key.data(), f->key.size() * sizeof(std::uint64_t));
+        bytes(f->row.data(), f->row.size() * sizeof(std::uint32_t));
+        penalties(f->data.data(), f->data.size());
+    }
+    if (!in_range) k.clear();
+}
+
+} // namespace
 
 namespace {
 
@@ -247,6 +279,7 @@ int phmm_error_model_create(phmm_error_model** out, const char* label)
     c.default_open = c.open_di.v[0];             // complex_open_penalty_ (basic_…:32-33)
     c.default_extend = c.ext_di.v[0];
     if (sequencer != 6 && sequencer != 7) set_snv(c, library);   // no SNV model for PacBio (error_model_factory.cpp:492-495)
+    set_key(*m);
     *out = m;
     return PHMM_OK;
 }
@@ -271,6 +304,7 @@ int phmm_error_model_create_custom(phmm_error_model** out, const char* model_tex
     c.custom_open = m->flat_open.view();
     c.custom_extend = m->flat_extend.view();
     set_snv(c, 1);                               // make_snv_error_model(default_model_config) (:587)
+    set_key(*m);
     *out = m;
     return PHMM_OK;
 }

@@ -21,6 +21,7 @@
 #include <cstddef>
 #include <cstdint>
 
+#include <string>
 #include <vector>
 
 #if defined(__CUDACC__)
@@ -700,6 +701,9 @@ struct phmm_error_model;
 namespace phmm_reset {
 // The flattened model of a phmm_error_model (its arrays live as long as the model). Defined in phmm_error_model.cpp.
 const Model& model_of(const phmm_error_model* m);
+// The model's content as bytes: models with equal keys give equal arrays for every sequence, so the request batcher merges their
+// requests. Empty when the model holds a penalty outside [0,127] (populate refuses such arrays): those requests run alone.
+const std::string& model_key(const phmm_error_model* m);
 // Host scratch that grows on demand: a haplotype whose runs overflow is recomputed with twice the capacity.
 struct HostScratch
 {
