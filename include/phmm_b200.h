@@ -337,7 +337,7 @@ typedef struct {
     int64_t gpu_calls;             /* engine calls: batches + requests run alone */
     int64_t merged_calls;          /* calls that carried more than one request */
     int64_t max_regions_per_call;  /* most requests in one call */
-    int64_t dp_cells;              /* phmm_last_dp_cells summed over the calls */
+    int64_t dp_cells;              /* phmm_last_dp_cells summed over the calls (the reruns below included) */
 } phmm_batcher_stats;
 
 /* device < 0: current CUDA device. opt NULL = defaults (clients 0, max_wait_us 500). PHMM_ERR_CUDA without a usable H100. */
@@ -355,6 +355,39 @@ int  phmm_batcher_populate_templates(phmm_batcher* b, const phmm_config* cfg, co
                                      const int64_t* template_off, int32_t n_templates, const phmm_flank_state* flank,
                                      double* out, int32_t* status);
 int  phmm_batcher_stats_get(const phmm_batcher* b, phmm_batcher_stats* out);
+
+/* Read assignment and realignment through the shared engine: compute_haplotype_support and ReadRealigner::realign come from the same
+ * region threads as populate, one small call per genotype or haplotype. Thread-safe and blocking; host memory. Arguments as
+ * phmm_assign_reads / phmm_realign_reads with space = PHMM_SPACE_HOST. They follow the policy above (leader, clients, max_wait_us,
+ * one engine call at a time, in turn with populate and mutation calls), each kind with a staging of its own.
+ *
+ * Contract: a request's return code and outputs are bit for bit what the plain call returns for it alone on its own engine: top, lnl
+ * and status of an assign request (for one that returns PHMM_ERR_SHORT_HAPLOTYPE its statuses; its top is unspecified, as alone), and
+ * mapping_position, likelihood, status and the CIGAR text up to its NUL of a realign request. Every request is checked on its own
+ * thread, with the plain call's checks and messages, before it joins a batch; a failing request returns at once and never changes
+ * another request's result. Errors of the whole call (CUDA, NOMEM) go to every member.
+ *
+ * Assign: a batch is one phmm_assign_reads call, the members' groups one after the other; requests with identical configs merge
+ * (a request without log_priors is staged with zeros, which give the same top and lnl). A request with more than 65535 haplotypes,
+ * more (read, haplotype) pairs than the batch budget, a haplotype longer than 65535 bp or a penalty outside [0,127] runs alone.
+ * Realign: a batch is one phmm_realign_reads call; requests merge when their configs and the flank state the call uses (none unless
+ * has_flank and cfg->use_flank_state) are equal, whatever their cigar_stride. The batch runs at its largest stride and each member
+ * gets its text at its own stride, with PHMM_STATUS_CIGAR_TRUNCATED and the truncated text where it would not have fitted alone. The
+ * batch's page-locked CIGAR staging is sized by the bytes the call writes, its pairs x its largest stride, at most 128 MiB. A request
+ * with more pairs or CIGAR bytes than the batch budget, or whose stride could not hold a single-run CIGAR of its longest read, runs
+ * alone.
+ *
+ * A merged call can fail where its members alone would not: phmm_assign_reads fails the whole call when one (haplotype, read) pair
+ * has more than 4096 mapping positions. When a merged call returns PHMM_ERR_INVALID, its leader reruns every member alone in the
+ * same turn on the engine, so that each gets its own result and message. phmm_batcher_reruns counts such merged calls; their
+ * reruns count in gpu_calls, and the DP cells of the failed call and of the reruns in dp_cells. */
+int  phmm_batcher_assign_reads(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                               const phmm_regions* groups, const double* log_priors, uint64_t* top, double* lnl, int32_t* status);
+int  phmm_batcher_realign_reads(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                                const phmm_pair* pairs, int64_t n_pairs, const phmm_flank_state* flank,
+                                int64_t* mapping_position, double* likelihood, char* cigar, int32_t cigar_stride, int32_t* status);
+/* Merged calls rerun one request at a time since creation (kept out of phmm_batcher_stats, whose layout callers compile against). */
+int64_t phmm_batcher_reruns(const phmm_batcher* b);
 
 /* Consumer of the matrix ("next" row N1): ConstantMixtureGenotypeLikelihoodModel::evaluate for G genotypes of one ploidy
  * (core/models/genotype/constant_mixture_genotype_likelihood_model.cpp:30-140) over a [H][R] matrix in `space`:

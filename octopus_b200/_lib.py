@@ -18,7 +18,8 @@ EXPORTS = ["phmm_version", "phmm_default_config", "phmm_create", "phmm_destroy",
            "phmm_populate_ld", "phmm_device_alloc", "phmm_device_free", "phmm_ipc_export", "phmm_ipc_open", "phmm_ipc_close",
            "phmm_batcher_create", "phmm_batcher_destroy", "phmm_batcher_last_error", "phmm_batcher_populate",
            "phmm_batcher_populate_templates", "phmm_batcher_stats_get", "phmm_populate_reset", "phmm_populate_regions_reset",
-           "phmm_populate_templates_reset", "phmm_batcher_populate_reset", "phmm_batcher_populate_templates_reset"]
+           "phmm_populate_templates_reset", "phmm_batcher_populate_reset", "phmm_batcher_populate_templates_reset",
+           "phmm_batcher_assign_reads", "phmm_batcher_realign_reads", "phmm_batcher_reruns"]
 
 
 class Config(C.Structure):
@@ -155,6 +156,14 @@ def load():
                                                     C.c_int32, C.POINTER(FlankState), C.c_void_p, C.c_void_p]
     lib.phmm_batcher_stats_get.restype = C.c_int
     lib.phmm_batcher_stats_get.argtypes = [C.c_void_p, C.POINTER(BatcherStats)]
+    lib.phmm_batcher_reruns.restype = C.c_int64
+    lib.phmm_batcher_reruns.argtypes = [C.c_void_p]
+    lib.phmm_batcher_assign_reads.restype = C.c_int
+    lib.phmm_batcher_assign_reads.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.POINTER(Regions),
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.phmm_batcher_realign_reads.restype = C.c_int
+    lib.phmm_batcher_realign_reads.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p,
+                                               C.c_int64, C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
     lib.phmm_populate_ld.restype = C.c_int
     lib.phmm_populate_ld.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads),
                                      C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_int64, C.c_void_p]

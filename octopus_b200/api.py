@@ -167,6 +167,38 @@ class _Alignments:
         return self.mp, self.lk, [text[j * s:(j + 1) * s].split(b"\0", 1)[0].decode() for j in range(self.n)], self.st
 
 
+def _realign(call, handle, sp, config, haps, reads, pairs, flank_state, cigar_stride, *space):
+    """One realign call (phmm_realign_reads or phmm_batcher_realign_reads; `space` the engine's trailing memory-space argument):
+    (return code, the result PairHMMEngine.realign_reads returns)."""
+    pr = sp.input(pairs, np.int32).reshape(-1, 2)
+    n = pr.shape[0]
+    res = _Alignments(sp, reads, n, cigar_stride)
+    rc = call(handle, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), sp.ptr(pr), n, _ref(_flank(flank_state)),
+              *res.pointers(), *space)
+    return rc, res.result()
+
+
+def _assign(call, handle, sp, config, haps, reads, hap_first, read_first, log_priors, want_likelihoods, want_status, *space):
+    """One assign call (phmm_assign_reads or phmm_batcher_assign_reads; `space` the engine's trailing memory-space argument):
+    (return code, the result PairHMMEngine.assign_reads returns)."""
+    regs, off = _regions(hap_first, read_first)
+    total = int(off[-1])
+    top = sp.empty(reads.n, np.int64 if sp.on_device else np.uint64)
+    lnl = sp.empty(total, np.float64) if want_likelihoods else None
+    status = sp.empty(total, np.int32) if want_status else None
+    pri = None if log_priors is None else sp.input(log_priors, np.float64)
+    if pri is not None and pri.shape[0] != haps.n:
+        raise ValueError("log_priors needs one value per haplotype of the block")
+    rc = call(handle, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), C.byref(regs), sp.ptr(pri), sp.ptr(top),
+              sp.ptr(lnl), sp.ptr(status), *space)
+    out = (top,)
+    if want_likelihoods:
+        out += (lnl,)
+    if want_status:
+        out += (status,)
+    return rc, out[0] if len(out) == 1 else out
+
+
 def _grow(attempt, cap):
     """attempt(cap) → (size needed, result). Most calls fit the first guess; a second call takes the exact size."""
     while True:
@@ -363,12 +395,9 @@ class PairHMMEngine(_Handle):
         only). pairs: (n, 2) int32 rows (read, hap). Returns (mapping_position[n], likelihood[n], cigars[list of str], status[n]) as
         align_reads; for device-resident blocks the three arrays are torch CUDA tensors."""
         sp = _Space.of(haps, reads)
-        pr = sp.input(pairs, np.int32).reshape(-1, 2)
-        n = pr.shape[0]
-        res = _Alignments(sp, reads, n, cigar_stride)
-        self._check(self._lib.phmm_realign_reads(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), sp.ptr(pr),
-                                                 n, _ref(_flank(flank_state)), *res.pointers(), sp.flag))
-        return res.result()
+        rc, res = _realign(self._lib.phmm_realign_reads, self._h, sp, config, haps, reads, pairs, flank_state, cigar_stride, sp.flag)
+        self._check(rc)
+        return res
 
     def genotype_likelihoods(self, lnl, genotypes):
         """ConstantMixtureGenotypeLikelihoodModel::evaluate for every row of `genotypes` ((G, ploidy) haplotype indices) over the
@@ -420,22 +449,10 @@ class PairHMMEngine(_Handle):
         want_status: numpy for host blocks, torch CUDA tensors for device-resident ones (top then as int64 with the same bits). With want_status a short haplotype does not
         raise; its statuses carry the extension and top is unspecified."""
         sp = _Space.of(haps, reads)
-        regs, off = _regions(hap_first, read_first)
-        total = int(off[-1])
-        top = sp.empty(reads.n, np.int64 if sp.on_device else np.uint64)
-        lnl = sp.empty(total, np.float64) if want_likelihoods else None
-        status = sp.empty(total, np.int32) if want_status else None
-        pri = None if log_priors is None else sp.input(log_priors, np.float64)
-        if pri is not None and pri.shape[0] != haps.n:
-            raise ValueError("log_priors needs one value per haplotype of the block")
-        self._check(self._lib.phmm_assign_reads(self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), C.byref(regs),
-                                                sp.ptr(pri), sp.ptr(top), sp.ptr(lnl), sp.ptr(status), sp.flag), want_status)
-        out = (top,)
-        if want_likelihoods:
-            out += (lnl,)
-        if want_status:
-            out += (status,)
-        return out[0] if len(out) == 1 else out
+        rc, res = _assign(self._lib.phmm_assign_reads, self._h, sp, config, haps, reads, hap_first, read_first, log_priors, want_likelihoods,
+                          want_status, sp.flag)
+        self._check(rc, want_status)
+        return res
 
     @staticmethod
     def split_regions(flat, off, hap_first, read_first):
@@ -475,9 +492,10 @@ class PairHMMEngine(_Handle):
 
 class PopulateBatcher(_Handle):
     """One engine shared by many host threads (phmm_batcher_*): the populate requests that concurrent threads have in flight run
-    as one multi-region kernel chain, their mutation-prime requests as one multi-set call. Calls are thread-safe and block; ctypes
-    releases the GIL during them, so Python threads really do wait together. Each result equals what ``PairHMMEngine.populate`` /
-    ``mutation_prime`` returns for the request alone. Host blocks only."""
+    as one multi-region kernel chain, their mutation-prime requests as one multi-set call, their assign and realign requests as one
+    assign / realign call. Calls are thread-safe and block; ctypes releases the GIL during them, so Python threads really do wait
+    together. Each result equals what ``PairHMMEngine.populate`` / ``mutation_prime`` / ``assign_reads`` / ``realign_reads`` returns
+    for the request alone. Host blocks only."""
     _destroy = "phmm_batcher_destroy"
 
     def __init__(self, device=-1, clients=0, max_wait_us=None):
@@ -496,6 +514,11 @@ class PopulateBatcher(_Handle):
         if rc != _lib.PHMM_OK:
             raise PhmmError(rc, "stats")
         return {f: int(getattr(s, f)) for f, _ in _lib.BatcherStats._fields_}
+
+    def reruns(self):
+        """Merged assign / realign calls that failed with PHMM_ERR_INVALID (one request's more than 4096 mapping positions) and were
+        rerun one request at a time, so that each request got its own result (phmm_batcher_reruns)."""
+        return int(self._lib.phmm_batcher_reruns(self._h))
 
     def populate(self, config, haps: HaplotypeBlock, reads: ReadBlock, positions=None, flank_state=None, want_status=False, error_model=None):
         """As PairHMMEngine.populate for host blocks: the (H, R) matrix (and the status matrix with want_status). With
@@ -521,6 +544,24 @@ class PopulateBatcher(_Handle):
         self._check(_call(self._lib, "phmm_batcher_populate_templates", self._h, config, haps, error_model, C.byref(reads.c_struct()),
                           toff.ctypes.data, T, _ref(_flank(flank_state)), _ptr(out), _ptr(status)), want_status)
         return (out, status) if want_status else out
+
+    def assign_reads(self, config, haps: HaplotypeBlock, reads: ReadBlock, hap_first, read_first, log_priors=None, want_likelihoods=False,
+                     want_status=False):
+        """As PairHMMEngine.assign_reads for host blocks (phmm_batcher_assign_reads): concurrent requests with equal configs run as one
+        call, each with the top sets, likelihoods and statuses it gets alone."""
+        assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
+        rc, res = _assign(self._lib.phmm_batcher_assign_reads, self._h, _HOST, config, haps, reads, hap_first, read_first, log_priors,
+                          want_likelihoods, want_status)
+        self._check(rc, want_status)
+        return res
+
+    def realign_reads(self, config, haps: HaplotypeBlock, reads: ReadBlock, pairs, flank_state=None, cigar_stride=None):
+        """As PairHMMEngine.realign_reads for host blocks (phmm_batcher_realign_reads): concurrent requests with equal configs and
+        flank states run as one call whatever their CIGAR strides, each with the result it gets alone at its own stride."""
+        assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
+        rc, res = _realign(self._lib.phmm_batcher_realign_reads, self._h, _HOST, config, haps, reads, pairs, flank_state, cigar_stride)
+        self._check(rc)
+        return res
 
     def mutation_prime(self, model, sequences):
         """As PairHMMEngine.mutation_prime, through the shared engine: concurrent requests whose models are equal by content run as

@@ -63,6 +63,70 @@ private:
     unsigned band_;
 };
 
+namespace detail {
+
+// ReadRealigner::realign's per-read step for every pair (phmm_realign_reads / phmm_batcher_realign_reads). Statuses as
+// phmm_align_reads (PHMM_STATUS_*; SHORT_HAP carries the required extension in the high 16 bits); host memory.
+struct PairAlignments
+{
+    std::vector<std::int64_t> mapping_position;
+    std::vector<double> likelihood;
+    std::vector<std::string> cigar;
+    std::vector<std::int32_t> status;
+};
+
+// The outputs of one realign call at the adapter's CIGAR stride (4 x the longest read + 64); call(stride, mapping_position,
+// likelihood, text, status) makes the call and throws on failure.
+template <typename Call>
+PairAlignments realign_reads(const phmm_reads& reads, std::size_t n, Call&& call)
+{
+    std::int64_t longest = 1;
+    for (std::int32_t r = 0; r < reads.n; ++r) longest = std::max<std::int64_t>(longest, reads.off[r + 1] - reads.off[r]);
+    const auto stride = static_cast<std::int32_t>(4 * longest + 64);
+    PairAlignments a;
+    a.mapping_position.resize(n); a.likelihood.resize(n); a.status.resize(n);
+    std::vector<char> text(std::max<std::size_t>(n, 1) * static_cast<std::size_t>(stride), 0);
+    call(stride, a.mapping_position.data(), a.likelihood.data(), text.data(), a.status.data());
+    a.cigar.reserve(n);
+    for (std::size_t j = 0; j < n; ++j) a.cigar.emplace_back(text.data() + j * static_cast<std::size_t>(stride));
+    return a;
+}
+
+// compute_haplotype_support's scoring and choice for many genotypes (phmm_assign_reads / phmm_batcher_assign_reads); host memory.
+// top[r] bit k = group-local haplotype k is in read r's find_map_haplotypes set. likelihood / status: the groups' [H_g][R_g]
+// matrices back to back. A short haplotype does not throw here: the code is PHMM_ERR_SHORT_HAPLOTYPE and the statuses carry the
+// extension.
+struct ReadAssignment
+{
+    std::vector<std::uint64_t> top;
+    std::vector<double> likelihood;
+    std::vector<std::int32_t> status;
+    int code = PHMM_OK;
+};
+
+// The outputs of one assign call; call(groups, priors, top, likelihood, status) returns the call's code.
+template <typename Call>
+ReadAssignment assign_reads(const phmm_haplotypes& haplotypes, const phmm_reads& reads, const std::vector<std::int32_t>& hap_first,
+                            const std::vector<std::int32_t>& read_first, const std::vector<double>* log_priors, bool want_likelihoods,
+                            Call&& call)
+{
+    if (hap_first.empty() || hap_first.size() != read_first.size()) throw Error {PHMM_ERR_INVALID, "group bounds need n + 1 entries each"};
+    const auto n = static_cast<std::int32_t>(hap_first.size() - 1);
+    if (log_priors && log_priors->size() != static_cast<std::size_t>(haplotypes.n)) throw Error {PHMM_ERR_INVALID, "one log prior per haplotype"};
+    std::size_t pairs = 0;
+    for (std::int32_t g = 0; g < n; ++g)
+        pairs += static_cast<std::size_t>(std::max(0, hap_first[g + 1] - hap_first[g])) * static_cast<std::size_t>(std::max(0, read_first[g + 1] - read_first[g]));
+    const phmm_regions groups {n, hap_first.data(), read_first.data(), nullptr};
+    ReadAssignment a;
+    a.top.resize(static_cast<std::size_t>(std::max(0, reads.n)));
+    a.status.resize(pairs);
+    if (want_likelihoods) a.likelihood.resize(pairs);
+    a.code = call(groups, log_priors ? log_priors->data() : nullptr, a.top.data(), want_likelihoods ? a.likelihood.data() : nullptr, a.status.data());
+    return a;
+}
+
+} // namespace detail
+
 class Engine
 {
 public:
@@ -98,59 +162,27 @@ public:
         }
     }
 
-    // ReadRealigner::realign's per-read step for every pair (phmm_realign_reads). Statuses as phmm_align_reads (PHMM_STATUS_*;
-    // SHORT_HAP carries the required extension in the high 16 bits); host memory.
-    struct PairAlignments
-    {
-        std::vector<std::int64_t> mapping_position;
-        std::vector<double> likelihood;
-        std::vector<std::string> cigar;
-        std::vector<std::int32_t> status;
-    };
+    // ReadRealigner::realign's per-read step for every pair (phmm_realign_reads); detail::PairAlignments.
+    using PairAlignments = detail::PairAlignments;
     PairAlignments realign_reads(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
                                  const std::vector<phmm_pair>& pairs, const phmm_flank_state* flank_state = nullptr) const
     {
-        const std::size_t n = pairs.size();
-        std::int64_t longest = 1;
-        for (std::int32_t r = 0; r < reads.n; ++r) longest = std::max<std::int64_t>(longest, reads.off[r + 1] - reads.off[r]);
-        const auto stride = static_cast<std::int32_t>(4 * longest + 64);
-        PairAlignments a;
-        a.mapping_position.resize(n); a.likelihood.resize(n); a.status.resize(n);
-        std::vector<char> text(std::max<std::size_t>(n, 1) * static_cast<std::size_t>(stride), 0);
-        check(phmm_realign_reads(get(), &config, &haplotypes, &reads, pairs.data(), static_cast<std::int64_t>(n), flank_state,
-                                 a.mapping_position.data(), a.likelihood.data(), text.data(), stride, a.status.data(), PHMM_SPACE_HOST));
-        a.cigar.reserve(n);
-        for (std::size_t j = 0; j < n; ++j) a.cigar.emplace_back(text.data() + j * static_cast<std::size_t>(stride));
-        return a;
+        return detail::realign_reads(reads, pairs.size(), [&] (std::int32_t stride, std::int64_t* mp, double* lk, char* text, std::int32_t* st) {
+            check(phmm_realign_reads(get(), &config, &haplotypes, &reads, pairs.data(), static_cast<std::int64_t>(pairs.size()), flank_state,
+                                     mp, lk, text, stride, st, PHMM_SPACE_HOST));
+        });
     }
 
-    // compute_haplotype_support's scoring and choice for many genotypes (phmm_assign_reads); host memory. top[r] bit k = group-local
-    // haplotype k is in read r's find_map_haplotypes set. likelihood / status: the groups' [H_g][R_g] matrices back to back. A short
-    // haplotype does not throw here: the return code is PHMM_ERR_SHORT_HAPLOTYPE and the statuses carry the extension.
-    struct ReadAssignment
-    {
-        std::vector<std::uint64_t> top;
-        std::vector<double> likelihood;
-        std::vector<std::int32_t> status;
-        int code = PHMM_OK;
-    };
+    // compute_haplotype_support's scoring and choice for many genotypes (phmm_assign_reads); detail::ReadAssignment.
+    using ReadAssignment = detail::ReadAssignment;
     ReadAssignment assign_reads(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
                                 const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
                                 const std::vector<double>* log_priors = nullptr, bool want_likelihoods = false) const
     {
-        if (hap_first.empty() || hap_first.size() != read_first.size()) throw Error {PHMM_ERR_INVALID, "group bounds need n + 1 entries each"};
-        const auto n = static_cast<std::int32_t>(hap_first.size() - 1);
-        if (log_priors && log_priors->size() != static_cast<std::size_t>(haplotypes.n)) throw Error {PHMM_ERR_INVALID, "one log prior per haplotype"};
-        std::size_t pairs = 0;
-        for (std::int32_t g = 0; g < n; ++g)
-            pairs += static_cast<std::size_t>(std::max(0, hap_first[g + 1] - hap_first[g])) * static_cast<std::size_t>(std::max(0, read_first[g + 1] - read_first[g]));
-        const phmm_regions groups {n, hap_first.data(), read_first.data(), nullptr};
-        ReadAssignment a;
-        a.top.resize(static_cast<std::size_t>(std::max(0, reads.n)));
-        a.status.resize(pairs);
-        if (want_likelihoods) a.likelihood.resize(pairs);
-        a.code = phmm_assign_reads(get(), &config, &haplotypes, &reads, &groups, log_priors ? log_priors->data() : nullptr, a.top.data(),
-                                   want_likelihoods ? a.likelihood.data() : nullptr, a.status.data(), PHMM_SPACE_HOST);
+        ReadAssignment a = detail::assign_reads(haplotypes, reads, hap_first, read_first, log_priors, want_likelihoods,
+                                                [&] (const phmm_regions& groups, const double* priors, std::uint64_t* top, double* lnl, std::int32_t* st) {
+            return phmm_assign_reads(get(), &config, &haplotypes, &reads, &groups, priors, top, lnl, st, PHMM_SPACE_HOST);
+        });
         if (a.code != PHMM_ERR_SHORT_HAPLOTYPE) check(a.code);
         return a;
     }
@@ -159,8 +191,8 @@ private:
 };
 
 // One engine for a whole process's threads (phmm_batcher): the populate calls that concurrent threads have in flight run as one
-// multi-region kernel chain, each with the result it would get on an Engine of its own. Copies share the batcher; every thread
-// may call it at once. clients: the number of threads that submit (Octopus's --threads); a batch is sent once that many wait,
+// multi-region kernel chain, their read assignments and realignments as one assign / realign call, each with the result it would
+// get on an Engine of its own. Copies share the batcher; every thread may call it at once. clients: the number of threads that submit (Octopus's --threads); a batch is sent once that many wait,
 // or max_wait_us after its first request arrived.
 class SharedEngine
 {
@@ -185,6 +217,30 @@ public:
         phmm_batcher_stats s {};
         check(phmm_batcher_stats_get(handle_.get(), &s));
         return s;
+    }
+    std::int64_t reruns() const { return phmm_batcher_reruns(handle_.get()); }
+
+    // Engine::realign_reads and Engine::assign_reads through the shared engine (phmm_batcher_realign_reads / _assign_reads)
+    using PairAlignments = detail::PairAlignments;
+    PairAlignments realign_reads(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
+                                 const std::vector<phmm_pair>& pairs, const phmm_flank_state* flank_state = nullptr) const
+    {
+        return detail::realign_reads(reads, pairs.size(), [&] (std::int32_t stride, std::int64_t* mp, double* lk, char* text, std::int32_t* st) {
+            check(phmm_batcher_realign_reads(get(), &config, &haplotypes, &reads, pairs.data(), static_cast<std::int64_t>(pairs.size()),
+                                             flank_state, mp, lk, text, stride, st));
+        });
+    }
+    using ReadAssignment = detail::ReadAssignment;
+    ReadAssignment assign_reads(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
+                                const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
+                                const std::vector<double>* log_priors = nullptr, bool want_likelihoods = false) const
+    {
+        ReadAssignment a = detail::assign_reads(haplotypes, reads, hap_first, read_first, log_priors, want_likelihoods,
+                                                [&] (const phmm_regions& groups, const double* priors, std::uint64_t* top, double* lnl, std::int32_t* st) {
+            return phmm_batcher_assign_reads(get(), &config, &haplotypes, &reads, &groups, priors, top, lnl, st);
+        });
+        if (a.code != PHMM_ERR_SHORT_HAPLOTYPE) check(a.code);
+        return a;
     }
 private:
     std::shared_ptr<phmm_batcher> handle_;
@@ -523,11 +579,12 @@ struct Realignment
     double likelihood;
 };
 
-// realign(reads, haplotype, model) (read_realigner.cpp:105-144) for haplotype `haplotype` of the block: every read mapped with the
-// uncapped k-mer mapper and aligned there, on the GPU. When a read's haplotype is too short, throws ShortHaplotypeError for the first
-// such read in read order — the reference's serial loop, whose required extension safe_realign (:196-207) applies.
-inline std::vector<Realignment> realign(const ReadBlock& reads, const HaplotypeBlock& haplotypes, std::size_t haplotype,
-                                        const phmm_config& config, const Engine& engine = Engine {}, const FlankState* flank_state = nullptr)
+namespace detail {
+
+// realign() on an Engine or a SharedEngine (both have realign_reads)
+template <typename AnyEngine>
+std::vector<Realignment> realign(const ReadBlock& reads, const HaplotypeBlock& haplotypes, std::size_t haplotype, const phmm_config& config,
+                                 const AnyEngine& engine, const FlankState* flank_state)
 {
     std::vector<phmm_pair> pairs(reads.size());
     for (std::size_t r = 0; r < reads.size(); ++r) pairs[r] = phmm_pair {static_cast<std::int32_t>(r), static_cast<std::int32_t>(haplotype)};
@@ -545,6 +602,25 @@ inline std::vector<Realignment> realign(const ReadBlock& reads, const HaplotypeB
     return result;
 }
 
+} // namespace detail
+
+// realign(reads, haplotype, model) (read_realigner.cpp:105-144) for haplotype `haplotype` of the block: every read mapped with the
+// uncapped k-mer mapper and aligned there, on the GPU. When a read's haplotype is too short, throws ShortHaplotypeError for the first
+// such read in read order — the reference's serial loop, whose required extension safe_realign (:196-207) applies.
+inline std::vector<Realignment> realign(const ReadBlock& reads, const HaplotypeBlock& haplotypes, std::size_t haplotype,
+                                        const phmm_config& config, const Engine& engine = Engine {}, const FlankState* flank_state = nullptr)
+{
+    return detail::realign(reads, haplotypes, haplotype, config, engine, flank_state);
+}
+
+// The same through a shared engine: a region thread's realignments merge with other threads' requests, with the same results and
+// exceptions.
+inline std::vector<Realignment> realign(const ReadBlock& reads, const HaplotypeBlock& haplotypes, std::size_t haplotype,
+                                        const phmm_config& config, const SharedEngine& engine, const FlankState* flank_state = nullptr)
+{
+    return detail::realign(reads, haplotypes, haplotype, config, engine, flank_state);
+}
+
 // AssignmentConfig::AmbiguousAction (core/tools/read_assigner.hpp). random needs the caller's RNG: apply it to
 // HaplotypeSupport::ambiguous yourself (the helper treats it as drop).
 enum class AmbiguousAction { drop, first, all, random };
@@ -558,14 +634,13 @@ struct HaplotypeSupport
     std::vector<std::pair<std::size_t, std::vector<unsigned>>> ambiguous;
 };
 
-// compute_haplotype_support (core/tools/read_assigner.cpp:322-459) for many genotypes in one GPU call: group g (one genotype, after the
-// caller's collapse) owns haplotypes [hap_first[g], hap_first[g+1]) and reads [read_first[g], read_first[g+1]). log_priors: one per
-// haplotype of the block, or null. When a haplotype is too short, throws ShortHaplotypeError for the first short (haplotype, read)
-// pair in the reference's order (groups in turn, haplotypes in genotype order, then reads), with the block's haplotype index.
-inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& reads, const HaplotypeBlock& haplotypes,
-                                                               const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
-                                                               const std::vector<double>* log_priors, AmbiguousAction action,
-                                                               const phmm_config& config, const Engine& engine = Engine {})
+namespace detail {
+
+// compute_haplotype_support() on an Engine or a SharedEngine (both have assign_reads)
+template <typename AnyEngine>
+std::vector<HaplotypeSupport> haplotype_support(const ReadBlock& reads, const HaplotypeBlock& haplotypes, const std::vector<std::int32_t>& hap_first,
+                                                const std::vector<std::int32_t>& read_first, const std::vector<double>* log_priors,
+                                                AmbiguousAction action, const phmm_config& config, const AnyEngine& engine)
 {
     const auto a = engine.assign_reads(config, haplotypes.view(), reads.view(), hap_first, read_first, log_priors);
     if (a.code == PHMM_ERR_SHORT_HAPLOTYPE) {
@@ -597,6 +672,30 @@ inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& 
         }
     }
     return result;
+}
+
+} // namespace detail
+
+// compute_haplotype_support (core/tools/read_assigner.cpp:322-459) for many genotypes in one GPU call: group g (one genotype, after the
+// caller's collapse) owns haplotypes [hap_first[g], hap_first[g+1]) and reads [read_first[g], read_first[g+1]). log_priors: one per
+// haplotype of the block, or null. When a haplotype is too short, throws ShortHaplotypeError for the first short (haplotype, read)
+// pair in the reference's order (groups in turn, haplotypes in genotype order, then reads), with the block's haplotype index.
+inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& reads, const HaplotypeBlock& haplotypes,
+                                                               const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
+                                                               const std::vector<double>* log_priors, AmbiguousAction action,
+                                                               const phmm_config& config, const Engine& engine = Engine {})
+{
+    return detail::haplotype_support(reads, haplotypes, hap_first, read_first, log_priors, action, config, engine);
+}
+
+// The same through a shared engine: a region thread's assignments merge with other threads' requests, with the same results and
+// exceptions.
+inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& reads, const HaplotypeBlock& haplotypes,
+                                                               const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
+                                                               const std::vector<double>* log_priors, AmbiguousAction action,
+                                                               const phmm_config& config, const SharedEngine& engine)
+{
+    return detail::haplotype_support(reads, haplotypes, hap_first, read_first, log_priors, action, config, engine);
 }
 
 using SampleName = std::string;

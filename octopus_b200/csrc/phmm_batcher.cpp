@@ -1,7 +1,8 @@
 // Shared engine for many host threads (include/phmm_b200.h, phmm_batcher_*): the populate requests that concurrent threads
 // have in flight are merged into one phmm_populate_regions call, their mutation-prime requests into one phmm_mutation_prime_sets
-// call. Host C++ over the public C ABI; a batch runs the engine's existing multi-region / multi-set kernel chain. No thread of its
-// own: the first member of a batch (its leader) makes the call.
+// call, their assign and realign requests into one phmm_assign_reads / phmm_realign_reads call. Host C++ over the public C ABI; a
+// batch runs the engine's existing multi-region / multi-set / pair-list kernel chain. No thread of its own: the first member of a
+// batch (its leader) makes the call.
 #include "../../include/phmm_b200.h"
 #include "phmm_batcher_seam.h"
 #include "phmm_checks.h"
@@ -11,6 +12,7 @@
 #include <chrono>
 #include <condition_variable>
 #include <cstring>
+#include <limits>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -23,17 +25,30 @@ thread_local std::string t_error;
 
 constexpr long long kMaxBatchHaps = 65535;          // the DP task word's 16-bit haplotype field (phmm_engine.cu, task_word_ok)
 constexpr long long kMaxBatchPairs = 4LL << 20;     // (haplotype, read) pairs of one merged call
+constexpr long long kMaxBatchCigarBytes = 128LL << 20;   // CIGAR text of one merged realign call: its pairs x its largest stride
+constexpr long long kMaxMapperHapBases = 65535LL * 65535LL;   // the k-mer mapper's haplotype block (phmm_checks::mapper_haplotypes)
 constexpr int kDefaultMaxWaitUs = 500;
 
 using Clock = std::chrono::steady_clock;
 
-// Element counts of a request or a batch; each request kind names its N counts.
-template <int N>
+// No count of a batch derived from its others.
+struct NoDerived { static void apply(long long*) {} };
+
+// Element counts of a request or a batch; each request kind names its N counts. The first SUMMED add up over a batch's members,
+// the others (a size every member's slot shares, such as the CIGAR stride) take the members' largest; then Derive::apply recomputes
+// the counts that follow from the others (a realign batch's CIGAR bytes: its pairs x its stride). max() is per count: a high-water
+// mark of each.
+template <int N, int SUMMED = N, typename Derive = NoDerived>
 struct Counts {
     long long n[N] = {};
     long long& operator[](int i) { return n[i]; }
     long long operator[](int i) const { return n[i]; }
-    Counts& operator+=(const Counts& o) { for (int i = 0; i < N; ++i) n[i] += o.n[i]; return *this; }
+    Counts& operator+=(const Counts& o)
+    {
+        for (int i = 0; i < N; ++i) n[i] = i < SUMMED ? n[i] + o.n[i] : std::max(n[i], o.n[i]);
+        Derive::apply(n);
+        return *this;
+    }
     bool within(const Counts& cap) const { for (int i = 0; i < N; ++i) if (n[i] > cap.n[i]) return false; return true; }
     static Counts max(const Counts& a, const Counts& b)
     {
@@ -64,12 +79,18 @@ struct Pinned {
     }
 };
 
+// What a kind whose merged call is never rerun reports: the DP cells of its call are the engine's count for its last call.
+struct KindBase {
+    static constexpr bool reran = false;
+    static int64_t dp_cells(const phmm_engine* e) { return phmm_last_dp_cells(e); }
+};
+
 // The request kinds. Each supplies what differs between them: its counts, its staging, its merge key and limits, its per-member
 // bookkeeping (a Kind object lives in each batch), the copy in, the merged engine call and the copy out.
 
 // What the two populate kinds share: their counts, the read side of their staging, a batch's regions (one per member; the batch is
 // one multi-region call) and the copy out.
-struct PopulateBase {
+struct PopulateBase : KindBase {
     enum { HAPS, HAP_BASES, READS, READ_BASES, PAIRS, N_COUNTS };
     using Sizes = Counts<N_COUNTS>;
 
@@ -104,7 +125,9 @@ struct PopulateBase {
             else std::memset(read_begin.p + at[READS], 0, (size_t)R * sizeof(int64_t));
             std::memcpy(bases.p + at[READ_BASES], reads->bases, (size_t)rb);
             std::memcpy(quals.p + at[READ_BASES], reads->quals, (size_t)rb);
-            std::memcpy(mapq.p + at[READS], reads->mapq, (size_t)R);
+            // a realign request without mapping qualities has a config that does not read them
+            if (reads->mapq) std::memcpy(mapq.p + at[READS], reads->mapq, (size_t)R);
+            else std::memset(mapq.p + at[READS], 0, (size_t)R);
             std::memcpy(reverse.p + at[READS], reads->reverse, (size_t)R);
         }
 
@@ -192,9 +215,11 @@ struct Populate : PopulateBase {
     explicit Populate(const Request& q) : PopulateBase(q.cfg) {}
 
     // the request into its slot at `at` (outside the lock: each member writes its own ranges only)
-    static void copy_in(Staging& st, const Sizes& at, const Request& q)
+    static void copy_in(Staging& st, const Sizes& at, const Request& q) { copy_in_blocks(st, at, q.haps, q.reads); }
+
+    // a request's two blocks into their slots at `at` (populate, assign and realign requests)
+    static void copy_in_blocks(Staging& st, const Sizes& at, const phmm_haplotypes* haps, const phmm_reads* reads)
     {
-        const phmm_haplotypes* haps = q.haps;
         const int H = haps->n;
         const long long hb = haps->off[H];
         if (at[HAPS] == 0) st.hap_off.p[0] = 0;
@@ -208,7 +233,7 @@ struct Populate : PopulateBase {
         std::memcpy(st.prior_r.p + at[HAP_BASES], haps->snv_prior_rev, (size_t)hb);
         std::memcpy(st.gap_open.p + at[HAP_BASES], haps->gap_open, (size_t)hb);
         std::memcpy(st.gap_extend.p + at[HAP_BASES], haps->gap_extend, (size_t)hb);
-        st.copy_in_reads(at, q.reads);
+        st.copy_in_reads(at, reads);
     }
 
     // the leader's call: the batch's members as the regions of one phmm_populate_regions call
@@ -282,7 +307,7 @@ struct PopulateReset : PopulateBase {
 
 // Mutation-prime requests: a batch is one phmm_mutation_prime_sets call and each member one of its sets; models equal by content
 // (phmm_mutation_model::key) merge.
-struct MutationPrime {
+struct MutationPrime : KindBase {
     enum { HAPS, BASES, PAIRS, N_COUNTS };
     using Sizes = Counts<N_COUNTS>;
 
@@ -343,6 +368,282 @@ struct MutationPrime {
     }
 };
 
+// What the assign and realign kinds share: their members' requests, and the rerun of a merged call that failed with
+// PHMM_ERR_INVALID. That is a failure a member's own call need not see (assign's more than 4096 mapping positions for one pair fail
+// the whole call), so the leader then calls the engine once per member, in the same engine turn, straight into the member's own
+// outputs, and each member returns its own code and message.
+template <typename Request>
+struct Members {
+    std::vector<const Request*> reqs;                     // alive while their threads wait in the batch
+    std::vector<std::pair<int, std::string>> solo;       // after a rerun: each member's code and message
+    bool reran = false;
+    int64_t cells = 0;                                    // after a rerun: the DP cells of the merged call and of every rerun
+
+    void add(const Request& q) { reqs.push_back(&q); }
+
+    template <typename Solo>
+    void rerun_if_invalid(phmm_engine* e, int rc, Solo&& solo_call)
+    {
+        if (rc != PHMM_ERR_INVALID || reqs.size() < 2) return;
+        cells = phmm_last_dp_cells(e);
+        for (const Request* q : reqs) {
+            const int r = solo_call(e, *q);
+            solo.emplace_back(r, r == PHMM_OK ? std::string() : std::string(phmm_last_error(e)));
+            cells += phmm_last_dp_cells(e);
+        }
+        reran = true;
+    }
+
+    int64_t dp_cells(const phmm_engine* e) const { return reran ? cells : phmm_last_dp_cells(e); }
+
+    // after a rerun: the member's own code, with its message in t_error
+    int own(const Request& q) const
+    {
+        const size_t i = (size_t)(std::find(reqs.begin(), reqs.end(), &q) - reqs.begin());
+        t_error = solo[i].second;
+        return solo[i].first;
+    }
+};
+
+// Assign requests: a batch is one phmm_assign_reads call whose groups are the members' groups one after the other; equal configs
+// merge. The staging is populate's plus the log priors (zeros for a member without) and the top sets; lnl and status are always
+// staged and copied out to the members that asked for them.
+struct Assign : Members<struct AssignRequestSized> {
+    using Sizes = PopulateBase::Sizes;
+    enum { HAPS = PopulateBase::HAPS, HAP_BASES = PopulateBase::HAP_BASES, READS = PopulateBase::READS, PAIRS = PopulateBase::PAIRS };
+    using Request = AssignRequestSized;
+
+    struct Staging : Populate::Staging {
+        Pinned<double> priors;
+        Pinned<uint64_t> top;
+
+        bool grow(const Sizes& s)
+        {
+            if (!(Populate::Staging::grow(s) && priors.ensure(s[HAPS]) && top.ensure(s[READS]))) return false;
+            cap[HAPS] = std::min(cap[HAPS], priors.cap);
+            cap[READS] = std::min(cap[READS], top.cap);
+            return true;
+        }
+    };
+
+    static Sizes initial_staging() { return PopulateBase::initial_staging(); }
+    static bool within_limits(const Sizes& s) { return PopulateBase::within_limits(s) && s[HAP_BASES] <= kMaxMapperHapBases; }
+    static std::string key(const Request& q);
+
+    phmm_config cfg;
+    const phmm_batcher_seam::AlignCalls* calls;
+    std::vector<int32_t> hap_first {0}, read_first {0};
+    std::vector<phmm_flank_state> flanks;
+
+    explicit Assign(const Request& q);
+    void add(const Request& q, const Sizes& used);
+    static void copy_in(Staging& st, const Sizes& at, const Request& q);
+    int run(phmm_engine* e, Staging& st, const Sizes& used);
+    int copy_out(const Staging& st, const Sizes& at, const Request& q, int rc, const std::string& err) const;
+};
+
+struct AssignRequestSized {
+    const phmm_batcher_seam::AssignRequest* r;
+    Assign::Sizes need;
+};
+
+std::string Assign::key(const Request& q) { return std::string(reinterpret_cast<const char*>(q.r->cfg), sizeof(phmm_config)); }
+
+Assign::Assign(const Request& q) : cfg(*q.r->cfg), calls(q.r->calls) {}
+
+// the member's groups, their bounds shifted to its slot (its slot ends at the batch's counts `used`); no flank is a flank state of 0
+void Assign::add(const Request& q, const Sizes& used)
+{
+    Members::add(q);
+    const phmm_regions* g = q.r->groups;
+    const long long h0 = used[HAPS] - q.need[HAPS], r0 = used[READS] - q.need[READS];
+    for (int i = 0; i < g->n; ++i) {
+        hap_first.push_back((int32_t)(h0 + g->hap_first[i + 1]));
+        read_first.push_back((int32_t)(r0 + g->read_first[i + 1]));
+        flanks.push_back(g->flank ? g->flank[i] : phmm_flank_state {0, 0, 0});
+    }
+}
+
+void Assign::copy_in(Staging& st, const Sizes& at, const Request& q)
+{
+    const phmm_batcher_seam::AssignRequest& r = *q.r;
+    Populate::copy_in_blocks(st, at, r.haps, r.reads);
+    // no priors and zero priors choose the same top sets: k_assign_top adds 0.0 for either
+    if (r.log_priors) std::memcpy(st.priors.p + at[HAPS], r.log_priors, (size_t)r.haps->n * sizeof(double));
+    else std::fill(st.priors.p + at[HAPS], st.priors.p + at[HAPS] + r.haps->n, 0.0);
+}
+
+int Assign::run(phmm_engine* e, Staging& st, const Sizes& used)
+{
+    const phmm_haplotypes hv {(int32_t)used[HAPS], st.hap_off.p, st.seq.p, st.mask_f.p, st.prior_f.p, st.mask_r.p, st.prior_r.p,
+                              st.gap_open.p, st.gap_extend.p, st.hap_begin.p};
+    const phmm_reads rv = st.reads(used);
+    const phmm_regions groups {(int32_t)flanks.size(), hap_first.data(), read_first.data(), flanks.data()};
+    const int rc = calls->assign(e, &cfg, &hv, &rv, &groups, st.priors.p, st.top.p, st.out.p, st.status.p, PHMM_SPACE_HOST);
+    rerun_if_invalid(e, rc, [](phmm_engine* en, const Request& q) {
+        const phmm_batcher_seam::AssignRequest& r = *q.r;
+        return r.calls->assign(en, r.cfg, r.haps, r.reads, r.groups, r.log_priors, r.top, r.lnl, r.status, PHMM_SPACE_HOST);
+    });
+    return rc;
+}
+
+// this member's reads' top sets and its groups' slots; its code from its own statuses, as the call's would be for it alone
+int Assign::copy_out(const Staging& st, const Sizes& at, const Request& q, int rc, const std::string& err) const
+{
+    if (reran) return own(q);
+    if (rc != PHMM_OK && rc != PHMM_ERR_SHORT_HAPLOTYPE) { t_error = err; return rc; }
+    const phmm_batcher_seam::AssignRequest& r = *q.r;
+    const long long P = q.need[PAIRS];
+    const int32_t* res_status = st.status.p + at[PAIRS];
+    rc = PHMM_OK;
+    for (long long i = 0; i < P; ++i) if ((res_status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) { rc = PHMM_ERR_SHORT_HAPLOTYPE; break; }
+    t_error = rc == PHMM_OK ? std::string() : std::string("Haplotype is too short for alignment");
+    std::memcpy(r.top, st.top.p + at[READS], (size_t)q.need[READS] * sizeof(uint64_t));
+    if (r.lnl) std::memcpy(r.lnl, st.out.p + at[PAIRS], (size_t)P * sizeof(double));
+    if (r.status) std::memcpy(r.status, res_status, (size_t)P * sizeof(int32_t));
+    return rc;
+}
+
+// The CIGAR text and status a pair gets at its own stride, from its text and status at the batch's stride (not smaller). The kernel
+// (cigar_emit / make_cigar_text, phmm_kernels.cuh) writes at most stride - 1 characters and a NUL, and turns status PHMM_STATUS_OK
+// into PHMM_STATUS_CIGAR_TRUNCATED unless the whole text is shorter than stride - 1 characters. An exact match's single '=' run is
+// the exception: it is cut without that status. Requests whose longest read's run would not fit their stride run alone, so here a
+// text too long for its stride is always a traceback's.
+int32_t restride_cigar(const char* text, int32_t status, char* out, int32_t stride)
+{
+    const size_t n = std::strlen(text), room = (size_t)stride - 1;
+    const size_t keep = std::min(n, room);
+    std::memcpy(out, text, keep);
+    out[keep] = 0;
+    return status == PHMM_STATUS_OK && n >= room ? PHMM_STATUS_CIGAR_TRUNCATED : status;
+}
+
+// whether a stride holds the single '=' run of an exact match of a read of `len` bases with room to spare (see restride_cigar)
+bool single_run_fits(long long len, int32_t stride)
+{
+    int digits = 1;
+    for (long long v = len; v >= 10; v /= 10) ++digits;
+    return digits + 1 < (long long)stride - 1;
+}
+
+// Realign requests: a batch is one phmm_realign_reads call over the members' blocks one after the other, their pair indices shifted
+// to their slots. Equal configs under equal effective flank states merge, whatever their strides: the call runs at the largest.
+struct Realign : Members<struct RealignRequestSized> {
+    enum { HAPS, HAP_BASES, READS, READ_BASES, PAIRS, STRIDE, CIGAR, N_COUNTS };
+    // the stride: the members' largest; CIGAR: the text bytes the call writes, its pairs x that stride. The staging's CIGAR buffer and
+    // the lane's high-water mark follow this count, never a product of the largest pair count and the largest stride seen apart.
+    struct CigarBytes { static void apply(long long* n) { n[CIGAR] = n[PAIRS] * n[STRIDE]; } };
+    using Sizes = Counts<N_COUNTS, STRIDE, CigarBytes>;
+    using Request = RealignRequestSized;
+
+    struct Staging {
+        Populate::Staging blocks;                              // its out / status: the likelihoods and statuses
+        Pinned<phmm_pair> pairs;
+        Pinned<int64_t> mapping_position;
+        Pinned<char> cigar;
+        Sizes cap;
+        bool busy = false;
+
+        bool grow(const Sizes& s)
+        {
+            if (!(blocks.grow(head(s)) && pairs.ensure(s[PAIRS]) && mapping_position.ensure(s[PAIRS]) && cigar.ensure(s[CIGAR])))
+                return false;
+            for (int i = 0; i < PopulateBase::N_COUNTS; ++i) cap[i] = blocks.cap[i];
+            cap[PAIRS] = std::min({cap[PAIRS], pairs.cap, mapping_position.cap});
+            cap[STRIDE] = std::numeric_limits<long long>::max();      // no room of its own: the CIGAR bytes hold it
+            cap[CIGAR] = cigar.cap;
+            return true;
+        }
+    };
+
+    static PopulateBase::Sizes head(const Sizes& s)
+    {
+        PopulateBase::Sizes h;
+        for (int i = 0; i < PopulateBase::N_COUNTS; ++i) h[i] = s[i];
+        return h;
+    }
+    // first staging size: some tens of requests of a few hundred reads of up to a few hundred bases
+    static Sizes initial_staging() { return {{1024, 1LL << 20, 1LL << 15, 4LL << 20, 1LL << 15, 0, 4LL << 20}}; }
+    static bool within_limits(const Sizes& s)
+    {
+        return s[PAIRS] <= kMaxBatchPairs && s[CIGAR] <= kMaxBatchCigarBytes && s[HAP_BASES] <= kMaxMapperHapBases;
+    }
+    static phmm_flank_state effective_flank(const phmm_config* cfg, const phmm_flank_state* f)
+    {
+        return f && f->has_flank && cfg->use_flank_state ? phmm_flank_state {1, f->lhs_flank, f->rhs_flank} : phmm_flank_state {0, 0, 0};
+    }
+    static std::string key(const Request& q);
+
+    phmm_config cfg;
+    phmm_flank_state flank;
+    const phmm_batcher_seam::AlignCalls* calls;
+    int32_t stride = 0;                                         // the batch's: its members' largest
+
+    explicit Realign(const Request& q);
+    void add(const Request& q, const Sizes& used) { Members::add(q); stride = (int32_t)used[STRIDE]; }
+    static void copy_in(Staging& st, const Sizes& at, const Request& q);
+    int run(phmm_engine* e, Staging& st, const Sizes& used);
+    int copy_out(const Staging& st, const Sizes& at, const Request& q, int rc, const std::string& err) const;
+};
+
+struct RealignRequestSized {
+    const phmm_batcher_seam::RealignRequest* r;
+    Realign::Sizes need;
+};
+
+// the config bytes and the flank state the call uses (phmm_realign_reads ignores a flank without has_flank or use_flank_state)
+std::string Realign::key(const Request& q)
+{
+    const phmm_flank_state f = effective_flank(q.r->cfg, q.r->flank);
+    std::string k(reinterpret_cast<const char*>(q.r->cfg), sizeof(phmm_config));
+    k.append(reinterpret_cast<const char*>(&f.has_flank), sizeof(f.has_flank));
+    k.append(reinterpret_cast<const char*>(&f.lhs_flank), sizeof(f.lhs_flank));
+    k.append(reinterpret_cast<const char*>(&f.rhs_flank), sizeof(f.rhs_flank));
+    return k;
+}
+
+Realign::Realign(const Request& q) : cfg(*q.r->cfg), flank(effective_flank(q.r->cfg, q.r->flank)), calls(q.r->calls) {}
+
+void Realign::copy_in(Staging& st, const Sizes& at, const Request& q)
+{
+    const phmm_batcher_seam::RealignRequest& r = *q.r;
+    Populate::copy_in_blocks(st.blocks, head(at), r.haps, r.reads);
+    for (int64_t j = 0; j < r.n_pairs; ++j)
+        st.pairs.p[at[PAIRS] + j] = phmm_pair {(int32_t)(at[READS] + r.pairs[j].read), (int32_t)(at[HAPS] + r.pairs[j].hap)};
+}
+
+int Realign::run(phmm_engine* e, Staging& st, const Sizes& used)
+{
+    const Populate::Staging& b = st.blocks;
+    const phmm_haplotypes hv {(int32_t)used[HAPS], b.hap_off.p, b.seq.p, b.mask_f.p, b.prior_f.p, b.mask_r.p, b.prior_r.p,
+                              b.gap_open.p, b.gap_extend.p, b.hap_begin.p};
+    const phmm_reads rv = b.reads(head(used));
+    const int rc = calls->realign(e, &cfg, &hv, &rv, st.pairs.p, used[PAIRS], &flank, st.mapping_position.p, b.out.p, st.cigar.p, stride,
+                                  b.status.p, PHMM_SPACE_HOST);
+    rerun_if_invalid(e, rc, [](phmm_engine* en, const Request& q) {
+        const phmm_batcher_seam::RealignRequest& r = *q.r;
+        return r.calls->realign(en, r.cfg, r.haps, r.reads, r.pairs, r.n_pairs, r.flank, r.mapping_position, r.likelihood, r.cigar,
+                                r.cigar_stride, r.status, PHMM_SPACE_HOST);
+    });
+    return rc;
+}
+
+// this member's pairs; each CIGAR text restated at the member's own stride
+int Realign::copy_out(const Staging& st, const Sizes& at, const Request& q, int rc, const std::string& err) const
+{
+    if (reran) return own(q);
+    if (rc != PHMM_OK) { t_error = err; return rc; }
+    const phmm_batcher_seam::RealignRequest& r = *q.r;
+    const long long p0 = at[PAIRS];
+    std::memcpy(r.mapping_position, st.mapping_position.p + p0, (size_t)r.n_pairs * sizeof(int64_t));
+    std::memcpy(r.likelihood, st.blocks.out.p + p0, (size_t)r.n_pairs * sizeof(double));
+    for (int64_t j = 0; j < r.n_pairs; ++j)
+        r.status[j] = restride_cigar(st.cigar.p + (size_t)(p0 + j) * stride, st.blocks.status.p[p0 + j], r.cigar + (size_t)j * r.cigar_stride,
+                                     r.cigar_stride);
+    t_error.clear();
+    return PHMM_OK;
+}
+
 // A batch of one kind's requests: the kind's own data and the shared life cycle.
 template <typename Kind>
 struct Batch {
@@ -382,21 +683,24 @@ struct phmm_batcher {
     Lane<Populate> populate;
     Lane<PopulateReset> populate_reset;
     Lane<MutationPrime> mutation;
+    Lane<Assign> assign;
+    Lane<Realign> realign;
     bool engine_busy = false;
     int waiting = 0;                                  // requests in batches not yet sent + requests running alone
     int in_flight = 0;                                // requests inside the batcher
     phmm_batcher_stats stats {};
+    int64_t reruns = 0;                               // merged calls rerun one member at a time
 };
 
 namespace {
 
-void count_call(phmm_batcher* b, int requests)
+void count_call(phmm_batcher* b, int requests, int64_t dp_cells)
 {
     b->stats.requests += requests;
     b->stats.gpu_calls += 1;
     if (requests > 1) b->stats.merged_calls += 1;
     b->stats.max_regions_per_call = std::max<int64_t>(b->stats.max_regions_per_call, requests);
-    b->stats.dp_cells += phmm_last_dp_cells(b->engine);
+    b->stats.dp_cells += dp_cells;
 }
 
 // A request a multi-region call cannot merge: one engine call of its own, call(engine), in turn with the batches.
@@ -412,7 +716,7 @@ int run_alone(phmm_batcher* b, Call&& call)
     const int rc = call(b->engine);
     t_error = rc == PHMM_OK ? std::string() : std::string(phmm_last_error(b->engine));
     lk.lock();
-    count_call(b, 1);
+    count_call(b, 1, phmm_last_dp_cells(b->engine));
     b->engine_busy = false;
     --b->waiting;
     b->cv.notify_all();
@@ -479,7 +783,7 @@ Batch<Kind>* join(phmm_batcher* b, Lane<Kind>& lane, const std::string& key, con
 // the staging outside the lock (each member its own ranges). The first member leads: it waits until `clients` requests wait, the
 // batch is full or its deadline has passed, and the engine is free, then seals the batch and makes the kind's call; the others
 // wait for it. Each member copies its own slice out (outside the lock) and returns its code; the last reader frees the staging
-// and the batch.
+// and the batch. A kind whose merged call can fail for one member's sake reruns its members alone inside run (Members).
 template <typename Kind>
 int take_part(phmm_batcher* b, Lane<Kind>& lane, const typename Kind::Request& q)
 {
@@ -513,7 +817,8 @@ int take_part(phmm_batcher* b, Lane<Kind>& lane, const typename Kind::Request& q
         bt->rc = bt->kind.run(b->engine, *bt->st, bt->used);
         if (bt->rc != PHMM_OK) bt->err = phmm_last_error(b->engine);
         lk.lock();
-        count_call(b, bt->members);
+        count_call(b, bt->members, bt->kind.dp_cells(b->engine));
+        if (bt->kind.reran) { b->reruns += 1; b->stats.gpu_calls += bt->members; }
         b->engine_busy = false;
         bt->done = true;
         b->cv.notify_all();
@@ -523,7 +828,7 @@ int take_part(phmm_batcher* b, Lane<Kind>& lane, const typename Kind::Request& q
     }
     lk.unlock();
 
-    const int rc = Kind::copy_out(*bt->st, at, q, bt->rc, bt->err);
+    const int rc = bt->kind.copy_out(*bt->st, at, q, bt->rc, bt->err);
 
     lk.lock();
     if (--bt->readers == 0) {
@@ -583,6 +888,75 @@ struct InFlight {
 };
 
 } // namespace
+
+int phmm_batcher_seam::submit_assign(phmm_batcher* b, const AssignRequest& r)
+{
+    if (!b) { t_error = "null batcher"; return PHMM_ERR_INVALID; }
+    // phmm_assign_reads' host checks in its order: the groups, the config and top, the group limits, the blocks, the mapper's limits
+    int rc;
+    if ((rc = phmm_checks::regions(r.haps, r.reads, r.groups, t_error)) != PHMM_OK) return rc;
+    if ((rc = phmm_checks::config_and_output(r.cfg, r.top, r.reads, t_error)) != PHMM_OK) return rc;
+    if ((rc = phmm_checks::assign_groups(r.groups, t_error)) != PHMM_OK) return rc;
+    if ((rc = phmm_checks::blocks(r.haps, r.reads, t_error)) != PHMM_OK) return rc;
+    long long len_min, len_max;
+    phmm_checks::read_length_range(r.reads, &len_min, &len_max);
+    const long long hap_bases = r.haps->off[r.haps->n], read_bases = r.reads->off[r.reads->n];
+    if ((rc = phmm_checks::offsets(r.haps->off[0], hap_bases, r.reads->off[0], read_bases, len_min, len_max, t_error)) != PHMM_OK) return rc;
+    long long max_hap = 0;
+    for (int h = 0; h < r.haps->n; ++h) max_hap = std::max<long long>(max_hap, r.haps->off[h + 1] - r.haps->off[h]);
+    if (r.cfg->map_positions) {
+        if ((rc = phmm_checks::mapper_reads(len_max, t_error)) != PHMM_OK) return rc;
+        if ((rc = phmm_checks::mapper_haplotypes(max_hap, hap_bases, t_error)) != PHMM_OK) return rc;
+    }
+    long long pairs = 0;
+    for (int g = 0; g < r.groups->n; ++g)
+        pairs += (long long)(r.groups->hap_first[g + 1] - r.groups->hap_first[g]) * (r.groups->read_first[g + 1] - r.groups->read_first[g]);
+    // a penalty outside [0,127] fails the call that holds it (after its mapping), and too large a request would not fit a batch
+    std::string penalty_error;
+    InFlight guard(b);
+    if (r.haps->n > kMaxBatchHaps || pairs > kMaxBatchPairs || max_hap > 65535 || phmm_checks::penalties(r.haps, hap_bases, penalty_error) != PHMM_OK) {
+        return run_alone(b, [&](phmm_engine* e) {
+            return r.calls->assign(e, r.cfg, r.haps, r.reads, r.groups, r.log_priors, r.top, r.lnl, r.status, PHMM_SPACE_HOST);
+        });
+    }
+    const Assign::Request q {&r, {{r.haps->n, hap_bases, r.reads->n, read_bases, pairs}}};
+    return take_part(b, b->assign, q);
+}
+
+int phmm_batcher_seam::submit_realign(phmm_batcher* b, const RealignRequest& r)
+{
+    if (!b) { t_error = "null batcher"; return PHMM_ERR_INVALID; }
+    // phmm_realign_reads' host checks in its order: the arguments, the reads' arrays, the blocks, the penalties, the pair indices,
+    // the mapper's limits
+    int rc;
+    if ((rc = phmm_checks::align_arguments(r.cfg, r.pairs, r.n_pairs, r.mapping_position, r.likelihood, r.cigar, r.cigar_stride, r.status,
+                                           t_error)) != PHMM_OK)
+        return rc;
+    if (r.n_pairs == 0) { t_error.clear(); return PHMM_OK; }
+    if ((rc = phmm_checks::align_reads(r.cfg, r.reads, t_error)) != PHMM_OK) return rc;
+    if ((rc = phmm_checks::blocks(r.haps, r.reads, t_error)) != PHMM_OK) return rc;
+    long long len_min, len_max;
+    phmm_checks::read_length_range(r.reads, &len_min, &len_max);
+    const long long hap_bases = r.haps->off[r.haps->n], read_bases = r.reads->off[r.reads->n];
+    if ((rc = phmm_checks::offsets(r.haps->off[0], hap_bases, r.reads->off[0], read_bases, len_min, len_max, t_error)) != PHMM_OK) return rc;
+    if ((rc = phmm_checks::penalties(r.haps, hap_bases, t_error)) != PHMM_OK) return rc;
+    if ((rc = phmm_checks::pair_indices(r.pairs, r.n_pairs, r.haps->n, r.reads->n, t_error)) != PHMM_OK) return rc;
+    if (r.cfg->map_positions) {
+        long long max_hap = 0;
+        for (int h = 0; h < r.haps->n; ++h) max_hap = std::max<long long>(max_hap, r.haps->off[h + 1] - r.haps->off[h]);
+        if ((rc = phmm_checks::mapper_reads(len_max, t_error)) != PHMM_OK) return rc;
+        if ((rc = phmm_checks::mapper_haplotypes(max_hap, hap_bases, t_error)) != PHMM_OK) return rc;
+    }
+    InFlight guard(b);
+    const Realign::Request q {&r, {{r.haps->n, hap_bases, r.reads->n, read_bases, r.n_pairs, r.cigar_stride, r.n_pairs * r.cigar_stride}}};
+    if (!Realign::within_limits(q.need) || !single_run_fits(len_max, r.cigar_stride)) {
+        return run_alone(b, [&](phmm_engine* e) {
+            return r.calls->realign(e, r.cfg, r.haps, r.reads, r.pairs, r.n_pairs, r.flank, r.mapping_position, r.likelihood, r.cigar,
+                                    r.cigar_stride, r.status, PHMM_SPACE_HOST);
+        });
+    }
+    return take_part(b, b->realign, q);
+}
 
 int phmm_batcher_seam::submit_reset(phmm_batcher* b, const ResetRequest& r)
 {
@@ -673,6 +1047,13 @@ int phmm_batcher_stats_get(const phmm_batcher* b, phmm_batcher_stats* out)
     std::lock_guard<std::mutex> lk(b->m);
     *out = b->stats;
     return PHMM_OK;
+}
+
+int64_t phmm_batcher_reruns(const phmm_batcher* b)
+{
+    if (!b) return 0;
+    std::lock_guard<std::mutex> lk(b->m);
+    return b->reruns;
 }
 
 } // extern "C"

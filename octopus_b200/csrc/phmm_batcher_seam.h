@@ -1,7 +1,7 @@
-// The seam between the request batcher (phmm_batcher.cpp) and its populate requests with an error model (phmm_batcher_reset.cpp).
-// phmm_batcher_reset.cpp computes a request's model key and hands the batcher the engine calls as function pointers, so that
-// phmm_batcher.cpp names no engine symbol beyond the plain populate ones and no error-model internals: a fake engine can stand
-// behind both.
+// The seam between the request batcher (phmm_batcher.cpp) and its populate requests with an error model (phmm_batcher_reset.cpp)
+// and its assign / realign requests (phmm_batcher_align.cpp). phmm_batcher_reset.cpp computes a request's model key; both hand the
+// batcher the engine calls as function pointers, so that phmm_batcher.cpp names no engine symbol beyond the plain populate and
+// mutation ones and no error-model internals: a fake engine can stand behind each part.
 #ifndef PHMM_BATCHER_SEAM_H
 #define PHMM_BATCHER_SEAM_H
 
@@ -35,6 +35,30 @@ struct ResetRequest {
 
 // Checks the request on the calling thread with phmm_populate_reset's checks and messages, then merges it or runs it alone.
 int submit_reset(phmm_batcher* b, const ResetRequest& q);
+
+// The engine calls of the assign and realign requests (phmm_batcher_align.cpp).
+struct AlignCalls {
+    decltype(&phmm_assign_reads) assign;
+    decltype(&phmm_realign_reads) realign;
+};
+
+// One request of phmm_batcher_assign_reads.
+struct AssignRequest {
+    const AlignCalls* calls;
+    const phmm_config* cfg; const phmm_haplotypes* haps; const phmm_reads* reads; const phmm_regions* groups;
+    const double* log_priors; uint64_t* top; double* lnl; int32_t* status;
+};
+
+// One request of phmm_batcher_realign_reads.
+struct RealignRequest {
+    const AlignCalls* calls;
+    const phmm_config* cfg; const phmm_haplotypes* haps; const phmm_reads* reads; const phmm_pair* pairs; int64_t n_pairs;
+    const phmm_flank_state* flank; int64_t* mapping_position; double* likelihood; char* cigar; int32_t cigar_stride; int32_t* status;
+};
+
+// Each checks the request on the calling thread with the plain call's checks and messages, then merges it or runs it alone.
+int submit_assign(phmm_batcher* b, const AssignRequest& q);
+int submit_realign(phmm_batcher* b, const RealignRequest& q);
 
 } // namespace phmm_batcher_seam
 

@@ -1,4 +1,4 @@
-// Host-side argument checks of the populate and mutation-prime entry points, shared by the engine (phmm_engine.cu) and the request batcher
+// Host-side argument checks of the populate, assign, align and mutation-prime entry points, shared by the engine (phmm_engine.cu) and the request batcher
 // (phmm_batcher.cpp) so that both report the same error codes and messages. Each check returns PHMM_OK or an error code and
 // sets `err`; the callers run them in the order populate reports errors in.
 #ifndef PHMM_CHECKS_H
@@ -63,6 +63,74 @@ inline int mapper_haplotypes(long long max_hap_len, long long hap_bases, std::st
 {
     if (max_hap_len > 65535) { err = "haplotype longer than 65535 bp: the device k-mer mapper indexes k-mer positions with 16 bits (pass explicit positions)"; return PHMM_ERR_INVALID; }
     if (hap_bases > 65535LL * 65535LL) { err = "haplotype block too large"; return PHMM_ERR_INVALID; }
+    return PHMM_OK;
+}
+
+// the uncapped pair mapper's read limit (phmm_map_pairs, phmm_realign_reads, phmm_assign_reads): votes are counted in 16 bits
+inline int mapper_reads(long long read_len_max, std::string& err)
+{
+    if (read_len_max > 65540) { err = "read longer than 65540 bp: the device k-mer mapper counts votes in 16 bits"; return PHMM_ERR_INVALID; }
+    return PHMM_OK;
+}
+
+// the region (group) list of phmm_populate_regions / phmm_assign_reads (host memory): bounds that cover both blocks exactly and at
+// least one haplotype and one read per region
+inline int regions(const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_regions* regions, std::string& err)
+{
+    if (!regions || regions->n <= 0 || !regions->hap_first || !regions->read_first || !haps || !reads) { err = "null / empty region list"; return PHMM_ERR_INVALID; }
+    if (regions->hap_first[0] != 0 || regions->read_first[0] != 0 || regions->hap_first[regions->n] != haps->n || regions->read_first[regions->n] != reads->n) {
+        err = "region ranges must cover the haplotype and read blocks exactly";
+        return PHMM_ERR_INVALID;
+    }
+    for (int g = 0; g < regions->n; ++g) {
+        if (regions->hap_first[g + 1] <= regions->hap_first[g] || regions->read_first[g + 1] <= regions->read_first[g]) {
+            err = "every region needs at least one haplotype and one read";
+            return PHMM_ERR_INVALID;
+        }
+    }
+    return PHMM_OK;
+}
+
+// phmm_assign_reads' limits on a checked group list: a read's top set is a 64-bit mask, and the call's result slots are counted in
+// 31 bits
+inline int assign_groups(const phmm_regions* groups, std::string& err)
+{
+    long long widest = 0, slots = 0;
+    for (int g = 0; g < groups->n; ++g) {
+        const long long nH = groups->hap_first[g + 1] - groups->hap_first[g], nR = groups->read_first[g + 1] - groups->read_first[g];
+        widest = std::max(widest, nH);
+        slots += nH * nR;
+    }
+    if (widest > 64) { err = "more than 64 haplotypes in one group: a read's top set is a 64-bit mask"; return PHMM_ERR_INVALID; }
+    if (slots > 0x7fffffffLL) { err = "more than 2^31 - 1 (read, haplotype) pairs in one call"; return PHMM_ERR_INVALID; }
+    return PHMM_OK;
+}
+
+// The aligning calls (phmm_align_reads, phmm_realign_reads, phmm_align_pairs): their output pointers, the CIGAR stride, the config
+// and the pair count, before anything else; a call of no pairs then returns PHMM_OK without touching anything.
+inline int align_arguments(const phmm_config* cfg, const phmm_pair* pairs, int64_t n_pairs, const void* mapping_position, const void* likelihood,
+                           const char* cigar, int32_t cigar_stride, const int32_t* status, std::string& err)
+{
+    if (!cfg || !pairs || !mapping_position || !likelihood || !cigar || !status || cigar_stride < 8) { err = "null argument / cigar_stride < 8"; return PHMM_ERR_INVALID; }
+    if (cfg->max_indel_error > 256) { err = "max_indel_error > 256"; return PHMM_ERR_BAND; }
+    if (cfg->nuc_prior < 0 || cfg->nuc_prior > 127) { err = "nuc_prior outside [0,127]"; return PHMM_ERR_INVALID; }
+    if (n_pairs < 0 || n_pairs > 0x7fffffff) { err = "pair count out of range"; return PHMM_ERR_INVALID; }
+    return PHMM_OK;
+}
+
+// the per-read arrays the aligning calls need: reverse always, mapping qualities where the config uses them
+inline int align_reads(const phmm_config* cfg, const phmm_reads* reads, std::string& err)
+{
+    if (!reads || !reads->reverse || (!reads->mapq && cfg->use_mapping_quality)) { err = "reads->mapq / reads->reverse required"; return PHMM_ERR_INVALID; }
+    return PHMM_OK;
+}
+
+// (read, haplotype) indices of a host-resident pair list
+inline int pair_indices(const phmm_pair* pairs, long long n, int n_haps, int n_reads, std::string& err)
+{
+    for (long long i = 0; i < n; ++i) {
+        if (pairs[i].read < 0 || pairs[i].read >= n_reads || pairs[i].hap < 0 || pairs[i].hap >= n_haps) { err = "pair index out of range"; return PHMM_ERR_INVALID; }
+    }
     return PHMM_OK;
 }
 

@@ -351,10 +351,7 @@ int begin_call(phmm_engine* e)
 // The (read, haplotype) indices of a host-space pair list: checked where they are cheap to read.
 int check_pairs(phmm_engine* e, const phmm_pair* pairs, int n, const Staged& s)
 {
-    for (int i = 0; i < n; ++i) {
-        if (pairs[i].read < 0 || pairs[i].read >= s.rd.n || pairs[i].hap < 0 || pairs[i].hap >= s.hp.n) { e->err = "pair index out of range"; return PHMM_ERR_INVALID; }
-    }
-    return PHMM_OK;
+    return phmm_checks::pair_indices(pairs, n, s.hp.n, s.rd.n, e->err);
 }
 
 // A caller's candidate positions, a CSR over n lists, on the device (copied for host space, aliased for device space); *total = off[n].
@@ -919,7 +916,8 @@ int phmm_engine_reset_haplotypes(phmm_engine* e, const phmm_error_model* m, int3
 static int pair_map_count(phmm_engine* e, const Staged& s, const int2* d_pairs, int n, long long* off_dev, long long* total)
 {
     int rc;
-    if (s.read_len_max - kKmer + 1 > 65535) { e->err = "read longer than 65540 bp: the device k-mer mapper counts votes in 16 bits"; return PHMM_ERR_INVALID; }
+    static_assert(kKmer == 6, "phmm_checks::mapper_reads assumes 6-mers");
+    if ((rc = phmm_checks::mapper_reads(s.read_len_max, e->err)) != PHMM_OK) return rc;
     if ((rc = prepare_mapper(e, s)) != PHMM_OK) return rc;
     CU(e->pm_best.ensure((size_t)n * sizeof(unsigned)));
     CU(e->pm_cnt.ensure((size_t)n * sizeof(int)));
@@ -976,15 +974,13 @@ static int align_impl(phmm_engine* e, const phmm_config* cfg, const phmm_haploty
                       int64_t* mapping_position, double* likelihood, char* cigar, int32_t cigar_stride, int32_t* status, int space,
                       bool map_on_device = false)
 {
-    if (!cfg || !pairs || !mapping_position || !likelihood || !cigar || !status || cigar_stride < 8) { e->err = "null argument / cigar_stride < 8"; return PHMM_ERR_INVALID; }
-    if (cfg->max_indel_error > 256) { e->err = "max_indel_error > 256"; return PHMM_ERR_BAND; }
-    if (cfg->nuc_prior < 0 || cfg->nuc_prior > 127) { e->err = "nuc_prior outside [0,127]"; return PHMM_ERR_INVALID; }
-    if (n_pairs < 0 || n_pairs > 0x7fffffff) { e->err = "pair count out of range"; return PHMM_ERR_INVALID; }
+    int rc = phmm_checks::align_arguments(cfg, pairs, n_pairs, mapping_position, likelihood, cigar, cigar_stride, status, e->err);
+    if (rc != PHMM_OK) return rc;
     if (n_pairs == 0) return PHMM_OK;
-    if (!reads || !reads->reverse || (!reads->mapq && cfg->use_mapping_quality)) { e->err = "reads->mapq / reads->reverse required"; return PHMM_ERR_INVALID; }
+    if ((rc = phmm_checks::align_reads(cfg, reads, e->err)) != PHMM_OK) return rc;
     const int band = round_band(std::max(1, cfg->max_indel_error));
     Staged s;
-    int rc = stage_batch(e, haps, reads, space, s);
+    rc = stage_batch(e, haps, reads, space, s);
     if (rc != PHMM_OK) return rc;
     const int n = (int)n_pairs;
     if (space == PHMM_SPACE_HOST && (rc = check_pairs(e, pairs, n, s))) return rc;
@@ -1332,13 +1328,10 @@ static void add_region(RegionSetup& setup, const phmm_config* cfg, int h0, int n
 static int region_setup(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
                         const phmm_regions* regions, RegionSetup& setup)
 {
-    if (!regions || regions->n <= 0 || !regions->hap_first || !regions->read_first || !haps || !reads) { e->err = "null / empty region list"; return PHMM_ERR_INVALID; }
-    if (regions->hap_first[0] != 0 || regions->read_first[0] != 0 || regions->hap_first[regions->n] != haps->n || regions->read_first[regions->n] != reads->n) {
-        e->err = "region ranges must cover the haplotype and read blocks exactly"; return PHMM_ERR_INVALID;
-    }
+    const int rc = phmm_checks::regions(haps, reads, regions, e->err);
+    if (rc != PHMM_OK) return rc;
     for (int g = 0; g < regions->n; ++g) {
         const int nH = regions->hap_first[g + 1] - regions->hap_first[g], nR = regions->read_first[g + 1] - regions->read_first[g];
-        if (nH <= 0 || nR <= 0) { e->err = "every region needs at least one haplotype and one read"; return PHMM_ERR_INVALID; }
         add_region(setup, cfg, regions->hap_first[g], nH, regions->read_first[g], nR, regions->flank ? regions->flank + g : nullptr);
     }
     return PHMM_OK;
@@ -2110,8 +2103,7 @@ int phmm_assign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haploty
     c.out = lnl; c.status = status; c.top = top;
     if ((rc = region_setup(e, cfg, haps, reads, groups, c.regions)) != PHMM_OK) return rc;
     if ((rc = phmm_checks::config_and_output(cfg, top, reads, e->err)) != PHMM_OK) return rc;
-    if (c.regions.Hmax > 64) { e->err = "more than 64 haplotypes in one group: a read's top set is a 64-bit mask"; return PHMM_ERR_INVALID; }
-    if (c.regions.total_out > 0x7fffffffLL) { e->err = "more than 2^31 - 1 (read, haplotype) pairs in one call"; return PHMM_ERR_INVALID; }
+    if ((rc = phmm_checks::assign_groups(groups, e->err)) != PHMM_OK) return rc;
     // the blocks are staged once: the pair mapper and the DP read the same device copies
     Staged s;
     if ((rc = stage_batch(e, haps, reads, space, s, false, true)) != PHMM_OK) return rc;
