@@ -265,6 +265,23 @@ int phmm_populate_regions(phmm_engine* e, const phmm_config* cfg,
 int phmm_assign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
                       const phmm_regions* groups, const double* log_priors, uint64_t* top, double* lnl, int32_t* status, int space);
 
+/* compute_haplotype_support over paired / linked templates (read_assigner.cpp:231-285, 45-64 with AlignedTemplate; the call
+ * BAMRealigner makes for every heterozygous genotype under the default --read-linkage paired, bam_realigner.cpp:241-300). Scoring is
+ * phmm_assign_reads' (every read with the uncapped mapper and evaluate); the choice is per TEMPLATE. Template t owns the reads
+ * [template_off[t], template_off[t+1]) of the block, in template order; template_off ([n_templates + 1]) is in HOST memory whatever
+ * `space`, starts at 0, ends at reads->n and increases strictly (every template has >= 1 read). Every group boundary read_first[g]
+ * is a template boundary, so each group owns >= 1 whole template.
+ *   top[t] (required, [n_templates]): bit k set <=> group-local haplotype k is in template t's find_map_haplotypes set over
+ *     sum_reads lnl + log_priors[h], the sum taken in read order from 0.0 (HaplotypeLikelihoodModel::evaluate(AlignedTemplate),
+ *     haplotype_likelihood_model.cpp:313-320); ties and empty sets as phmm_assign_reads.
+ *   lnl (optional): the template values, the groups' [H_g][T_g] matrices back to back (T_g: group g's templates).
+ *   status (optional): per READ, the groups' [H_g][R_g] matrices back to back, as phmm_assign_reads.
+ * groups, log_priors, errors, the 4096-position limit and SHORT_HAP statuses as phmm_assign_reads; with a single-read template per
+ * read the call returns exactly what phmm_assign_reads does. */
+int phmm_assign_templates(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                          const phmm_regions* groups, const int64_t* template_off, int32_t n_templates,
+                          const double* log_priors, uint64_t* top, double* lnl, int32_t* status, int space);
+
 /* phmm_populate with device-resident inputs and an output row stride: out[h * out_ld + r], out_ld >= R (status, optional, stays dense
  * [H][R]). `out` is any device-accessible address — in particular a window of ANOTHER GPU's matrix mapped with phmm_ipc_open: the
  * epilogue kernel then stores this rank's columns of a read-sharded [H, R_total] matrix (or its slab of a per-rank stack) straight
@@ -386,6 +403,13 @@ int  phmm_batcher_assign_reads(phmm_batcher* b, const phmm_config* cfg, const ph
 int  phmm_batcher_realign_reads(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
                                 const phmm_pair* pairs, int64_t n_pairs, const phmm_flank_state* flank,
                                 int64_t* mapping_position, double* likelihood, char* cigar, int32_t cigar_stride, int32_t* status);
+/* Template assignment through the shared engine: arguments as phmm_assign_templates with space = PHMM_SPACE_HOST, contract and policy
+ * as phmm_batcher_assign_reads (bit for bit the plain call alone; checked on the calling thread; a merged call that returns
+ * PHMM_ERR_INVALID is rerun member by member). A batch is one phmm_assign_templates call, the members' groups and templates one after
+ * the other; only template requests with identical configs merge, never with phmm_batcher_assign_reads requests. */
+int  phmm_batcher_assign_templates(phmm_batcher* b, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                                   const phmm_regions* groups, const int64_t* template_off, int32_t n_templates,
+                                   const double* log_priors, uint64_t* top, double* lnl, int32_t* status);
 /* Merged calls rerun one request at a time since creation (kept out of phmm_batcher_stats, whose layout callers compile against). */
 int64_t phmm_batcher_reruns(const phmm_batcher* b);
 

@@ -12,6 +12,7 @@ MUT_MAX_HAPLOTYPES, MUT_MAX_LENGTH, MUT_MAX_PAIRS = 4096, 65535, 1 << 26
 
 EXPORTS = ["phmm_version", "phmm_default_config", "phmm_create", "phmm_destroy", "phmm_last_error", "phmm_launch_count",
            "phmm_last_dp_kernel_ms", "phmm_last_dp_cells", "phmm_align_scores", "phmm_align_traceback", "phmm_align_reads", "phmm_align_pairs", "phmm_map_pairs", "phmm_realign_reads", "phmm_genotype_likelihoods", "phmm_populate", "phmm_populate_templates", "phmm_populate_regions", "phmm_assign_reads",
+           "phmm_assign_templates",
            "phmm_error_model_create", "phmm_error_model_create_custom", "phmm_error_model_destroy", "phmm_error_model_last_error",
            "phmm_reset_haplotypes", "phmm_engine_reset_haplotypes", "phmm_tandem_repeats", "phmm_mutation_model_create", "phmm_mutation_model_destroy", "phmm_mutation_context",
            "phmm_mutation_prime", "phmm_mutation_prime_sets", "phmm_batcher_mutation_prime", "phmm_wait_event", "phmm_engine_stream", "phmm_reserve_sms", "phmm_host_alloc", "phmm_host_free",
@@ -19,7 +20,7 @@ EXPORTS = ["phmm_version", "phmm_default_config", "phmm_create", "phmm_destroy",
            "phmm_batcher_create", "phmm_batcher_destroy", "phmm_batcher_last_error", "phmm_batcher_populate",
            "phmm_batcher_populate_templates", "phmm_batcher_stats_get", "phmm_populate_reset", "phmm_populate_regions_reset",
            "phmm_populate_templates_reset", "phmm_batcher_populate_reset", "phmm_batcher_populate_templates_reset",
-           "phmm_batcher_assign_reads", "phmm_batcher_realign_reads", "phmm_batcher_reruns"]
+           "phmm_batcher_assign_reads", "phmm_batcher_realign_reads", "phmm_batcher_reruns", "phmm_batcher_assign_templates"]
 
 
 class Config(C.Structure):
@@ -123,6 +124,9 @@ def load():
     lib.phmm_assign_reads.restype = C.c_int
     lib.phmm_assign_reads.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.POINTER(Regions),
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    lib.phmm_assign_templates.restype = C.c_int
+    lib.phmm_assign_templates.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.POINTER(Regions),
+                                          C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     lib.phmm_populate_templates.restype = C.c_int
     lib.phmm_populate_templates.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p, C.c_int32,
                                             C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_int]
@@ -161,6 +165,9 @@ def load():
     lib.phmm_batcher_assign_reads.restype = C.c_int
     lib.phmm_batcher_assign_reads.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.POINTER(Regions),
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.phmm_batcher_assign_templates.restype = C.c_int
+    lib.phmm_batcher_assign_templates.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.POINTER(Regions),
+                                                  C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.phmm_batcher_realign_reads.restype = C.c_int
     lib.phmm_batcher_realign_reads.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads), C.c_void_p,
                                                C.c_int64, C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]

@@ -178,18 +178,35 @@ def _realign(call, handle, sp, config, haps, reads, pairs, flank_state, cigar_st
     return rc, res.result()
 
 
-def _assign(call, handle, sp, config, haps, reads, hap_first, read_first, log_priors, want_likelihoods, want_status, *space):
-    """One assign call (phmm_assign_reads or phmm_batcher_assign_reads; `space` the engine's trailing memory-space argument):
-    (return code, the result PairHMMEngine.assign_reads returns)."""
+def _template_groups(template_off, template_first):
+    """Groups given in templates → (template offsets as host int64, the groups' read_first): group g's reads start at its first
+    template's first read."""
+    toff = np.ascontiguousarray(template_off.cpu().numpy() if _is_torch(template_off) else template_off, dtype=np.int64)
+    tf = np.ascontiguousarray(template_first, dtype=np.int64)
+    if toff.ndim != 1 or len(toff) < 2 or tf.ndim != 1 or len(tf) < 2 or tf.min() < 0 or tf.max() >= len(toff):
+        raise ValueError("template_first must index template_off, which needs at least one template")
+    return toff, toff[tf]
+
+
+def _assign(call, handle, sp, config, haps, reads, hap_first, read_first, log_priors, want_likelihoods, want_status, *space,
+            templates=None):
+    """One assign call (phmm_assign_reads or phmm_batcher_assign_reads; with templates = (template_off, template_first),
+    phmm_assign_templates or phmm_batcher_assign_templates; `space` the engine's trailing memory-space argument):
+    (return code, the result PairHMMEngine.assign_reads / assign_templates returns)."""
     regs, off = _regions(hap_first, read_first)
-    total = int(off[-1])
-    top = sp.empty(reads.n, np.int64 if sp.on_device else np.uint64)
-    lnl = sp.empty(total, np.float64) if want_likelihoods else None
-    status = sp.empty(total, np.int32) if want_status else None
+    n_top, n_values, tmpl = reads.n, int(off[-1]), ()
+    if templates is not None:
+        toff, template_first = templates
+        n_top = len(toff) - 1
+        n_values = int(_regions(hap_first, template_first)[1][-1])
+        tmpl = (toff.ctypes.data, n_top)
+    top = sp.empty(n_top, np.int64 if sp.on_device else np.uint64)
+    lnl = sp.empty(n_values, np.float64) if want_likelihoods else None
+    status = sp.empty(int(off[-1]), np.int32) if want_status else None
     pri = None if log_priors is None else sp.input(log_priors, np.float64)
     if pri is not None and pri.shape[0] != haps.n:
         raise ValueError("log_priors needs one value per haplotype of the block")
-    rc = call(handle, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), C.byref(regs), sp.ptr(pri), sp.ptr(top),
+    rc = call(handle, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), C.byref(regs), *tmpl, sp.ptr(pri), sp.ptr(top),
               sp.ptr(lnl), sp.ptr(status), *space)
     out = (top,)
     if want_likelihoods:
@@ -454,6 +471,22 @@ class PairHMMEngine(_Handle):
         self._check(rc, want_status)
         return res
 
+    def assign_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, hap_first, template_first, log_priors=None,
+                         want_likelihoods=False, want_status=False):
+        """compute_haplotype_support over paired / linked templates for many genotypes in one call (phmm_assign_templates). Template
+        t owns reads [template_off[t], template_off[t+1]) (at least one; template_off is moved to the host). Group g owns haplotypes
+        [hap_first[g], hap_first[g+1]) and templates [template_first[g], template_first[g+1]). Scoring as assign_reads; the choice is
+        per template, over the sum of its reads' likelihoods in read order plus the log prior.
+        Returns top ([T] uint64: bit k = group-local haplotype k is in the template's find_map_haplotypes set), plus the flat template
+        likelihoods (the groups' [H_g, T_g] matrices back to back) when want_likelihoods and the per-READ statuses (the groups'
+        [H_g, R_g] matrices) when want_status; numpy or torch CUDA tensors as assign_reads."""
+        sp = _Space.of(haps, reads)
+        toff, read_first = _template_groups(template_off, template_first)
+        rc, res = _assign(self._lib.phmm_assign_templates, self._h, sp, config, haps, reads, hap_first, read_first, log_priors,
+                          want_likelihoods, want_status, sp.flag, templates=(toff, template_first))
+        self._check(rc, want_status)
+        return res
+
     @staticmethod
     def split_regions(flat, off, hap_first, read_first):
         """The per-region [H_g, R_g] views of a populate_regions result."""
@@ -552,6 +585,17 @@ class PopulateBatcher(_Handle):
         assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
         rc, res = _assign(self._lib.phmm_batcher_assign_reads, self._h, _HOST, config, haps, reads, hap_first, read_first, log_priors,
                           want_likelihoods, want_status)
+        self._check(rc, want_status)
+        return res
+
+    def assign_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, hap_first, template_first, log_priors=None,
+                         want_likelihoods=False, want_status=False):
+        """As PairHMMEngine.assign_templates for host blocks (phmm_batcher_assign_templates): concurrent template requests with equal
+        configs run as one call, each with the top sets, template likelihoods and statuses it gets alone."""
+        assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
+        toff, read_first = _template_groups(template_off, template_first)
+        rc, res = _assign(self._lib.phmm_batcher_assign_templates, self._h, _HOST, config, haps, reads, hap_first, read_first, log_priors,
+                          want_likelihoods, want_status, templates=(toff, template_first))
         self._check(rc, want_status)
         return res
 

@@ -6,9 +6,10 @@ import sys
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB = os.path.join(_HERE, "libphmm_b200.so")
-SOURCES = ["phmm_engine.cu", "phmm_error_model.cpp", "phmm_batcher.cpp", "phmm_batcher_reset.cpp", "phmm_batcher_align.cpp"]
+SOURCES = ["phmm_engine.cu", "phmm_error_model.cpp", "phmm_batcher.cpp", "phmm_batcher_reset.cpp", "phmm_batcher_align.cpp",
+           "phmm_batcher_templates.cpp"]
 DEPS = ["phmm_engine.cu", "phmm_kernels.cuh", "phmm_device.cuh", "phmm_checks.h", "phmm_mutation.h", "phmm_reset.cuh", "phmm_error_model.cpp", "phmm_error_model_tables.inc",
-        "phmm_batcher.cpp", "phmm_batcher_reset.cpp", "phmm_batcher_align.cpp", "phmm_batcher_seam.h", os.path.join("..", "..", "include", "phmm_b200.h")]
+        "phmm_batcher.cpp", "phmm_batcher_reset.cpp", "phmm_batcher_align.cpp", "phmm_batcher_templates.cpp", "phmm_batcher_seam.h", os.path.join("..", "..", "include", "phmm_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]
 

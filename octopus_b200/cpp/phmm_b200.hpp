@@ -92,37 +92,62 @@ PairAlignments realign_reads(const phmm_reads& reads, std::size_t n, Call&& call
     return a;
 }
 
-// compute_haplotype_support's scoring and choice for many genotypes (phmm_assign_reads / phmm_batcher_assign_reads); host memory.
-// top[r] bit k = group-local haplotype k is in read r's find_map_haplotypes set. likelihood / status: the groups' [H_g][R_g]
-// matrices back to back. A short haplotype does not throw here: the code is PHMM_ERR_SHORT_HAPLOTYPE and the statuses carry the
-// extension.
+// compute_haplotype_support's scoring and choice for many genotypes (phmm_assign_reads / phmm_batcher_assign_reads, or per template
+// phmm_assign_templates / phmm_batcher_assign_templates); host memory. top[i] bit k = group-local haplotype k is in item i's
+// find_map_haplotypes set, an item being a read (or a template). likelihood: the groups' [H_g][items_g] matrices back to back; status:
+// the groups' [H_g][R_g] matrices, per read either way. A short haplotype does not throw here: the code is PHMM_ERR_SHORT_HAPLOTYPE
+// and the statuses carry the extension.
 struct ReadAssignment
 {
     std::vector<std::uint64_t> top;
     std::vector<double> likelihood;
     std::vector<std::int32_t> status;
+    std::vector<std::int32_t> read_first;      // the groups' first reads: the layout of status (for a template call, derived once
+                                               // from template_off)
     int code = PHMM_OK;
 };
 
-// The outputs of one assign call; call(groups, priors, top, likelihood, status) returns the call's code.
-template <typename Call>
-ReadAssignment assign_reads(const phmm_haplotypes& haplotypes, const phmm_reads& reads, const std::vector<std::int32_t>& hap_first,
-                            const std::vector<std::int32_t>& read_first, const std::vector<double>* log_priors, bool want_likelihoods,
-                            Call&& call)
+// sum over the groups of H_g x (first[g + 1] - first[g])
+inline std::size_t group_slots(const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& first)
 {
-    if (hap_first.empty() || hap_first.size() != read_first.size()) throw Error {PHMM_ERR_INVALID, "group bounds need n + 1 entries each"};
+    std::size_t slots = 0;
+    for (std::size_t g = 0; g + 1 < hap_first.size(); ++g)
+        slots += static_cast<std::size_t>(std::max(0, hap_first[g + 1] - hap_first[g])) * static_cast<std::size_t>(std::max(0, first[g + 1] - first[g]));
+    return slots;
+}
+
+// The outputs of one assign call of n_items items, the groups' items starting at item_first (read_first for a read call);
+// call(groups, priors, top, likelihood, status) returns the call's code.
+template <typename Call>
+ReadAssignment assign(const phmm_haplotypes& haplotypes, std::int64_t n_items, const std::vector<std::int32_t>& hap_first,
+                      const std::vector<std::int32_t>& read_first, const std::vector<std::int32_t>& item_first, const std::vector<double>* log_priors,
+                      bool want_likelihoods, Call&& call)
+{
+    if (hap_first.empty() || hap_first.size() != read_first.size() || hap_first.size() != item_first.size())
+        throw Error {PHMM_ERR_INVALID, "group bounds need n + 1 entries each"};
     const auto n = static_cast<std::int32_t>(hap_first.size() - 1);
     if (log_priors && log_priors->size() != static_cast<std::size_t>(haplotypes.n)) throw Error {PHMM_ERR_INVALID, "one log prior per haplotype"};
-    std::size_t pairs = 0;
-    for (std::int32_t g = 0; g < n; ++g)
-        pairs += static_cast<std::size_t>(std::max(0, hap_first[g + 1] - hap_first[g])) * static_cast<std::size_t>(std::max(0, read_first[g + 1] - read_first[g]));
     const phmm_regions groups {n, hap_first.data(), read_first.data(), nullptr};
     ReadAssignment a;
-    a.top.resize(static_cast<std::size_t>(std::max(0, reads.n)));
-    a.status.resize(pairs);
-    if (want_likelihoods) a.likelihood.resize(pairs);
+    a.top.resize(static_cast<std::size_t>(std::max<std::int64_t>(0, n_items)));
+    a.status.resize(group_slots(hap_first, read_first));
+    if (want_likelihoods) a.likelihood.resize(group_slots(hap_first, item_first));
+    a.read_first = read_first;
     a.code = call(groups, log_priors ? log_priors->data() : nullptr, a.top.data(), want_likelihoods ? a.likelihood.data() : nullptr, a.status.data());
     return a;
+}
+
+// The groups' first reads of a template call whose groups start at the templates template_first (template_off: n_templates + 1
+// read offsets).
+inline std::vector<std::int32_t> template_read_first(const std::int64_t* template_off, std::int32_t n_templates, const std::vector<std::int32_t>& template_first)
+{
+    std::vector<std::int32_t> read_first;
+    read_first.reserve(template_first.size());
+    for (std::int32_t t : template_first) {
+        if (!template_off || t < 0 || t > n_templates) throw Error {PHMM_ERR_INVALID, "template_first must index template_off"};
+        read_first.push_back(static_cast<std::int32_t>(template_off[t]));
+    }
+    return read_first;
 }
 
 } // namespace detail
@@ -179,9 +204,26 @@ public:
                                 const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
                                 const std::vector<double>* log_priors = nullptr, bool want_likelihoods = false) const
     {
-        ReadAssignment a = detail::assign_reads(haplotypes, reads, hap_first, read_first, log_priors, want_likelihoods,
-                                                [&] (const phmm_regions& groups, const double* priors, std::uint64_t* top, double* lnl, std::int32_t* st) {
+        ReadAssignment a = detail::assign(haplotypes, reads.n, hap_first, read_first, read_first, log_priors, want_likelihoods,
+                                          [&] (const phmm_regions& groups, const double* priors, std::uint64_t* top, double* lnl, std::int32_t* st) {
             return phmm_assign_reads(get(), &config, &haplotypes, &reads, &groups, priors, top, lnl, st, PHMM_SPACE_HOST);
+        });
+        if (a.code != PHMM_ERR_SHORT_HAPLOTYPE) check(a.code);
+        return a;
+    }
+
+    // The same per template (phmm_assign_templates): template t owns reads [template_off[t], template_off[t+1]); group g owns
+    // haplotypes [hap_first[g], hap_first[g+1]) and templates [template_first[g], template_first[g+1]). top and likelihood are per
+    // template, status per read.
+    ReadAssignment assign_templates(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
+                                    const std::int64_t* template_off, std::int32_t n_templates, const std::vector<std::int32_t>& hap_first,
+                                    const std::vector<std::int32_t>& template_first, const std::vector<double>* log_priors = nullptr,
+                                    bool want_likelihoods = false) const
+    {
+        const auto read_first = detail::template_read_first(template_off, n_templates, template_first);
+        ReadAssignment a = detail::assign(haplotypes, n_templates, hap_first, read_first, template_first, log_priors, want_likelihoods,
+                                          [&] (const phmm_regions& groups, const double* priors, std::uint64_t* top, double* lnl, std::int32_t* st) {
+            return phmm_assign_templates(get(), &config, &haplotypes, &reads, &groups, template_off, n_templates, priors, top, lnl, st, PHMM_SPACE_HOST);
         });
         if (a.code != PHMM_ERR_SHORT_HAPLOTYPE) check(a.code);
         return a;
@@ -220,7 +262,8 @@ public:
     }
     std::int64_t reruns() const { return phmm_batcher_reruns(handle_.get()); }
 
-    // Engine::realign_reads and Engine::assign_reads through the shared engine (phmm_batcher_realign_reads / _assign_reads)
+    // Engine::realign_reads, Engine::assign_reads and Engine::assign_templates through the shared engine (phmm_batcher_realign_reads /
+    // _assign_reads / _assign_templates)
     using PairAlignments = detail::PairAlignments;
     PairAlignments realign_reads(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
                                  const std::vector<phmm_pair>& pairs, const phmm_flank_state* flank_state = nullptr) const
@@ -235,9 +278,22 @@ public:
                                 const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& read_first,
                                 const std::vector<double>* log_priors = nullptr, bool want_likelihoods = false) const
     {
-        ReadAssignment a = detail::assign_reads(haplotypes, reads, hap_first, read_first, log_priors, want_likelihoods,
-                                                [&] (const phmm_regions& groups, const double* priors, std::uint64_t* top, double* lnl, std::int32_t* st) {
+        ReadAssignment a = detail::assign(haplotypes, reads.n, hap_first, read_first, read_first, log_priors, want_likelihoods,
+                                          [&] (const phmm_regions& groups, const double* priors, std::uint64_t* top, double* lnl, std::int32_t* st) {
             return phmm_batcher_assign_reads(get(), &config, &haplotypes, &reads, &groups, priors, top, lnl, st);
+        });
+        if (a.code != PHMM_ERR_SHORT_HAPLOTYPE) check(a.code);
+        return a;
+    }
+    ReadAssignment assign_templates(const phmm_config& config, const phmm_haplotypes& haplotypes, const phmm_reads& reads,
+                                    const std::int64_t* template_off, std::int32_t n_templates, const std::vector<std::int32_t>& hap_first,
+                                    const std::vector<std::int32_t>& template_first, const std::vector<double>* log_priors = nullptr,
+                                    bool want_likelihoods = false) const
+    {
+        const auto read_first = detail::template_read_first(template_off, n_templates, template_first);
+        ReadAssignment a = detail::assign(haplotypes, n_templates, hap_first, read_first, template_first, log_priors, want_likelihoods,
+                                          [&] (const phmm_regions& groups, const double* priors, std::uint64_t* top, double* lnl, std::int32_t* st) {
+            return phmm_batcher_assign_templates(get(), &config, &haplotypes, &reads, &groups, template_off, n_templates, priors, top, lnl, st);
         });
         if (a.code != PHMM_ERR_SHORT_HAPLOTYPE) check(a.code);
         return a;
@@ -636,14 +692,13 @@ struct HaplotypeSupport
 
 namespace detail {
 
-// compute_haplotype_support() on an Engine or a SharedEngine (both have assign_reads)
-template <typename AnyEngine>
-std::vector<HaplotypeSupport> haplotype_support(const ReadBlock& reads, const HaplotypeBlock& haplotypes, const std::vector<std::int32_t>& hap_first,
-                                                const std::vector<std::int32_t>& read_first, const std::vector<double>* log_priors,
-                                                AmbiguousAction action, const phmm_config& config, const AnyEngine& engine)
+// The groups' supports from an assignment whose items (reads or templates) start at item_first per group; the assignment's own
+// read_first lays out its statuses. Throws ShortHaplotypeError for the first short pair in the reference's order.
+inline std::vector<HaplotypeSupport> support(const ReadAssignment& a, const std::vector<std::int32_t>& hap_first,
+                                             const std::vector<std::int32_t>& item_first, AmbiguousAction action)
 {
-    const auto a = engine.assign_reads(config, haplotypes.view(), reads.view(), hap_first, read_first, log_priors);
     if (a.code == PHMM_ERR_SHORT_HAPLOTYPE) {
+        const std::vector<std::int32_t>& read_first = a.read_first;
         std::size_t slot = 0;
         for (std::size_t g = 0; g + 1 < hap_first.size(); ++g) {
             const auto nh = static_cast<std::size_t>(hap_first[g + 1] - hap_first[g]), nr = static_cast<std::size_t>(read_first[g + 1] - read_first[g]);
@@ -654,11 +709,11 @@ std::vector<HaplotypeSupport> haplotype_support(const ReadBlock& reads, const Ha
     }
     std::vector<HaplotypeSupport> result(hap_first.size() - 1);
     for (std::size_t g = 0; g + 1 < hap_first.size(); ++g) {
-        const auto nh = static_cast<std::size_t>(hap_first[g + 1] - hap_first[g]), nr = static_cast<std::size_t>(read_first[g + 1] - read_first[g]);
+        const auto nh = static_cast<std::size_t>(hap_first[g + 1] - hap_first[g]), nr = static_cast<std::size_t>(item_first[g + 1] - item_first[g]);
         HaplotypeSupport& s = result[g];
         s.reads.resize(nh);
         for (std::size_t i = 0; i < nr; ++i) {
-            const std::size_t r = static_cast<std::size_t>(read_first[g]) + i;
+            const std::size_t r = static_cast<std::size_t>(item_first[g]) + i;
             const std::uint64_t top = a.top[r];
             if ((top & (top - 1)) == 0) {                       // one haplotype
                 for (unsigned k = 0; k < nh; ++k) if (top >> k & 1u) s.reads[k].push_back(r);
@@ -672,6 +727,26 @@ std::vector<HaplotypeSupport> haplotype_support(const ReadBlock& reads, const Ha
         }
     }
     return result;
+}
+
+// compute_haplotype_support() on an Engine or a SharedEngine (both have assign_reads and assign_templates)
+template <typename AnyEngine>
+std::vector<HaplotypeSupport> haplotype_support(const ReadBlock& reads, const HaplotypeBlock& haplotypes, const std::vector<std::int32_t>& hap_first,
+                                                const std::vector<std::int32_t>& read_first, const std::vector<double>* log_priors,
+                                                AmbiguousAction action, const phmm_config& config, const AnyEngine& engine)
+{
+    return support(engine.assign_reads(config, haplotypes.view(), reads.view(), hap_first, read_first, log_priors), hap_first, read_first, action);
+}
+
+template <typename AnyEngine>
+std::vector<HaplotypeSupport> template_support(const TemplateBlock& templates, const HaplotypeBlock& haplotypes, const std::vector<std::int32_t>& hap_first,
+                                               const std::vector<std::int32_t>& template_first, const std::vector<double>* log_priors,
+                                               AmbiguousAction action, const phmm_config& config, const AnyEngine& engine)
+{
+    const auto n_templates = static_cast<std::int32_t>(templates.size());
+    const auto a = engine.assign_templates(config, haplotypes.view(), templates.reads.view(), templates.off.data(), n_templates, hap_first,
+                                           template_first, log_priors);
+    return support(a, hap_first, template_first, action);
 }
 
 } // namespace detail
@@ -696,6 +771,30 @@ inline std::vector<HaplotypeSupport> compute_haplotype_support(const ReadBlock& 
                                                                const phmm_config& config, const SharedEngine& engine)
 {
     return detail::haplotype_support(reads, haplotypes, hap_first, read_first, log_priors, action, config, engine);
+}
+
+// compute_haplotype_support over AlignedTemplates (read_assigner.cpp:322-459 with the template overload; BAMRealigner's call under
+// --read-linkage paired, bam_realigner.cpp:241-300) for many genotypes in one GPU call: group g owns haplotypes [hap_first[g],
+// hap_first[g+1]) and TEMPLATES [template_first[g], template_first[g+1]) of the block. Every read of a template is scored as
+// compute_haplotype_support scores reads; a template's value is the sum of its reads', and the choice is per template. The returned
+// HaplotypeSupport holds TEMPLATE indices (into the block), in its reads and in its ambiguous list. When a haplotype is too short,
+// throws ShortHaplotypeError for the first short (haplotype, read) pair in the reference's order (groups in turn, haplotypes in
+// genotype order, then reads: the template loop's order), with the block's haplotype index.
+inline std::vector<HaplotypeSupport> compute_haplotype_support(const TemplateBlock& templates, const HaplotypeBlock& haplotypes,
+                                                               const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& template_first,
+                                                               const std::vector<double>* log_priors, AmbiguousAction action,
+                                                               const phmm_config& config, const Engine& engine = Engine {})
+{
+    return detail::template_support(templates, haplotypes, hap_first, template_first, log_priors, action, config, engine);
+}
+
+// The same through a shared engine, with the same results and exceptions.
+inline std::vector<HaplotypeSupport> compute_haplotype_support(const TemplateBlock& templates, const HaplotypeBlock& haplotypes,
+                                                               const std::vector<std::int32_t>& hap_first, const std::vector<std::int32_t>& template_first,
+                                                               const std::vector<double>* log_priors, AmbiguousAction action,
+                                                               const phmm_config& config, const SharedEngine& engine)
+{
+    return detail::template_support(templates, haplotypes, hap_first, template_first, log_priors, action, config, engine);
 }
 
 using SampleName = std::string;

@@ -1,6 +1,7 @@
 // Shared engine for many host threads (include/phmm_b200.h, phmm_batcher_*): the populate requests that concurrent threads
 // have in flight are merged into one phmm_populate_regions call, their mutation-prime requests into one phmm_mutation_prime_sets
-// call, their assign and realign requests into one phmm_assign_reads / phmm_realign_reads call. Host C++ over the public C ABI; a
+// call, their assign, template assign and realign requests into one phmm_assign_reads / phmm_assign_templates / phmm_realign_reads
+// call. Host C++ over the public C ABI; a
 // batch runs the engine's existing multi-region / multi-set / pair-list kernel chain. No thread of its own: the first member of a
 // batch (its leader) makes the call.
 #include "../../include/phmm_b200.h"
@@ -407,7 +408,10 @@ struct Members {
 
 // Assign requests: a batch is one phmm_assign_reads call whose groups are the members' groups one after the other; equal configs
 // merge. The staging is populate's plus the log priors (zeros for a member without) and the top sets; lnl and status are always
-// staged and copied out to the members that asked for them.
+// staged and copied out to the members that asked for them. Template requests (phmm_batcher_assign_templates) merge only with each
+// other: their batch is one phmm_assign_templates call whose templates are the members' one after the other. Their top sets (one per
+// template, at most one per read) and template values (at most one per pair) fit the read-sized staging; each member's share of
+// them starts where the members before it end, which Assign::add records in the member's request.
 struct Assign : Members<struct AssignRequestSized> {
     using Sizes = PopulateBase::Sizes;
     enum { HAPS = PopulateBase::HAPS, HAP_BASES = PopulateBase::HAP_BASES, READS = PopulateBase::READS, PAIRS = PopulateBase::PAIRS };
@@ -432,8 +436,11 @@ struct Assign : Members<struct AssignRequestSized> {
 
     phmm_config cfg;
     const phmm_batcher_seam::AlignCalls* calls;
+    const phmm_batcher_seam::TemplateCalls* template_calls;       // a batch of template requests
     std::vector<int32_t> hap_first {0}, read_first {0};
     std::vector<phmm_flank_state> flanks;
+    std::vector<int64_t> template_off {0};
+    long long template_values = 0;                               // the template values of the members so far
 
     explicit Assign(const Request& q);
     void add(const Request& q, const Sizes& used);
@@ -445,11 +452,40 @@ struct Assign : Members<struct AssignRequestSized> {
 struct AssignRequestSized {
     const phmm_batcher_seam::AssignRequest* r;
     Assign::Sizes need;
+    long long template_values;          // a template request: its groups' [H_g][T_g] values
+    // a template request: its first template and first template value in the batch, set by Assign::add under the batcher's lock
+    // and read by copy_out after the call
+    mutable long long template_first = 0, value_first = 0;
 };
 
-std::string Assign::key(const Request& q) { return std::string(reinterpret_cast<const char*>(q.r->cfg), sizeof(phmm_config)); }
+std::string Assign::key(const Request& q)
+{
+    return std::string(reinterpret_cast<const char*>(q.r->cfg), sizeof(phmm_config)) + (q.r->template_calls ? "templates" : "reads");
+}
 
-Assign::Assign(const Request& q) : cfg(*q.r->cfg), calls(q.r->calls) {}
+Assign::Assign(const Request& q) : cfg(*q.r->cfg), calls(q.r->calls), template_calls(q.r->template_calls) {}
+
+// a request's own engine call, as the plain entry point makes it
+int assign_alone(phmm_engine* e, const phmm_batcher_seam::AssignRequest& r)
+{
+    if (r.template_calls)
+        return r.template_calls->assign(e, r.cfg, r.haps, r.reads, r.groups, r.template_off, r.n_templates, r.log_priors, r.top, r.lnl, r.status,
+                                        PHMM_SPACE_HOST);
+    return r.calls->assign(e, r.cfg, r.haps, r.reads, r.groups, r.log_priors, r.top, r.lnl, r.status, PHMM_SPACE_HOST);
+}
+
+// the [H_g][T_g] values of a template request's checked groups and templates
+long long count_template_values(const phmm_batcher_seam::AssignRequest& r)
+{
+    long long values = 0;
+    int t = 0;
+    for (int g = 0; g < r.groups->n; ++g) {
+        const int t0 = t;
+        while (t < r.n_templates && r.template_off[t] < r.groups->read_first[g + 1]) ++t;
+        values += (long long)(r.groups->hap_first[g + 1] - r.groups->hap_first[g]) * (t - t0);
+    }
+    return values;
+}
 
 // the member's groups, their bounds shifted to its slot (its slot ends at the batch's counts `used`); no flank is a flank state of 0
 void Assign::add(const Request& q, const Sizes& used)
@@ -461,6 +497,12 @@ void Assign::add(const Request& q, const Sizes& used)
         hap_first.push_back((int32_t)(h0 + g->hap_first[i + 1]));
         read_first.push_back((int32_t)(r0 + g->read_first[i + 1]));
         flanks.push_back(g->flank ? g->flank[i] : phmm_flank_state {0, 0, 0});
+    }
+    if (template_calls) {
+        q.template_first = (long long)template_off.size() - 1;
+        q.value_first = template_values;
+        for (int t = 0; t < q.r->n_templates; ++t) template_off.push_back(r0 + q.r->template_off[t + 1]);
+        template_values += q.template_values;
     }
 }
 
@@ -479,15 +521,15 @@ int Assign::run(phmm_engine* e, Staging& st, const Sizes& used)
                               st.gap_open.p, st.gap_extend.p, st.hap_begin.p};
     const phmm_reads rv = st.reads(used);
     const phmm_regions groups {(int32_t)flanks.size(), hap_first.data(), read_first.data(), flanks.data()};
-    const int rc = calls->assign(e, &cfg, &hv, &rv, &groups, st.priors.p, st.top.p, st.out.p, st.status.p, PHMM_SPACE_HOST);
-    rerun_if_invalid(e, rc, [](phmm_engine* en, const Request& q) {
-        const phmm_batcher_seam::AssignRequest& r = *q.r;
-        return r.calls->assign(en, r.cfg, r.haps, r.reads, r.groups, r.log_priors, r.top, r.lnl, r.status, PHMM_SPACE_HOST);
-    });
+    const int rc = template_calls ? template_calls->assign(e, &cfg, &hv, &rv, &groups, template_off.data(), (int32_t)template_off.size() - 1,
+                                                           st.priors.p, st.top.p, st.out.p, st.status.p, PHMM_SPACE_HOST)
+                                  : calls->assign(e, &cfg, &hv, &rv, &groups, st.priors.p, st.top.p, st.out.p, st.status.p, PHMM_SPACE_HOST);
+    rerun_if_invalid(e, rc, [](phmm_engine* en, const Request& q) { return assign_alone(en, *q.r); });
     return rc;
 }
 
-// this member's reads' top sets and its groups' slots; its code from its own statuses, as the call's would be for it alone
+// this member's reads' (or templates') top sets and its groups' slots (or template values); its code from its own statuses, as the
+// call's would be for it alone
 int Assign::copy_out(const Staging& st, const Sizes& at, const Request& q, int rc, const std::string& err) const
 {
     if (reran) return own(q);
@@ -498,8 +540,13 @@ int Assign::copy_out(const Staging& st, const Sizes& at, const Request& q, int r
     rc = PHMM_OK;
     for (long long i = 0; i < P; ++i) if ((res_status[i] & 0xFFFF) == PHMM_STATUS_SHORT_HAP) { rc = PHMM_ERR_SHORT_HAPLOTYPE; break; }
     t_error = rc == PHMM_OK ? std::string() : std::string("Haplotype is too short for alignment");
-    std::memcpy(r.top, st.top.p + at[READS], (size_t)q.need[READS] * sizeof(uint64_t));
-    if (r.lnl) std::memcpy(r.lnl, st.out.p + at[PAIRS], (size_t)P * sizeof(double));
+    if (template_calls) {
+        std::memcpy(r.top, st.top.p + q.template_first, (size_t)r.n_templates * sizeof(uint64_t));
+        if (r.lnl) std::memcpy(r.lnl, st.out.p + q.value_first, (size_t)q.template_values * sizeof(double));
+    } else {
+        std::memcpy(r.top, st.top.p + at[READS], (size_t)q.need[READS] * sizeof(uint64_t));
+        if (r.lnl) std::memcpy(r.lnl, st.out.p + at[PAIRS], (size_t)P * sizeof(double));
+    }
     if (r.status) std::memcpy(r.status, res_status, (size_t)P * sizeof(int32_t));
     return rc;
 }
@@ -892,11 +939,13 @@ struct InFlight {
 int phmm_batcher_seam::submit_assign(phmm_batcher* b, const AssignRequest& r)
 {
     if (!b) { t_error = "null batcher"; return PHMM_ERR_INVALID; }
-    // phmm_assign_reads' host checks in its order: the groups, the config and top, the group limits, the blocks, the mapper's limits
+    // phmm_assign_reads' (phmm_assign_templates') host checks in its order: the groups, the config and top, the group limits, (the
+    // templates,) the blocks, the mapper's limits
     int rc;
     if ((rc = phmm_checks::regions(r.haps, r.reads, r.groups, t_error)) != PHMM_OK) return rc;
     if ((rc = phmm_checks::config_and_output(r.cfg, r.top, r.reads, t_error)) != PHMM_OK) return rc;
     if ((rc = phmm_checks::assign_groups(r.groups, t_error)) != PHMM_OK) return rc;
+    if (r.template_calls && (rc = phmm_checks::assign_templates(r.template_off, r.n_templates, r.reads, r.groups, t_error)) != PHMM_OK) return rc;
     if ((rc = phmm_checks::blocks(r.haps, r.reads, t_error)) != PHMM_OK) return rc;
     long long len_min, len_max;
     phmm_checks::read_length_range(r.reads, &len_min, &len_max);
@@ -915,11 +964,9 @@ int phmm_batcher_seam::submit_assign(phmm_batcher* b, const AssignRequest& r)
     std::string penalty_error;
     InFlight guard(b);
     if (r.haps->n > kMaxBatchHaps || pairs > kMaxBatchPairs || max_hap > 65535 || phmm_checks::penalties(r.haps, hap_bases, penalty_error) != PHMM_OK) {
-        return run_alone(b, [&](phmm_engine* e) {
-            return r.calls->assign(e, r.cfg, r.haps, r.reads, r.groups, r.log_priors, r.top, r.lnl, r.status, PHMM_SPACE_HOST);
-        });
+        return run_alone(b, [&](phmm_engine* e) { return assign_alone(e, r); });
     }
-    const Assign::Request q {&r, {{r.haps->n, hap_bases, r.reads->n, read_bases, pairs}}};
+    const Assign::Request q {&r, {{r.haps->n, hap_bases, r.reads->n, read_bases, pairs}}, r.template_calls ? count_template_values(r) : 0};
     return take_part(b, b->assign, q);
 }
 

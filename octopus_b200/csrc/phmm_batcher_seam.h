@@ -1,6 +1,6 @@
-// The seam between the request batcher (phmm_batcher.cpp) and its populate requests with an error model (phmm_batcher_reset.cpp)
-// and its assign / realign requests (phmm_batcher_align.cpp). phmm_batcher_reset.cpp computes a request's model key; both hand the
-// batcher the engine calls as function pointers, so that phmm_batcher.cpp names no engine symbol beyond the plain populate and
+// The seam between the request batcher (phmm_batcher.cpp) and its populate requests with an error model (phmm_batcher_reset.cpp),
+// its assign / realign requests (phmm_batcher_align.cpp) and its template assign requests (phmm_batcher_templates.cpp).
+// phmm_batcher_reset.cpp computes a request's model key; each hands the batcher the engine calls as function pointers, so that phmm_batcher.cpp names no engine symbol beyond the plain populate and
 // mutation ones and no error-model internals: a fake engine can stand behind each part.
 #ifndef PHMM_BATCHER_SEAM_H
 #define PHMM_BATCHER_SEAM_H
@@ -42,11 +42,19 @@ struct AlignCalls {
     decltype(&phmm_realign_reads) realign;
 };
 
-// One request of phmm_batcher_assign_reads.
+// The engine call of the template assign requests (phmm_batcher_templates.cpp).
+struct TemplateCalls {
+    decltype(&phmm_assign_templates) assign;
+};
+
+// One request of phmm_batcher_assign_reads (template_calls NULL) or phmm_batcher_assign_templates (calls NULL): top and lnl are then
+// per template.
 struct AssignRequest {
     const AlignCalls* calls;
     const phmm_config* cfg; const phmm_haplotypes* haps; const phmm_reads* reads; const phmm_regions* groups;
     const double* log_priors; uint64_t* top; double* lnl; int32_t* status;
+    const TemplateCalls* template_calls = nullptr;
+    const int64_t* template_off = nullptr; int32_t n_templates = 0;
 };
 
 // One request of phmm_batcher_realign_reads.

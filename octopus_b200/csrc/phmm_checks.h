@@ -171,6 +171,24 @@ inline int template_offsets(const int64_t* template_off, int32_t n_templates, co
     return PHMM_OK;
 }
 
+// phmm_assign_templates' templates (host memory) on a checked group list: they cover the reads exactly, each has at least one read,
+// and no group boundary falls inside one
+inline int assign_templates(const int64_t* template_off, int32_t n_templates, const phmm_reads* reads, const phmm_regions* groups, std::string& err)
+{
+    if (!template_off || n_templates <= 0) { err = "null / empty template offsets"; return PHMM_ERR_INVALID; }
+    if (template_off[0] != 0 || template_off[n_templates] != reads->n) { err = "template offsets must cover the reads exactly"; return PHMM_ERR_INVALID; }
+    for (int t = 0; t < n_templates; ++t) {
+        if (template_off[t + 1] <= template_off[t]) { err = "template offsets must be strictly increasing (every template needs a read)"; return PHMM_ERR_INVALID; }
+    }
+    // both lists increase strictly, so one merge pass finds every group boundary among the template boundaries
+    int t = 0;
+    for (int g = 1; g < groups->n; ++g) {
+        while (t < n_templates && template_off[t] < groups->read_first[g]) ++t;
+        if (template_off[t] != groups->read_first[g]) { err = "a group boundary falls inside a template"; return PHMM_ERR_INVALID; }
+    }
+    return PHMM_OK;
+}
+
 // phmm_mutation_prime's checks of one haplotype set (host memory), in its order
 inline int mutation_haplotype_count(int64_t n, std::string& err)
 {

@@ -74,6 +74,7 @@ struct phmm_engine {
     DBuf rhash, kbins, kitems, kpos, kcnt, ftasks, fcnt, gtasks, atasks, gcnt, sched, sorted, fb_scratch, fb_pairs, npre_f, npre_r;
     DBuf pm_best, pm_cnt, pm_inl, pm_part, pm_misc;   // the pair mapper's first pass (k_kmer_map_pairs) and its offset scan
     DBuf as_pairs, as_prior, as_top;                  // phmm_assign_reads: slot-ordered pair list, log priors, top sets
+    DBuf at_groups, at_off, at_lnl;                   // phmm_assign_templates: per-group template layout, template offsets, values
     DBuf mu_in, mu_list, mu_res, mu_cig, mu_out;      // phmm_mutation_prime: staged set, DP pair list, per-tile results, CIGARs, matrix
     DBuf rs_sub, rs_model, rs_words, rs_runs, rs_flags;   // phmm_engine_reset_haplotypes: flags, model tables, scratch slots, overflow
     std::vector<cudaEvent_t> tile_events;
@@ -1338,8 +1339,9 @@ static int region_setup(phmm_engine* e, const phmm_config* cfg, const phmm_haplo
 }
 
 // One populate call as its entry point describes it. Every call has a region list. Candidate position lists and templates need a
-// single region; `staged` marks phmm_assign_reads, whose matrix stays on the device: the call chooses every read's haplotypes
-// there (k_assign_top) and copies out top and the optional out / status only.
+// single region; `staged` marks phmm_assign_reads / phmm_assign_templates, whose matrix stays on the device: the call chooses every
+// read's (k_assign_top) or every template's (k_assign_template_top) haplotypes there and copies out top and the optional out / status
+// only. An assign call with templates has them in any number of regions: out is then the regions' [H_g][T_g] template values.
 struct PopulateCall {
     const phmm_config* cfg = nullptr;
     const phmm_haplotypes* haps = nullptr;
@@ -1360,7 +1362,8 @@ struct PopulateCall {
     const int32_t* mapped_pos = nullptr;
     long long n_mapped = 0;
     const double* log_priors = nullptr;
-    uint64_t* top = nullptr;
+    uint64_t* top = nullptr;                        // per read, or per template when the call has templates
+    std::vector<TemplateGroup> template_groups;     // phmm_assign_templates: each region's templates (template_off in host memory)
     // the _reset entry points: `haps` holds the sequences block's n / off / seq / begin only; pop_reset derives the six arrays from
     // the sequences under `model` on the device, and the call populates from those
     bool reset = false;
@@ -1448,7 +1451,7 @@ static int pop_stage(phmm_engine* e, const PopulateCall& c, PopState& st)
     if (rc != PHMM_OK) return rc;
     const bool several = c.regions.regs.size() > 1;
     if (c.listed() && several) { e->err = "candidate position lists are not supported with several regions"; return PHMM_ERR_INVALID; }
-    if (c.template_off && several) { e->err = "templates are not supported with several regions"; return PHMM_ERR_INVALID; }
+    if (c.template_off && several && !c.assign()) { e->err = "templates are not supported with several regions"; return PHMM_ERR_INVALID; }
     Staged& s = st.s;
     if (c.assign()) s = *c.staged;
     else if (c.reset) rc = stage_batch(e, &st.reset_haps, c.reads, c.space, s, false, true, PHMM_SPACE_DEVICE, &st.reset_off_host);
@@ -1985,7 +1988,35 @@ static int pop_finish(phmm_engine* e, const PopulateCall& c, PopState& st)
     CU(cudaGetLastError());
     // only a host-space chunk of a larger matrix is copied out row by row: device-space calls wrote their rows in place
     const bool pitched = host && c.out_pitch != 0 && c.out_pitch != R;
-    if (c.template_off) {
+    if (c.assign()) {
+        // every read's or every template's top set from the finished matrix; then only top and the optional out / status leave the device
+        const bool by_template = c.template_off != nullptr;
+        const long long n_top = by_template ? c.n_templates : R;
+        unsigned long long* d_top = (unsigned long long*)c.top;
+        if (host) { CU(e->as_top.ensure((size_t)n_top * sizeof(uint64_t))); d_top = e->as_top.as<unsigned long long>(); }
+        double* d_values = st.d_out;
+        long long n_values = HR;
+        if (by_template) {
+            const TemplateGroup& last = c.template_groups.back();
+            n_values = last.tout_off + (long long)c.regions.regs.back().nH * last.nT;
+            const long long* d_toff;
+            const TemplateGroup* d_groups;
+            if ((rc = stage(e, e->at_off, (const long long*)c.template_off, (size_t)c.n_templates + 1, PHMM_SPACE_HOST, &d_toff))) return rc;
+            if ((rc = stage(e, e->at_groups, c.template_groups.data(), c.template_groups.size(), PHMM_SPACE_HOST, &d_groups))) return rc;
+            d_values = c.out;
+            if (host && c.out) { CU(e->at_lnl.ensure((size_t)n_values * sizeof(double))); d_values = e->at_lnl.as<double>(); }
+            k_assign_template_top<<<(unsigned)((c.n_templates + 127) / 128), 128, 0, e->stream>>>(c.n_templates, st.G, e->regs.as<RegionInfo>(),
+                                                                                                   d_groups, d_toff, st.d_out, c.log_priors, d_top, d_values);
+        } else {
+            k_assign_top<<<(unsigned)((st.G + 3) / 4), 128, 0, e->stream>>>(st.G, e->regs.as<RegionInfo>(), st.d_out, c.log_priors, d_top);
+        }
+        LAUNCHED();
+        CU(cudaGetLastError());
+        if (host) {
+            CU(cudaMemcpyAsync(c.top, d_top, (size_t)n_top * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+            if (c.out) CU(cudaMemcpyAsync(c.out, d_values, (size_t)n_values * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        }
+    } else if (c.template_off) {
         // paired / linked reads: one value per (haplotype, template)
         const long long* d_toff;
         if ((rc = stage(e, e->tasks_lane, (const long long*)c.template_off, (size_t)c.n_templates + 1, c.space, &d_toff))) return rc;
@@ -1996,17 +2027,6 @@ static int pop_finish(phmm_engine* e, const PopulateCall& c, PopState& st)
         LAUNCHED();
         CU(cudaGetLastError());
         if (host) CU(cudaMemcpyAsync(c.out, d_tout, (size_t)HT * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
-    } else if (c.assign()) {
-        // every read's top set from the finished matrix; then only top and the optional out / status leave the device
-        unsigned long long* d_top = (unsigned long long*)c.top;
-        if (host) { CU(e->as_top.ensure((size_t)R * sizeof(uint64_t))); d_top = e->as_top.as<unsigned long long>(); }
-        k_assign_top<<<(unsigned)((st.G + 3) / 4), 128, 0, e->stream>>>(st.G, e->regs.as<RegionInfo>(), st.d_out, c.log_priors, d_top);
-        LAUNCHED();
-        CU(cudaGetLastError());
-        if (host) {
-            CU(cudaMemcpyAsync(c.top, d_top, (size_t)R * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-            if (c.out) CU(cudaMemcpyAsync(c.out, st.d_out, (size_t)HR * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
-        }
     } else if (pitched) {
         CU(cudaMemcpy2DAsync(c.out, (size_t)c.out_pitch * sizeof(double), st.d_out, (size_t)R * sizeof(double), (size_t)R * sizeof(double), H, cudaMemcpyDeviceToHost, e->stream));
     } else if (host) {
@@ -2093,8 +2113,13 @@ int phmm_populate_regions(phmm_engine* e, const phmm_config* cfg,
     return populate_impl(e, c);
 }
 
-int phmm_assign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
-                      const phmm_regions* groups, const double* log_priors, uint64_t* top, double* lnl, int32_t* status, int space)
+} // extern "C"
+
+// The body of phmm_assign_reads and phmm_assign_templates: the group checks, then (templates: their checks and layout) one staging,
+// the uncapped pair mapper over the slot pairs and populate_impl, which chooses the top sets on the device.
+static int assign_impl(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads, const phmm_regions* groups,
+                       const int64_t* template_off, int32_t n_templates, const double* log_priors, uint64_t* top, double* lnl, int32_t* status,
+                       int space, bool by_template)
 {
     int rc;
     if ((rc = begin_call(e))) return rc;
@@ -2104,6 +2129,18 @@ int phmm_assign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haploty
     if ((rc = region_setup(e, cfg, haps, reads, groups, c.regions)) != PHMM_OK) return rc;
     if ((rc = phmm_checks::config_and_output(cfg, top, reads, e->err)) != PHMM_OK) return rc;
     if ((rc = phmm_checks::assign_groups(groups, e->err)) != PHMM_OK) return rc;
+    if (by_template) {
+        if ((rc = phmm_checks::assign_templates(template_off, n_templates, reads, groups, e->err)) != PHMM_OK) return rc;
+        c.template_off = template_off; c.n_templates = n_templates;
+        long long tout = 0;
+        int t = 0;
+        for (const RegionInfo& r : c.regions.regs) {
+            const int t0 = t;
+            while (t < n_templates && template_off[t] < r.r0 + r.nR) ++t;
+            c.template_groups.push_back({t0, t - t0, tout});
+            tout += (long long)r.nH * (t - t0);
+        }
+    }
     // the blocks are staged once: the pair mapper and the DP read the same device copies
     Staged s;
     if ((rc = stage_batch(e, haps, reads, space, s, false, true)) != PHMM_OK) return rc;
@@ -2121,6 +2158,21 @@ int phmm_assign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haploty
         c.mapped_off = e->c_off.as<long long>(); c.mapped_pos = e->c_pos.as<int32_t>();
     }
     return populate_impl(e, c);
+}
+
+extern "C" {
+
+int phmm_assign_reads(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                      const phmm_regions* groups, const double* log_priors, uint64_t* top, double* lnl, int32_t* status, int space)
+{
+    return assign_impl(e, cfg, haps, reads, groups, nullptr, 0, log_priors, top, lnl, status, space, false);
+}
+
+int phmm_assign_templates(phmm_engine* e, const phmm_config* cfg, const phmm_haplotypes* haps, const phmm_reads* reads,
+                          const phmm_regions* groups, const int64_t* template_off, int32_t n_templates,
+                          const double* log_priors, uint64_t* top, double* lnl, int32_t* status, int space)
+{
+    return assign_impl(e, cfg, haps, reads, groups, template_off, n_templates, log_priors, top, lnl, status, space, true);
 }
 
 int phmm_populate_ld(phmm_engine* e, const phmm_config* cfg,

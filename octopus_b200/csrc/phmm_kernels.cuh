@@ -917,6 +917,45 @@ __global__ void k_assign_top(const int n_regions, const RegionInfo* __restrict__
     }
 }
 
+// phmm_assign_templates: the templates of one group (region), [t0, t0 + nT) of the call's list, and where its [nH][nT] template
+// values start in the caller's lnl.
+struct TemplateGroup { int t0, nT; long long tout_off; };
+
+// find_map_haplotypes over AlignedTemplates (read_assigner.cpp:45-64) for every template of every group: one thread per template of
+// the call, so a group of tens of thousands of templates spreads over the whole grid as a call of many small groups does. The
+// thread finds its group by binary search over the groups' first templates. Template t owns the reads [toff[t], toff[t+1]) of its
+// group. Its value for haplotype k is the sum of its reads' finished values out[pair_slot] left to right from 0.0 (k_template_sum's
+// order, HaplotypeLikelihoodModel::evaluate(AlignedTemplate), haplotype_likelihood_model.cpp:313-320), written to tlnl when it is
+// given; the prior is added and the set chosen by k_assign_top's rule. top[t] bit k = haplotype h0 + k is in template t's set.
+__global__ void k_assign_template_top(const int n_templates, const int n_regions, const RegionInfo* __restrict__ regs,
+                                      const TemplateGroup* __restrict__ tgroups, const long long* __restrict__ toff,
+                                      const double* __restrict__ out, const double* __restrict__ log_priors,
+                                      unsigned long long* __restrict__ top, double* __restrict__ tlnl)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_templates) return;
+    const int t = (int)i;
+    int lo = 0, hi = n_regions;                 // largest g with tgroups[g].t0 <= t (every group owns >= 1 template)
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (tgroups[mid].t0 <= t) lo = mid; else hi = mid; }
+    const RegionInfo reg = regs[lo];
+    const TemplateGroup tg = tgroups[lo];
+    const int tl = t - tg.t0;
+    const long long first = toff[t] - reg.r0, last = toff[t + 1] - reg.r0;
+    double max_value = -1.7976931348623157e308;                          // std::numeric_limits<double>::lowest()
+    unsigned long long set = 0ull;
+    for (int k = 0; k < reg.nH; ++k) {
+        const double* row = out + reg.out_off + (long long)k * reg.nR;
+        double sum = 0.0;
+        for (long long rl = first; rl < last; ++rl) sum = __dadd_rn(sum, row[rl]);
+        if (tlnl) tlnl[tg.tout_off + (long long)k * tg.nT + tl] = sum;
+        const double cur = __dadd_rn(sum, log_priors ? log_priors[reg.h0 + k] : 0.0);
+        if (almost_equal_ulp1(cur, max_value)) set |= 1ull << k;
+        else if (cur > max_value) { set = 1ull << k; max_value = cur; }
+    }
+    if (set == 0ull) set = reg.nH == 64 ? ~0ull : (1ull << reg.nH) - 1ull;
+    top[t] = set;
+}
+
 // Fast-path DP over the task lists the classify pass (k_populate_generic<.., true>) produced. Persistent warps: each warp
 // repeatedly claims G consecutive read pairs of equal length (G = 1, 2 or 4 lane groups; G > 1 keeps the lanes busy when a
 // read has fewer than 32 tasks, i.e. few haplotypes), stages each pair's row entries in shared memory once, and runs
