@@ -416,7 +416,9 @@ int64_t phmm_batcher_reruns(const phmm_batcher* b);
 /* Consumer of the matrix ("next" row N1): ConstantMixtureGenotypeLikelihoodModel::evaluate for G genotypes of one ploidy
  * (core/models/genotype/constant_mixture_genotype_likelihood_model.cpp:30-140) over a [H][R] matrix in `space`:
  *   out[g] = sum_r ( log_sum_exp_{h in genotype g} lnl[h*R + r] - ln ploidy ),   genotypes[g*ploidy + k] = haplotype index.
- * Keeping the matrix on the device and returning G numbers instead of H*R removes the D2H / gather volume. */
+ * Keeping the matrix on the device and returning G numbers instead of H*R removes the D2H / gather volume. 0 <= ploidy <= 64;
+ * ploidy 0 writes G zeros and reads neither lnl nor genotypes (which may then be null). An index outside [0, n_haplotypes)
+ * returns PHMM_ERR_INVALID, in either space (device-space indices are checked by the kernel before it reads the matrix). */
 int phmm_genotype_likelihoods(phmm_engine* e, const double* lnl, int32_t n_haplotypes, int32_t n_reads,
                               const int32_t* genotypes, int32_t n_genotypes, int32_t ploidy, double* out, int space);
 

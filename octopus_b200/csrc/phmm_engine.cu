@@ -709,22 +709,34 @@ int phmm_genotype_likelihoods(phmm_engine* e, const double* lnl, int32_t H, int3
                               const int32_t* genotypes, int32_t G, int32_t ploidy, double* out, int space)
 {
     if (int rc0 = begin_call(e)) return rc0;
-    if (!lnl || !genotypes || !out || H <= 0 || R <= 0 || G < 0 || ploidy < 0 || ploidy > 64) { e->err = "bad argument"; return PHMM_ERR_INVALID; }
-    if (G == 0) return PHMM_OK;
+    if (!lnl || H <= 0 || R <= 0 || G < 0 || ploidy < 0 || ploidy > 64) { e->err = "bad argument"; return PHMM_ERR_INVALID; }
+    if (G == 0) return PHMM_OK;       // empty arrays may come as null pointers (an empty torch tensor's data pointer)
+    if (!out || (!genotypes && ploidy > 0)) { e->err = "bad argument"; return PHMM_ERR_INVALID; }
+    if (ploidy == 0) {   // the empty genotype's likelihood is 0 (ln 1) whatever the reads; nothing is read
+        if (space == PHMM_SPACE_HOST) { std::fill(out, out + G, 0.0); return PHMM_OK; }
+        CU(cudaMemsetAsync(out, 0, (size_t)G * sizeof(double), e->stream));
+        CU(cudaStreamSynchronize(e->stream));
+        return PHMM_OK;
+    }
     const double* d_lnl; const int32_t* d_gt;
     int rc;
-    if ((rc = stage(e, e->out, lnl, (size_t)H * R, space, &d_lnl))) return rc;
-    if ((rc = stage(e, e->pairs, genotypes, (size_t)G * std::max(ploidy, 1), space, &d_gt))) return rc;
-    if (space == PHMM_SPACE_HOST) {   // haplotype indices are checked where they are cheap to read
+    if (space == PHMM_SPACE_HOST) {   // haplotype indices are checked where they are cheap to read (the kernel checks device ones)
         for (long long i = 0; i < (long long)G * ploidy; ++i) if (genotypes[i] < 0 || genotypes[i] >= H) { e->err = "haplotype index out of range"; return PHMM_ERR_INVALID; }
     }
+    if ((rc = stage(e, e->out, lnl, (size_t)H * R, space, &d_lnl))) return rc;
+    if ((rc = stage(e, e->pairs, genotypes, (size_t)G * ploidy, space, &d_gt))) return rc;
     CU(e->scores.ensure((size_t)G * sizeof(double)));
+    CU(e->counters.ensure(sizeof(int)));
+    CU(cudaMemsetAsync(e->counters.p, 0, sizeof(int), e->stream));
     double* d_out = space == PHMM_SPACE_DEVICE ? out : e->scores.as<double>();
-    k_genotype_likelihoods<<<G, 256, 0, e->stream>>>(d_lnl, R, d_gt, ploidy, d_out);
+    k_genotype_likelihoods<<<G, 256, 0, e->stream>>>(d_lnl, H, R, d_gt, ploidy, d_out, e->counters.as<int>());
     LAUNCHED();
     CU(cudaGetLastError());
+    int bad = 0;
+    CU(cudaMemcpyAsync(&bad, e->counters.p, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
     if (space == PHMM_SPACE_HOST) CU(cudaMemcpyAsync(out, d_out, (size_t)G * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
+    if (bad) { e->err = "haplotype index out of range"; return PHMM_ERR_INVALID; }
     return PHMM_OK;
 }
 

@@ -1834,12 +1834,28 @@ __global__ void k_template_sum(const double* __restrict__ lnl, const int H, cons
 // N1 (SURVEY.md §8f): ConstantMixtureGenotypeLikelihoodModel::evaluate on the resident [H][R] matrix
 // (core/models/genotype/constant_mixture_genotype_likelihood_model.cpp:30-140): one block per genotype,
 // ln p(reads | g) = sum_r ( log_sum_exp_{h in g} lnl[h][r] - ln ploidy ); homozygous genotypes reduce to a plain sum.
+// 1 <= ploidy <= 64 (the host answers ploidy 0 itself). A genotype with an index outside [0, H) reads nothing from lnl: its
+// out[g] is NaN and *bad gets bit 0, which the host turns into PHMM_ERR_INVALID.
 __global__ void __launch_bounds__(256)
-k_genotype_likelihoods(const double* __restrict__ lnl, const int R, const int* __restrict__ genotypes, const int ploidy, double* __restrict__ out)
+k_genotype_likelihoods(const double* __restrict__ lnl, const int H, const int R, const int* __restrict__ genotypes, const int ploidy,
+                       double* __restrict__ out, int* __restrict__ bad)
 {
     __shared__ double partial[256];
+    __shared__ int gt[64];
+    __shared__ int out_of_range;
     const int g = blockIdx.x;
-    const int* gt = genotypes + (size_t)g * ploidy;
+    if (threadIdx.x == 0) out_of_range = 0;
+    __syncthreads();
+    if ((int)threadIdx.x < ploidy) {
+        const int h = genotypes[(size_t)g * ploidy + threadIdx.x];
+        gt[threadIdx.x] = h;
+        if (h < 0 || h >= H) out_of_range = 1;
+    }
+    __syncthreads();
+    if (out_of_range) {
+        if (threadIdx.x == 0) { out[g] = __longlong_as_double(0x7ff8000000000000LL); atomicOr(bad, 1); }
+        return;
+    }
     bool homo = true;
     for (int k = 1; k < ploidy; ++k) homo = homo && gt[k] == gt[0];
     const double ln_ploidy = log((double)ploidy);
@@ -1855,7 +1871,7 @@ k_genotype_likelihoods(const double* __restrict__ lnl, const int R, const int* _
     partial[threadIdx.x] = acc;
     __syncthreads();
     for (int s = 128; s > 0; s >>= 1) { if ((int)threadIdx.x < s) partial[threadIdx.x] += partial[threadIdx.x + s]; __syncthreads(); }
-    if (threadIdx.x == 0) out[g] = ploidy == 0 ? 0.0 : partial[0];
+    if (threadIdx.x == 0) out[g] = partial[0];
 }
 
 __global__ void k_fill_int(int* __restrict__ p, const long long n, const int v)

@@ -582,31 +582,73 @@ int oracle_model_align(int band, const char* hap, int hap_len, const char* read,
     return 0;
 }
 
-/* N1 — ConstantMixtureGenotypeLikelihoodModel::evaluate (core/models/genotype/constant_mixture_genotype_likelihood_model.cpp:30-140)
- * over a [H][R] matrix: ln p(reads | genotype) = sum_r ( ln sum_{h in g} p(r | h) - ln ploidy ), sequential accumulation like
- * std::accumulate / std::inner_product; homozygous → plain sum (:87-89), diploid → log_sum_exp(a, b) - ln 2 (:90-96),
- * otherwise max + log(sum exp(x - max)) - ln ploidy (:131-140; the triploid special forms :98-129 are the same quantity). */
+/* maths::log_sum_exp (utils/maths.hpp) over n >= 1 terms: the largest term plus ln of the sum, taken in order, of exp(x_k - max).
+ * The three-term overload is this with n = 3 (0 + x is exact). */
+static double log_sum_exp_n(const double* x, int n)
+{
+    double mx = x[0];
+    for (int k = 1; k < n; ++k) if (x[k] > mx) mx = x[k];
+    double s = 0.0;
+    for (int k = 0; k < n; ++k) s += exp(x[k] - mx);
+    return mx + log(s);
+}
+
+/* N1 — ConstantMixtureGenotypeLikelihoodModel::evaluate(const Genotype<IndexedHaplotype<>>&) (core/models/genotype/
+ * constant_mixture_genotype_likelihood_model.cpp:66-77, 163-319) over a [H][R] matrix, form by form as the reference dispatches:
+ * ln p(reads | g) = sum_r ( ln sum_{h in g} p(r | h) - ln ploidy ), accumulated read by read from 0 like std::accumulate /
+ * std::inner_product. A run of m equal adjacent indices enters once, as ln m + its value:
+ *   ploidy 0: 0;  1: the plain sum;  2: homozygous the plain sum, else log_sum_exp(a, b) - ln 2 (log1p form);
+ *   3: homozygous the plain sum, [a a b] log_sum_exp(ln 2 + a, b), [a b b] log_sum_exp(a, ln 2 + b), else the three-term form,
+ *      each - ln 3;
+ *   4: homozygous the plain sum, [a a a b] / [a b b b] log_sum_exp(ln 3 + a, b) / (a, ln 3 + b) - ln 4, [a a b b]
+ *      log_sum_exp(a, b) - ln 2, [a a b c] / [a b b c] / [a b c c] the three-term form with ln 2 on the doubled one, - ln 4,
+ *      else the four-term form - ln 4;
+ *   5 and up: the buffer form, log_sum_exp over all ploidy values - ln ploidy, with no homozygous shortcut.
+ * The constants ln 2, ln 3, ln 4 are the doubles nearest them, as the reference's lookup table holds them. */
 void oracle_genotype_likelihoods(const double* lnl, int H, int R, const int32_t* genotypes, int G, int ploidy, double* out)
 {
+    static const double LN2 = 0.693147180559945309417232121458176568, LN3 = 1.098612288668109691395245236922525705,
+                        LN4 = 1.386294361119890618834464242916353136;
     (void)H;
     for (int g = 0; g < G; ++g) {
         const int32_t* gt = genotypes + (size_t)g * ploidy;
-        int homo = 1;
-        for (int k = 1; k < ploidy; ++k) if (gt[k] != gt[0]) homo = 0;
-        double acc = 0.0;
-        if (ploidy == 0) { out[g] = 0.0; continue; }
-        if (homo) {
-            for (int r = 0; r < R; ++r) acc += lnl[(size_t)gt[0] * R + r];
+        const double* row[64];
+        for (int k = 0; k < ploidy; ++k) row[k] = lnl + (size_t)gt[k] * R;
+        double acc = 0.0, x[64];
+        if (ploidy == 0) {
+            /* the empty genotype: ln 1 */
+        } else if (ploidy == 1 || (ploidy <= 4 && gt[0] == gt[1] && (ploidy < 3 || gt[1] == gt[2]) && (ploidy < 4 || gt[2] == gt[3]))) {
+            for (int r = 0; r < R; ++r) acc += row[0][r];
         } else if (ploidy == 2) {
-            for (int r = 0; r < R; ++r) acc += log_sum_exp2(lnl[(size_t)gt[0] * R + r], lnl[(size_t)gt[1] * R + r]) - 0.693147180559945309417232121458176568;
+            for (int r = 0; r < R; ++r) acc += log_sum_exp2(row[0][r], row[1][r]) - LN2;
+        } else if (ploidy == 3) {
+            const int e01 = gt[0] == gt[1], e12 = gt[1] == gt[2];
+            for (int r = 0; r < R; ++r) {
+                double v;
+                if (e01) v = log_sum_exp2(LN2 + row[0][r], row[2][r]);
+                else if (e12) v = log_sum_exp2(row[0][r], LN2 + row[1][r]);
+                else { x[0] = row[0][r]; x[1] = row[1][r]; x[2] = row[2][r]; v = log_sum_exp_n(x, 3); }
+                acc += v - LN3;
+            }
+        } else if (ploidy == 4) {
+            const int e01 = gt[0] == gt[1], e12 = gt[1] == gt[2], e23 = gt[2] == gt[3];
+            for (int r = 0; r < R; ++r) {
+                const double a = row[0][r], b = row[1][r], c = row[2][r], d = row[3][r];
+                double v;
+                if (e01 && e12) v = log_sum_exp2(LN3 + a, d) - LN4;
+                else if (e01 && e23) v = log_sum_exp2(a, c) - LN2;
+                else if (e01) { x[0] = LN2 + a; x[1] = c; x[2] = d; v = log_sum_exp_n(x, 3) - LN4; }
+                else if (e12 && e23) v = log_sum_exp2(a, LN3 + b) - LN4;
+                else if (e12) { x[0] = a; x[1] = LN2 + b; x[2] = d; v = log_sum_exp_n(x, 3) - LN4; }
+                else if (e23) { x[0] = a; x[1] = b; x[2] = LN2 + c; v = log_sum_exp_n(x, 3) - LN4; }
+                else { x[0] = a; x[1] = b; x[2] = c; x[3] = d; v = log_sum_exp_n(x, 4) - LN4; }
+                acc += v;
+            }
         } else {
             const double ln_ploidy = log((double)ploidy);
             for (int r = 0; r < R; ++r) {
-                double mx = lnl[(size_t)gt[0] * R + r];
-                for (int k = 1; k < ploidy; ++k) { const double v = lnl[(size_t)gt[k] * R + r]; if (v > mx) mx = v; }
-                double sum = 0.0;
-                for (int k = 0; k < ploidy; ++k) sum += exp(lnl[(size_t)gt[k] * R + r] - mx);
-                acc += mx + log(sum) - ln_ploidy;
+                for (int k = 0; k < ploidy; ++k) x[k] = row[k][r];
+                acc += log_sum_exp_n(x, ploidy) - ln_ploidy;
             }
         }
         out[g] = acc;

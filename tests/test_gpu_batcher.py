@@ -3,6 +3,7 @@ into one multi-region kernel chain, each request with exactly the result it gets
 import ctypes as C
 import os
 import subprocess
+import tempfile
 import threading
 
 import numpy as np
@@ -13,21 +14,22 @@ from helpers import random_positions, random_region
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cpp", "test_batcher.cpp")
-EXE = os.path.join(ROOT, "tests", "cpp", "test_batcher")
 BAD_PENALTY = "snv prior / gap penalty outside [0,127]"
 
 
 def _build_cpp():
+    """Compile the driver into a fresh temporary directory (the source tree may be read-only) and return its path."""
     from octopus_b200 import build
     build.build()
+    exe = os.path.join(tempfile.mkdtemp(prefix="test_batcher_"), "test_batcher")
     subprocess.run(["g++", "-std=c++14", "-O1", "-pthread", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "octopus_b200", "cpp"),
-                    SRC, "-o", EXE, "-L", os.path.join(ROOT, "octopus_b200"), "-lphmm_b200",
+                    SRC, "-o", exe, "-L", os.path.join(ROOT, "octopus_b200"), "-lphmm_b200",
                     "-Wl,-rpath," + os.path.join(ROOT, "octopus_b200")], check=True)
+    return exe
 
 
 def test_cpp_shared_engine_driver_compiles():
-    _build_cpp()
-    assert os.path.exists(EXE)
+    assert os.path.exists(_build_cpp())
 
 
 def test_batcher_create_without_gpu_is_a_cuda_error():
@@ -270,6 +272,6 @@ def test_lone_thread_is_never_stuck_waiting_for_clients():
 
 @pytest.mark.gpu
 def test_cpp_threads_share_one_engine():
-    _build_cpp()
-    out = subprocess.run([EXE], capture_output=True, text=True, timeout=300)
+    exe = _build_cpp()
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0 and "BATCHER ok" in out.stdout, out.stdout + out.stderr

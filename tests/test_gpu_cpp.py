@@ -1,6 +1,7 @@
 """A plain C++ program (g++, no torch) drives the engine through the C ABI and the C++ adapter header."""
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 import pytest
@@ -9,26 +10,27 @@ from exact import assert_mix_within_bound, assert_same_penalties, penalties
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cpp", "test_cabi.cpp")
-EXE = os.path.join(ROOT, "tests", "cpp", "test_cabi")
 
 
 def _build():
+    """Compile the program into a fresh temporary directory (the source tree may be read-only) and return its path."""
     from octopus_b200 import build
     build.build()
+    exe = os.path.join(tempfile.mkdtemp(prefix="test_cabi_"), "test_cabi")
     subprocess.run(["g++", "-std=c++14", "-O1", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "octopus_b200", "cpp"),
-                    SRC, "-o", EXE, "-L", os.path.join(ROOT, "octopus_b200"), "-lphmm_b200",
+                    SRC, "-o", exe, "-L", os.path.join(ROOT, "octopus_b200"), "-lphmm_b200",
                     "-Wl,-rpath," + os.path.join(ROOT, "octopus_b200")], check=True)
+    return exe
 
 
 def test_cpp_adapter_compiles_against_the_abi():
-    _build()
-    assert os.path.exists(EXE)
+    assert os.path.exists(_build())
 
 
 @pytest.mark.gpu
 def test_cpp_client_matches_oracle_exactly(coracle):
-    _build()
-    out = subprocess.run([EXE], capture_output=True, text=True, timeout=120)
+    exe = _build()
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stdout + out.stderr
     lines = dict((l.split()[0] + (l.split()[1] if l.startswith(("ROW", "EXACT")) else ""), l.split()) for l in out.stdout.strip().splitlines())
     assert lines["KAT"][1:] == ["84", "84", "0", "CCCCACGTATATATATATATATGGGGACGT", "CCCCACGT---------------GGGACGT"]

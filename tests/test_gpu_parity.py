@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from exact import (LOWEST, assert_mix_within_bound, assert_same_penalties, assert_sums_within_bound, effective_mapq, penalties)
+from genotype_exact import assert_within_bound, exact_genotypes, kernel_chain
 from helpers import random_positions, random_region
 
 pytestmark = pytest.mark.gpu
@@ -274,8 +275,10 @@ def test_genotype_likelihood_reduction_on_the_resident_matrix(engine, coracle):
         got_dev = engine.genotype_likelihoods(m_dev, gts)
         got_host = engine.genotype_likelihoods(m, gts)
         assert isinstance(got_dev, torch.Tensor)
+        ex = exact_genotypes(m, gts)
         for got in (got_dev.cpu().numpy(), got_host):
-            assert np.all(np.abs(got - want) <= 1e-9 * np.maximum(np.abs(want), 1.0)), ploidy
+            assert_within_bound(got, ex, kernel_chain(m.shape[1]), "ploidy %d" % ploidy)
+        assert_within_bound(want, ex, m.shape[1], "oracle, ploidy %d" % ploidy)
 
 
 def test_populate_edge_cases(engine, coracle):

@@ -4,6 +4,7 @@ with max_mapping_positions = the haplotype length, and phmm_realign_reads agains
 the C oracle's restatements of both stand in (tests/test_realign_oracle.py pins its mapper to the reference's)."""
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 import pytest
@@ -327,17 +328,17 @@ def test_large_call_equals_its_two_halves(engine):
 
 
 CPP_SRC = os.path.join(ROOT, "tests", "cpp", "test_realign.cpp")
-CPP_EXE = os.path.join(ROOT, "tests", "cpp", "test_realign")
 
 
 def test_cpp_realign_helper(refhmm, coracle):
     from octopus_b200 import build
     from octopus_b200.batch import pack_haplotypes, pack_reads
     build.build()
+    exe = os.path.join(tempfile.mkdtemp(prefix="test_realign_"), "test_realign")     # the source tree may be read-only
     subprocess.run(["g++", "-std=c++14", "-O1", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "octopus_b200", "cpp"),
-                    CPP_SRC, "-o", CPP_EXE, "-L", os.path.join(ROOT, "octopus_b200"), "-lphmm_b200",
+                    CPP_SRC, "-o", exe, "-L", os.path.join(ROOT, "octopus_b200"), "-lphmm_b200",
                     "-Wl,-rpath," + os.path.join(ROOT, "octopus_b200")], check=True)
-    out = subprocess.run([CPP_EXE], capture_output=True, text=True, timeout=120)
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stdout + out.stderr
     lines = [l.split() for l in out.stdout.strip().splitlines()]
     # the same blocks as the program builds
