@@ -16,7 +16,9 @@
  *
  * Conventions: plain pointers and sizes only; every pointer of one call lives in the memory space named by
  * `space` (host memory, or device memory of the engine's GPU); the caller owns all buffers; calls are
- * synchronous (results complete on return) unless stated; functions return PHMM_OK or a negative error code
+ * synchronous (results complete on return) unless stated; device-space pointers are read and written on the
+ * engine's own stream, so work on another stream that still produces or reads them must be ordered before the
+ * call with phmm_wait_event; functions return PHMM_OK or a negative error code
  * and never throw — the C++ adapter (octopus_b200/cpp/phmm_b200.hpp) re-throws the reference's exceptions.
  * An engine handle is not re-entrant (one per host thread, like the reference's per-thread model copies,
  * haplotype_likelihood_array.cpp:172); threads that want to share one engine use a phmm_batcher.

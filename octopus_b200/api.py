@@ -43,12 +43,13 @@ def _is_torch(x):
 
 class _Space:
     """The memory space of one call: numpy arrays on the host, or torch tensors on one CUDA device."""
-    __slots__ = ("device", "on_device", "flag")
+    __slots__ = ("device", "on_device", "flag", "enqueued")
 
     def __init__(self, device=None):
         self.device = device
         self.on_device = device is not None
         self.flag = _lib.SPACE_DEVICE if self.on_device else _lib.SPACE_HOST
+        self.enqueued = False       # the call's own conversions, fills or allocations went to torch's current stream
 
     @classmethod
     def of(cls, haps, reads):
@@ -65,6 +66,7 @@ class _Space:
         """An output array; zeroed where the call may leave entries unwritten."""
         if self.on_device:
             import torch
+            self.enqueued = True
             return (torch.zeros if zeroed else torch.empty)(shape, dtype=self.dtype(dtype), device=self.device)
         return (np.zeros if zeroed else np.empty)(shape, dtype=dtype)
 
@@ -73,8 +75,18 @@ class _Space:
         if self.on_device:
             import torch
             t = x if _is_torch(x) else torch.as_tensor(np.ascontiguousarray(x, dtype=dtype), device=self.device)
-            return t.to(device=self.device, dtype=self.dtype(dtype)).contiguous()
+            t = t.to(device=self.device, dtype=self.dtype(dtype)).contiguous()
+            self.enqueued |= t is not x
+            return t
         return np.ascontiguousarray(x, dtype=dtype)
+
+    def order(self, engine):
+        """Right before the C call: make the engine's stream wait for torch's current stream if this call put work there itself.
+        The engine reads and writes on its own stream, so it must start after a conversion or a zero-fill, and after queued work
+        still reading an output block the caching allocator handed back from a freed tensor. Buffers the caller supplies as they
+        are take no wait; the caller orders those with engine.wait_event."""
+        if self.enqueued:
+            engine._wait_for_current_stream(self.device)
 
     ptr = staticmethod(_ptr)        # the data pointer of a numpy array or torch tensor, or None
 
@@ -167,13 +179,14 @@ class _Alignments:
         return self.mp, self.lk, [text[j * s:(j + 1) * s].split(b"\0", 1)[0].decode() for j in range(self.n)], self.st
 
 
-def _realign(call, handle, sp, config, haps, reads, pairs, flank_state, cigar_stride, *space):
-    """One realign call (phmm_realign_reads or phmm_batcher_realign_reads; `space` the engine's trailing memory-space argument):
-    (return code, the result PairHMMEngine.realign_reads returns)."""
+def _realign(call, owner, sp, config, haps, reads, pairs, flank_state, cigar_stride, *space):
+    """One realign call (phmm_realign_reads or phmm_batcher_realign_reads on owner's handle; `space` the engine's trailing
+    memory-space argument): (return code, the result PairHMMEngine.realign_reads returns)."""
     pr = sp.input(pairs, np.int32).reshape(-1, 2)
     n = pr.shape[0]
     res = _Alignments(sp, reads, n, cigar_stride)
-    rc = call(handle, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), sp.ptr(pr), n, _ref(_flank(flank_state)),
+    sp.order(owner)
+    rc = call(owner._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), sp.ptr(pr), n, _ref(_flank(flank_state)),
               *res.pointers(), *space)
     return rc, res.result()
 
@@ -188,10 +201,10 @@ def _template_groups(template_off, template_first):
     return toff, toff[tf]
 
 
-def _assign(call, handle, sp, config, haps, reads, hap_first, read_first, log_priors, want_likelihoods, want_status, *space,
+def _assign(call, owner, sp, config, haps, reads, hap_first, read_first, log_priors, want_likelihoods, want_status, *space,
             templates=None):
-    """One assign call (phmm_assign_reads or phmm_batcher_assign_reads; with templates = (template_off, template_first),
-    phmm_assign_templates or phmm_batcher_assign_templates; `space` the engine's trailing memory-space argument):
+    """One assign call (phmm_assign_reads or phmm_batcher_assign_reads on owner's handle; with templates = (template_off,
+    template_first), phmm_assign_templates or phmm_batcher_assign_templates; `space` the engine's trailing memory-space argument):
     (return code, the result PairHMMEngine.assign_reads / assign_templates returns)."""
     regs, off = _regions(hap_first, read_first)
     n_top, n_values, tmpl = reads.n, int(off[-1]), ()
@@ -206,7 +219,8 @@ def _assign(call, handle, sp, config, haps, reads, hap_first, read_first, log_pr
     pri = None if log_priors is None else sp.input(log_priors, np.float64)
     if pri is not None and pri.shape[0] != haps.n:
         raise ValueError("log_priors needs one value per haplotype of the block")
-    rc = call(handle, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), C.byref(regs), *tmpl, sp.ptr(pri), sp.ptr(top),
+    sp.order(owner)
+    rc = call(owner._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), C.byref(regs), *tmpl, sp.ptr(pri), sp.ptr(top),
               sp.ptr(lnl), sp.ptr(status), *space)
     out = (top,)
     if want_likelihoods:
@@ -271,6 +285,7 @@ class _Handle:
 class PairHMMEngine(_Handle):
     """One engine handle (not re-entrant; one per host thread, like the reference's per-thread model copies)."""
     _destroy = "phmm_destroy"
+    _stream_event = None
 
     def __init__(self, device=-1):
         self._create("phmm_create", int(device))
@@ -281,9 +296,22 @@ class PairHMMEngine(_Handle):
     # -- stream ordering -----------------------------------------------------------------------------------------
     def wait_event(self, event):
         """Make the engine's stream wait (on the device) for a CUDA event — a torch.cuda.Event or a raw cudaEvent_t — recorded
-        after work on another stream that still reads a buffer the next call will overwrite (phmm_wait_event)."""
+        after work on another stream that still writes a buffer the next call reads, or still reads one it will overwrite
+        (phmm_wait_event). Every call runs on the engine's own stream. A device-space call that converts an argument or
+        allocates an output or status tensor waits for torch's current stream itself, through this method. Device buffers the caller
+        passes as they are (blocks, pairs, priors or ``out``, already in the right dtype and layout) are the caller's to order:
+        record an event after the work that produces or still reads them and hand it here before the call."""
         handle = getattr(event, "cuda_event", event)
         self._check(self._lib.phmm_wait_event(self._h, C.c_void_p(int(handle))))
+
+    def _wait_for_current_stream(self, device):
+        """wait_event on an event recorded now on torch's current stream of `device`. One event per engine, recorded again each
+        time: the wait takes the event's state when it is issued, and an engine serves one thread."""
+        import torch
+        if self._stream_event is None:
+            self._stream_event = torch.cuda.Event()
+        self._stream_event.record(torch.cuda.current_stream(device))
+        self.wait_event(self._stream_event)
 
     def reserve_sms(self, n):
         """Keep the first n SMs free of persistent DP blocks, for a collective running beside the next call (phmm_reserve_sms)."""
@@ -338,6 +366,7 @@ class PairHMMEngine(_Handle):
             t = t.reshape(-1, 4)
         n = t.shape[0]
         out = sp.empty(n, np.int32)
+        sp.order(self)
         self._check(self._lib.phmm_align_scores(self._h, int(band), int(precision_bits), int(nuc_prior), C.byref(haps.c_struct()),
                                                 C.byref(reads.c_struct()), sp.ptr(t), n, sp.ptr(out), sp.flag))
         return out
@@ -401,6 +430,7 @@ class PairHMMEngine(_Handle):
 
         def attempt(cap):
             off, pos = sp.empty(n + 1, np.int64), sp.empty(cap, np.int32)
+            sp.order(self)
             self._check(self._lib.phmm_map_pairs(self._h, hs, rs, sp.ptr(pr), n, sp.ptr(off), sp.ptr(pos), cap, sp.flag))
             total = int(off[-1])
             return total, (off, pos[:total])
@@ -412,7 +442,7 @@ class PairHMMEngine(_Handle):
         only). pairs: (n, 2) int32 rows (read, hap). Returns (mapping_position[n], likelihood[n], cigars[list of str], status[n]) as
         align_reads; for device-resident blocks the three arrays are torch CUDA tensors."""
         sp = _Space.of(haps, reads)
-        rc, res = _realign(self._lib.phmm_realign_reads, self._h, sp, config, haps, reads, pairs, flank_state, cigar_stride, sp.flag)
+        rc, res = _realign(self._lib.phmm_realign_reads, self, sp, config, haps, reads, pairs, flank_state, cigar_stride, sp.flag)
         self._check(rc)
         return res
 
@@ -422,6 +452,7 @@ class PairHMMEngine(_Handle):
         sp = _Space(lnl.device if _is_torch(lnl) else None)
         m, gt = sp.input(lnl, np.float64), sp.input(genotypes, np.int32)
         out = sp.empty(gt.shape[0], np.float64)
+        sp.order(self)
         self._check(self._lib.phmm_genotype_likelihoods(self._h, sp.ptr(m), m.shape[0], m.shape[1], sp.ptr(gt), gt.shape[0], gt.shape[1],
                                                         sp.ptr(out), sp.flag))
         return out
@@ -451,6 +482,7 @@ class PairHMMEngine(_Handle):
         if out is None:
             out = sp.empty(total, np.float64)
         status = sp.empty(total, np.int32) if want_status else None
+        sp.order(self)
         self._check(_call(self._lib, "phmm_populate_regions", self._h, config, haps, error_model, C.byref(reads.c_struct()), C.byref(regs),
                           sp.ptr(out), sp.ptr(status), sp.flag), want_status)
         return (out, off, status) if want_status else (out, off)
@@ -466,7 +498,7 @@ class PairHMMEngine(_Handle):
         want_status: numpy for host blocks, torch CUDA tensors for device-resident ones (top then as int64 with the same bits). With want_status a short haplotype does not
         raise; its statuses carry the extension and top is unspecified."""
         sp = _Space.of(haps, reads)
-        rc, res = _assign(self._lib.phmm_assign_reads, self._h, sp, config, haps, reads, hap_first, read_first, log_priors, want_likelihoods,
+        rc, res = _assign(self._lib.phmm_assign_reads, self, sp, config, haps, reads, hap_first, read_first, log_priors, want_likelihoods,
                           want_status, sp.flag)
         self._check(rc, want_status)
         return res
@@ -482,7 +514,7 @@ class PairHMMEngine(_Handle):
         [H_g, R_g] matrices) when want_status; numpy or torch CUDA tensors as assign_reads."""
         sp = _Space.of(haps, reads)
         toff, read_first = _template_groups(template_off, template_first)
-        rc, res = _assign(self._lib.phmm_assign_templates, self._h, sp, config, haps, reads, hap_first, read_first, log_priors,
+        rc, res = _assign(self._lib.phmm_assign_templates, self, sp, config, haps, reads, hap_first, read_first, log_priors,
                           want_likelihoods, want_status, sp.flag, templates=(toff, template_first))
         self._check(rc, want_status)
         return res
@@ -498,7 +530,10 @@ class PairHMMEngine(_Handle):
         """Returns the (H, R) matrix of ln-likelihoods (numpy float64, or a torch CUDA tensor for device-resident blocks).
         positions: None or (off[H*R+1] int64, pos int32) CSR in [H][R] order. flank_state: None or (lhs_flank, rhs_flank).
         With ``error_model`` (an ErrorModel), haps is a HaplotypeSequences block: the GPU runs the model's reset() for every
-        haplotype in the same call (phmm_populate_reset), with the result of error_model.reset + populate."""
+        haplotype in the same call (phmm_populate_reset), with the result of error_model.reset + populate.
+        out: None, or a float64 [H, R] CUDA tensor (or a column window of a wider one) for device-resident blocks. Without it the
+        call allocates the result and waits for torch's current stream first; with it, and without want_status or positions to
+        convert, the call issues no wait, so work still reading ``out`` from an earlier step must be ordered with wait_event."""
         sp = _Space.of(haps, reads)
         H, R = haps.n, reads.n
         if out is None:
@@ -506,14 +541,15 @@ class PairHMMEngine(_Handle):
         status = sp.empty((H, R), np.int32) if want_status else None
         if sp.on_device and (tuple(out.shape) != (H, R) or out.dtype != sp.dtype(np.float64) or (R > 1 and out.stride(1) != 1)):
             raise ValueError("out must be a float64 [H, R] tensor with unit column stride")
+        if error_model is not None and sp.on_device and H > 1 and out.stride(0) != R:
+            raise ValueError("populate with an error model writes a dense [H, R] matrix")
+        pos = _ref(_positions(sp, positions))
+        sp.order(self)
         if error_model is not None:
-            if sp.on_device and H > 1 and out.stride(0) != R:
-                raise ValueError("populate with an error model writes a dense [H, R] matrix")
-            self._check(_call(self._lib, "phmm_populate", self._h, config, haps, error_model, C.byref(reads.c_struct()),
-                              _ref(_positions(sp, positions)), _ref(_flank(flank_state)), sp.ptr(out), sp.ptr(status), sp.flag), want_status)
+            self._check(_call(self._lib, "phmm_populate", self._h, config, haps, error_model, C.byref(reads.c_struct()), pos,
+                              _ref(_flank(flank_state)), sp.ptr(out), sp.ptr(status), sp.flag), want_status)
             return (out, status) if want_status else out
-        args = (self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), _ref(_positions(sp, positions)),
-                _ref(_flank(flank_state)))
+        args = (self._h, _config(config), C.byref(haps.c_struct()), C.byref(reads.c_struct()), pos, _ref(_flank(flank_state)))
         if sp.on_device and H > 1 and out.stride(0) != R:
             # a column window of a wider matrix — possibly another GPU's (octopus_b200.peer): phmm_populate_ld
             rc = self._lib.phmm_populate_ld(*args, sp.ptr(out), int(out.stride(0)), sp.ptr(status))
@@ -583,7 +619,7 @@ class PopulateBatcher(_Handle):
         """As PairHMMEngine.assign_reads for host blocks (phmm_batcher_assign_reads): concurrent requests with equal configs run as one
         call, each with the top sets, likelihoods and statuses it gets alone."""
         assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
-        rc, res = _assign(self._lib.phmm_batcher_assign_reads, self._h, _HOST, config, haps, reads, hap_first, read_first, log_priors,
+        rc, res = _assign(self._lib.phmm_batcher_assign_reads, self, _HOST, config, haps, reads, hap_first, read_first, log_priors,
                           want_likelihoods, want_status)
         self._check(rc, want_status)
         return res
@@ -594,7 +630,7 @@ class PopulateBatcher(_Handle):
         configs run as one call, each with the top sets, template likelihoods and statuses it gets alone."""
         assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
         toff, read_first = _template_groups(template_off, template_first)
-        rc, res = _assign(self._lib.phmm_batcher_assign_templates, self._h, _HOST, config, haps, reads, hap_first, read_first, log_priors,
+        rc, res = _assign(self._lib.phmm_batcher_assign_templates, self, _HOST, config, haps, reads, hap_first, read_first, log_priors,
                           want_likelihoods, want_status, templates=(toff, template_first))
         self._check(rc, want_status)
         return res
@@ -603,7 +639,7 @@ class PopulateBatcher(_Handle):
         """As PairHMMEngine.realign_reads for host blocks (phmm_batcher_realign_reads): concurrent requests with equal configs and
         flank states run as one call whatever their CIGAR strides, each with the result it gets alone at its own stride."""
         assert not haps.on_device and not reads.on_device, "the batcher takes host blocks"
-        rc, res = _realign(self._lib.phmm_batcher_realign_reads, self._h, _HOST, config, haps, reads, pairs, flank_state, cigar_stride)
+        rc, res = _realign(self._lib.phmm_batcher_realign_reads, self, _HOST, config, haps, reads, pairs, flank_state, cigar_stride)
         self._check(rc)
         return res
 
@@ -708,6 +744,7 @@ class ErrorModel(_Handle):
         total = int(off[-1])
         mf, mr = sp.empty(total, np.uint8), sp.empty(total, np.uint8)
         pf, pr, go, ge = (sp.empty(total, np.int8) for _ in range(4))
+        sp.order(engine)
         engine._check(self._lib.phmm_engine_reset_haplotypes(engine._h, self._h, len(off) - 1, sp.ptr(off), sp.ptr(seq), sp.ptr(sub),
                                                              sp.ptr(mf), sp.ptr(pf), sp.ptr(mr), sp.ptr(pr), sp.ptr(go), sp.ptr(ge), sp.flag))
         if not sp.on_device:
