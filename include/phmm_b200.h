@@ -424,6 +424,22 @@ int64_t phmm_batcher_reruns(const phmm_batcher* b);
 int phmm_genotype_likelihoods(phmm_engine* e, const double* lnl, int32_t n_haplotypes, int32_t n_reads,
                               const int32_t* genotypes, int32_t n_genotypes, int32_t ploidy, double* out, int space);
 
+/* Consumer of the matrix: SubcloneModel / SomaticSubcloneModel::evaluate's variational Bayes inference, every seed in one call
+ * (run_variational_bayes, core/models/genotype/variational_bayes_mixture_model.hpp:653-669, its save_memory = false path), in double.
+ * Sample s owns the matrix columns [sample_off[s], sample_off[s+1]) (sample_off in host memory in either space, 0 .. R, not
+ * decreasing; a sample may have no reads). genotypes[g*K + k] = haplotype of component k (repeats allowed); prior_alphas[s*K + k];
+ * genotype_log_priors[G]; seeds[i*G + g] = seed i's initial genotype log posteriors. Each seed iterates until its ELBO improves by
+ * less than epsilon, or for max_iterations. Outputs: the max-evidence seed's posteriors, log posteriors and alphas [S][K];
+ * the evidence-weighted posteriors; the max log evidence and its seed; optionally (may be null) every seed's final log
+ * evidence and iteration count. 1 <= K <= 100, G >= 1, n_seeds >= 1, S >= 1, max_iterations >= 1, H <= 50000, and every
+ * index in [0, H), else PHMM_ERR_INVALID in either space (device-space indices are checked by the kernel). */
+int phmm_variational_bayes(phmm_engine* e, const double* lnl, int32_t n_haplotypes, int32_t n_reads, const int64_t* sample_off,
+                           int32_t n_samples, const int32_t* genotypes, int32_t n_genotypes, int32_t K, const double* prior_alphas,
+                           const double* genotype_log_priors, const double* seeds, int32_t n_seeds, double epsilon,
+                           int32_t max_iterations, double* posteriors, double* log_posteriors, double* alphas,
+                           double* weighted_posteriors, double* max_log_evidence, int32_t* max_seed, double* seed_log_evidence,
+                           int32_t* seed_iterations, int space);
+
 /* ---------------------------------------------------------------------------------------------------------------------
  * HaplotypeLikelihoodModel::reset (haplotype_likelihood_model.cpp:60-78): the per-haplotype penalty arrays of phmm_haplotypes
  * from the haplotype sequences, by the reference's error models — on host threads (phmm_reset_haplotypes, no GPU needed) or on

@@ -457,6 +457,34 @@ class PairHMMEngine(_Handle):
                                                         sp.ptr(out), sp.flag))
         return out
 
+    def variational_bayes(self, lnl, genotypes, prior_alphas, genotype_log_priors, seeds, sample_off=None, epsilon=0.05,
+                          max_iterations=1000):
+        """run_variational_bayes (variational_bayes_mixture_model.hpp:653-669) of SubcloneModel::evaluate over the (H, R) matrix
+        `lnl` (numpy on the host, or a torch CUDA tensor left where populate produced it), every seed in one call (phmm_variational_bayes).
+        genotypes: (G, K) haplotype indices; prior_alphas: (S, K); genotype_log_priors: (G,); seeds: (n_seeds, G) initial log
+        posteriors; sample_off: S + 1 column offsets of the samples (default: one sample over every column). Returns a VBResult;
+        for a device matrix its arrays (and the two scalars, as 0-d tensors) stay on the device."""
+        sp = _Space(lnl.device if _is_torch(lnl) else None)
+        m, gt = sp.input(lnl, np.float64), sp.input(genotypes, np.int32)
+        pa, lp, sd = sp.input(prior_alphas, np.float64), sp.input(genotype_log_priors, np.float64), sp.input(seeds, np.float64)
+        if gt.ndim != 2 or pa.ndim != 2 or sd.ndim != 2 or m.ndim != 2:
+            raise ValueError("lnl, genotypes, prior_alphas and seeds must be 2-dimensional")
+        off = np.ascontiguousarray([0, m.shape[1]] if sample_off is None else sample_off, dtype=np.int64)
+        G, K, S = gt.shape[0], gt.shape[1], len(off) - 1
+        if pa.shape != (S, K) or lp.shape != (G,) or sd.shape[1] != G:
+            raise ValueError("prior_alphas must be (S, K), genotype_log_priors (G,) and seeds (n_seeds, G)")
+        post, lpost, wpost = sp.empty(G, np.float64), sp.empty(G, np.float64), sp.empty(G, np.float64)
+        alphas, mev, ms = sp.empty((S, K), np.float64), sp.empty((), np.float64), sp.empty((), np.int32)
+        sev, sit = sp.empty(sd.shape[0], np.float64), sp.empty(sd.shape[0], np.int32)
+        sp.order(self)
+        self._check(self._lib.phmm_variational_bayes(self._h, sp.ptr(m), m.shape[0], m.shape[1], off.ctypes.data, S, sp.ptr(gt), G, K,
+                                                     sp.ptr(pa), sp.ptr(lp), sp.ptr(sd), sd.shape[0], float(epsilon), int(max_iterations),
+                                                     sp.ptr(post), sp.ptr(lpost), sp.ptr(alphas), sp.ptr(wpost), sp.ptr(mev), sp.ptr(ms),
+                                                     sp.ptr(sev), sp.ptr(sit), sp.flag))
+        if not sp.on_device:
+            mev, ms = float(mev), int(ms)
+        return VBResult(post, lpost, alphas, mev, wpost, ms, sev, sit)
+
     # -- batch boundary ----------------------------------------------------------------------------------------
     def populate_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, flank_state=None, error_model=None):
         """HaplotypeLikelihoodArray::populate(TemplateMap): host blocks; template t = reads [template_off[t], template_off[t+1]).
@@ -790,6 +818,18 @@ class HaplotypeLikelihoodModel:
         return b
 
 
+class VBResult:
+    """VBResultPacket (variational_bayes_mixture_model.hpp:645-651) of one variational_bayes call: the max-evidence seed's
+    genotype_posteriors, genotype_log_posteriors and alphas ([S, K]), max_log_evidence, evidence_weighted_genotype_posteriors;
+    and which seed that was (max_seed), every seed's final log evidence and its number of iterations."""
+    __slots__ = ("genotype_posteriors", "genotype_log_posteriors", "alphas", "max_log_evidence",
+                 "evidence_weighted_genotype_posteriors", "max_seed", "seed_log_evidences", "seed_iterations")
+
+    def __init__(self, *values):
+        for name, v in zip(self.__slots__, values):
+            setattr(self, name, v)
+
+
 class HaplotypeLikelihoodArray:
     """likelihoods_[haplotype][sample][read or template] (haplotype_likelihood_array.hpp:34-175).
 
@@ -913,6 +953,23 @@ class HaplotypeLikelihoodArray:
             return
         assert all(a < b for a, b in zip(keep, keep[1:])) and 0 <= keep[0] and keep[-1] < self.likelihoods.shape[0]
         self.likelihoods = self.likelihoods[keep]
+
+    def variational_bayes(self, samples, genotypes, prior_alphas, genotype_log_priors, seeds, epsilon=0.05, max_iterations=1000):
+        """SubcloneModel::evaluate's inference (PairHMMEngine.variational_bayes) over these samples' columns, in the given order;
+        prior_alphas[i] belongs to samples[i]. The samples' column ranges are passed as they are when they are the array's samples
+        in its order, and gathered back to back otherwise."""
+        idx = [self._sample_index(s) for s in samples]
+        if idx == list(range(len(self._samples))):
+            lnl, off = self.likelihoods, self._off
+        else:
+            parts = [self.likelihoods[:, self._off[s]:self._off[s + 1]] for s in idx]
+            if isinstance(self.likelihoods, np.ndarray):
+                lnl = np.concatenate(parts, axis=1)
+            else:
+                import torch
+                lnl = torch.cat(parts, dim=1)
+            off = np.concatenate([[0], np.cumsum([self._off[s + 1] - self._off[s] for s in idx])])
+        return self.engine.variational_bayes(lnl, genotypes, prior_alphas, genotype_log_priors, seeds, off, epsilon, max_iterations)
 
     def merge_samples(self, samples=None, new_sample=None):
         """merge_samples (:362-409): a one-sample array holding the chosen samples' likelihoods back to back; primed."""

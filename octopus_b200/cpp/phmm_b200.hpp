@@ -24,6 +24,7 @@
 #include <new>
 #include <stdexcept>
 #include <string>
+#include <unordered_map>
 #include <utility>
 #include <vector>
 
@@ -1140,6 +1141,85 @@ private:
 // hmm::align. Those templates are the reference's own code, so this type exists only where its header has been included before
 // this one (Octopus's build; tests/cpp/test_dropin.cpp): it differs from octopus::hmm::PairHMM in the kernel member alone, a
 // GpuPairHMMDyn (runtime band).
+// SubcloneModel / SomaticSubcloneModel::evaluate's inference (run_variational_bayes, variational_bayes_mixture_model.hpp:653-669;
+// subclone_model.hpp:303) on the GPU, every seed in one phmm_variational_bayes call, in double. genotypes[g][k]: haplotype index of
+// component k (the germline haplotypes first for SomaticSubcloneModel); every genotype has the same K (1 to 100). prior_alphas holds
+// one K-vector per sample; seeds[i] is seed i's initial genotype log posteriors. The result is shaped like
+// SubcloneModelBase::InferredLatents. Throws Error for input phmm_variational_bayes refuses.
+struct VariationalBayesParameters { double epsilon = 0.05; unsigned max_iterations = 1000; };
+
+struct VBLatents
+{
+    std::vector<double> genotype_probabilities;
+    std::vector<double> genotype_log_probabilities;
+    std::unordered_map<SampleName, std::vector<double>> alphas;
+};
+
+struct InferredLatents
+{
+    VBLatents max_evidence_params;
+    std::vector<double> genotype_log_priors;
+    std::vector<double> weighted_genotype_posteriors;
+    double approx_log_evidence = 0.0;
+};
+
+inline InferredLatents run_variational_bayes(Engine& engine, const HaplotypeLikelihoodArray& likelihoods, const std::vector<SampleName>& samples,
+                                             const std::vector<std::vector<std::int32_t>>& genotypes,
+                                             const std::unordered_map<SampleName, std::vector<double>>& prior_alphas,
+                                             std::vector<double> genotype_log_priors, const VariationalBayesParameters& params,
+                                             const std::vector<std::vector<double>>& seeds)
+{
+    const std::size_t G = genotypes.size(), H = likelihoods.num_haplotypes(), S = samples.size();
+    const std::size_t K = G ? genotypes.front().size() : 0;
+    std::vector<std::int64_t> off {0};
+    for (const auto& s : samples) off.push_back(off.back() + static_cast<std::int64_t>(likelihoods.num_likelihoods(s)));
+    const auto R = static_cast<std::size_t>(off.back());
+    std::vector<double> lnl(H * R);       // the samples' columns back to back, in the given sample order
+    for (std::size_t h = 0; h < H; ++h)
+        for (std::size_t s = 0; s < S; ++s) {
+            const auto span = likelihoods(samples[s], h);
+            std::copy(span.begin(), span.end(), lnl.begin() + static_cast<std::ptrdiff_t>(h * R + static_cast<std::size_t>(off[s])));
+        }
+    std::vector<std::int32_t> gt;
+    gt.reserve(G * K);
+    for (const auto& g : genotypes) {
+        if (g.size() != K) throw Error {PHMM_ERR_INVALID, "genotypes of different sizes"};
+        gt.insert(gt.end(), g.begin(), g.end());
+    }
+    std::vector<double> pa;
+    pa.reserve(S * K);
+    for (const auto& s : samples) {
+        const auto& a = prior_alphas.at(s);
+        if (a.size() != K) throw Error {PHMM_ERR_INVALID, "prior alphas of the wrong size"};
+        pa.insert(pa.end(), a.begin(), a.end());
+    }
+    std::vector<double> sd;
+    sd.reserve(seeds.size() * G);
+    for (const auto& v : seeds) {
+        if (v.size() != G) throw Error {PHMM_ERR_INVALID, "seed of the wrong size"};
+        sd.insert(sd.end(), v.begin(), v.end());
+    }
+    if (genotype_log_priors.size() != G) throw Error {PHMM_ERR_INVALID, "genotype_log_priors of the wrong size"};
+    InferredLatents r;
+    r.max_evidence_params.genotype_probabilities.resize(G);
+    r.max_evidence_params.genotype_log_probabilities.resize(G);
+    r.weighted_genotype_posteriors.resize(G);
+    std::vector<double> alphas(S * K);
+    std::int32_t max_seed = 0;
+    engine.check(phmm_variational_bayes(engine.get(), lnl.data(), static_cast<std::int32_t>(H), static_cast<std::int32_t>(R), off.data(),
+                                        static_cast<std::int32_t>(S), gt.data(), static_cast<std::int32_t>(G), static_cast<std::int32_t>(K),
+                                        pa.data(), genotype_log_priors.data(), sd.data(), static_cast<std::int32_t>(seeds.size()), params.epsilon,
+                                        static_cast<std::int32_t>(std::min<unsigned>(params.max_iterations, 0x7fffffffu)),
+                                        r.max_evidence_params.genotype_probabilities.data(), r.max_evidence_params.genotype_log_probabilities.data(),
+                                        alphas.data(), r.weighted_genotype_posteriors.data(), &r.approx_log_evidence, &max_seed, nullptr, nullptr,
+                                        PHMM_SPACE_HOST));
+    for (std::size_t s = 0; s < S; ++s)
+        r.max_evidence_params.alphas.emplace(samples[s], std::vector<double>(alphas.begin() + static_cast<std::ptrdiff_t>(s * K),
+                                                                              alphas.begin() + static_cast<std::ptrdiff_t>((s + 1) * K)));
+    r.genotype_log_priors = std::move(genotype_log_priors);
+    return r;
+}
+
 #ifdef pair_hmm_hpp   // the include guard of the reference's src/core/models/pairhmm/pair_hmm.hpp
 template <typename Parameters, int BandSize = 0>
 class PairHMM

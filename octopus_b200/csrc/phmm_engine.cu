@@ -5,6 +5,7 @@
 #include "phmm_checks.h"
 #include "phmm_mutation.h"
 #include "phmm_kernels.cuh"
+#include "phmm_vb.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -77,6 +78,7 @@ struct phmm_engine {
     DBuf at_groups, at_off, at_lnl;                   // phmm_assign_templates: per-group template layout, template offsets, values
     DBuf mu_in, mu_list, mu_res, mu_cig, mu_out;      // phmm_mutation_prime: staged set, DP pair list, per-tile results, CIGARs, matrix
     DBuf rs_sub, rs_model, rs_words, rs_runs, rs_flags;   // phmm_engine_reset_haplotypes: flags, model tables, scratch slots, overflow
+    DBuf vb_lnl, vb_gt, vb_in, vb_idx, vb_ws, vb_seed, vb_out;   // phmm_variational_bayes: staged inputs, genotype index, workspace, results
     std::vector<cudaEvent_t> tile_events;
     std::vector<int2> info_host;
     // per-kernel launch configuration already applied / queried (the runtime calls are not free and need not be repeated)
@@ -737,6 +739,116 @@ int phmm_genotype_likelihoods(phmm_engine* e, const double* lnl, int32_t H, int3
     if (space == PHMM_SPACE_HOST) CU(cudaMemcpyAsync(out, d_out, (size_t)G * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
     if (bad) { e->err = "haplotype index out of range"; return PHMM_ERR_INVALID; }
+    return PHMM_OK;
+}
+
+// -------------------------------------------------------------------------------------------------------------
+// phmm_variational_bayes
+// -------------------------------------------------------------------------------------------------------------
+// Device memory the seeds' workspaces may take at once: blocks = min(seeds, 2 per SM, this budget / one workspace).
+static constexpr size_t kVbWorkspaceBudget = (size_t)2 << 30;
+static constexpr int kVbMaxHaplotypes = 50000;   // k_vb_index keeps one int per haplotype in shared memory
+
+int phmm_variational_bayes(phmm_engine* e, const double* lnl, int32_t H, int32_t R, const int64_t* sample_off, int32_t S,
+                           const int32_t* genotypes, int32_t G, int32_t K, const double* prior_alphas, const double* genotype_log_priors,
+                           const double* seeds, int32_t n_seeds, double epsilon, int32_t max_iterations,
+                           double* posteriors, double* log_posteriors, double* alphas, double* weighted_posteriors,
+                           double* max_log_evidence, int32_t* max_seed, double* seed_log_evidence, int32_t* seed_iterations, int space)
+{
+    using namespace phmm::vb;
+    if (int rc0 = begin_call(e)) return rc0;
+    if (K < 1 || K > kMaxK) { e->err = "K must be in [1, 100]"; return PHMM_ERR_INVALID; }
+    if (G < 1 || n_seeds < 1 || S < 1) { e->err = "no genotypes, seeds or samples"; return PHMM_ERR_INVALID; }
+    if (max_iterations < 1) { e->err = "max_iterations must be at least 1"; return PHMM_ERR_INVALID; }
+    if (H < 1 || H > kVbMaxHaplotypes || R < 0) { e->err = "bad matrix shape (1 <= H <= 50000, R >= 0)"; return PHMM_ERR_INVALID; }
+    if ((!lnl && R > 0) || !sample_off || !genotypes || !prior_alphas || !genotype_log_priors || !seeds || !posteriors || !log_posteriors ||
+        !alphas || !weighted_posteriors || !max_log_evidence || !max_seed) { e->err = "bad argument"; return PHMM_ERR_INVALID; }
+    if (sample_off[0] != 0 || sample_off[S] != R) { e->err = "sample_off must run from 0 to R"; return PHMM_ERR_INVALID; }
+    for (int s = 0; s < S; ++s) if (sample_off[s + 1] < sample_off[s]) { e->err = "sample_off decreases"; return PHMM_ERR_INVALID; }
+    if (space == PHMM_SPACE_HOST)   // the kernel checks device-space indices
+        for (long long i = 0; i < (long long)G * K; ++i) if (genotypes[i] < 0 || genotypes[i] >= H) { e->err = "haplotype index out of range"; return PHMM_ERR_INVALID; }
+
+    const long long KH = (long long)K * H, KG = (long long)K * G, SK = (long long)S * K;
+    const double *d_lnl, *d_prior, *d_lp, *d_seeds; const int32_t* d_gt;
+    int rc;
+    if ((rc = stage(e, e->vb_lnl, lnl, (size_t)H * R, space, &d_lnl))) return rc;
+    if ((rc = stage(e, e->vb_gt, genotypes, (size_t)KG, space, &d_gt))) return rc;
+    if (space == PHMM_SPACE_HOST) {
+        CU(e->vb_in.ensure((SK + G + (size_t)n_seeds * G) * sizeof(double)));
+        double* p = e->vb_in.as<double>();
+        CU(cudaMemcpyAsync(p, prior_alphas, SK * sizeof(double), cudaMemcpyHostToDevice, e->stream));
+        CU(cudaMemcpyAsync(p + SK, genotype_log_priors, G * sizeof(double), cudaMemcpyHostToDevice, e->stream));
+        CU(cudaMemcpyAsync(p + SK + G, seeds, (size_t)n_seeds * G * sizeof(double), cudaMemcpyHostToDevice, e->stream));
+        d_prior = p; d_lp = p + SK; d_seeds = p + SK + G;
+    } else {
+        d_prior = prior_alphas; d_lp = genotype_log_priors; d_seeds = seeds;
+    }
+
+    // ints: cnt, start, kh [K*H]; nk [K]; L, sid [K*G]; bad; soff [S+1]; first, modes [G]; n_modes, max_seed; map, iters [n_seeds]
+    const long long n_int = 3 * KH + K + 2 * KG + 1 + (S + 1) + 2LL * G + 2 + 2LL * n_seeds;
+    CU(e->vb_idx.ensure((size_t)n_int * sizeof(int)));
+    int* ip = e->vb_idx.as<int>();
+    int *cnt = ip, *start = cnt + KH, *kh = start + KH, *nk = kh + KH, *L = nk + K, *sid = L + KG, *bad = sid + KG, *soff = bad + 1,
+        *first = soff + S + 1, *modes = first + G, *n_modes = modes + G, *d_max_seed = n_modes + 1, *map = d_max_seed + 1, *iters = map + n_seeds;
+    std::vector<int> soff_host(sample_off, sample_off + S + 1);
+    CU(cudaMemcpyAsync(soff, soff_host.data(), (S + 1) * sizeof(int), cudaMemcpyHostToDevice, e->stream));
+    CU(cudaMemsetAsync(bad, 0, sizeof(int), e->stream));
+    CU(cudaMemsetAsync(first, 0x7f, G * sizeof(int), e->stream));   // 0x7f7f7f7f: above every seed index
+
+    // doubles: lpost [n_seeds][G]; ev [n_seeds]; alpha [n_seeds][S][K]; weights [G]; keys [G] (u64)
+    const long long n_dbl = (long long)n_seeds * G + n_seeds + n_seeds * SK + 2LL * G;
+    CU(e->vb_seed.ensure((size_t)n_dbl * sizeof(double)));
+    double* dp = e->vb_seed.as<double>();
+    double *lpost = dp, *ev = lpost + (long long)n_seeds * G, *seed_alpha = ev + n_seeds, *weights = seed_alpha + n_seeds * SK,
+           *keys = weights + G;
+    CU(cudaMemsetAsync(keys, 0, G * sizeof(double), e->stream));
+
+    const long long ws = Workspace::doubles(H, R, S, G, K);
+    const long long by_budget = std::max<long long>(1, (long long)(kVbWorkspaceBudget / sizeof(double)) / ws);
+    const int blocks = (int)std::min<long long>({(long long)n_seeds, 2LL * std::max(1, e->sm_count), by_budget});
+    CU(e->vb_ws.ensure((size_t)blocks * ws * sizeof(double)));
+
+    const size_t smem = (size_t)H * sizeof(int);
+    if (smem > 48 * 1024) CU(cudaFuncSetAttribute(k_vb_index, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_vb_index<<<K, 256, smem, e->stream>>>(d_gt, G, K, H, cnt, start, kh, nk, L, sid, bad);
+    LAUNCHED();
+    Args a{d_lnl, H, R, S, G, K, n_seeds, soff, d_gt, d_prior, d_lp, d_seeds, epsilon, max_iterations,
+           cnt, start, kh, nk, L, sid, bad, e->vb_ws.as<double>(), ws, lpost, ev, iters, map, seed_alpha};
+    k_vb_seeds<<<blocks, kThreads, 0, e->stream>>>(a);
+    LAUNCHED();
+    const unsigned seed_grid = (unsigned)((n_seeds + 255) / 256), g_grid = (unsigned)((G + 255) / 256);
+    unsigned long long* ukeys = reinterpret_cast<unsigned long long*>(keys);
+    k_vb_mode_max<<<seed_grid, 256, 0, e->stream>>>(bad, ev, map, n_seeds, ukeys);
+    k_vb_mode_first<<<seed_grid, 256, 0, e->stream>>>(bad, ev, map, n_seeds, ukeys, first);
+    k_vb_modes_compact<<<1, kFinishThreads, 0, e->stream>>>(bad, ev, n_seeds, first, G, modes, weights, n_modes, d_max_seed);
+    LAUNCHED(); LAUNCHED(); LAUNCHED();
+
+    double *o_post = posteriors, *o_lpost = log_posteriors, *o_w = weighted_posteriors, *o_alpha = alphas, *o_mev = max_log_evidence;
+    int* o_ms = max_seed;
+    if (space == PHMM_SPACE_HOST) {
+        CU(e->vb_out.ensure((3 * (size_t)G + SK + 2) * sizeof(double)));
+        o_post = e->vb_out.as<double>(); o_lpost = o_post + G; o_w = o_lpost + G; o_alpha = o_w + G; o_mev = o_alpha + SK;
+        o_ms = reinterpret_cast<int*>(o_mev + 1);
+    }
+    k_vb_weighted<<<g_grid, 256, 0, e->stream>>>(bad, lpost, G, modes, weights, n_modes, d_max_seed, o_w, o_post, o_lpost);
+    k_vb_normalise<<<1, kFinishThreads, 0, e->stream>>>(bad, G, o_w, o_post, ev, seed_alpha, (int)SK, d_max_seed, o_alpha, o_mev, o_ms);
+    LAUNCHED(); LAUNCHED();
+    CU(cudaGetLastError());
+    const cudaMemcpyKind out_kind = space == PHMM_SPACE_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    if (seed_log_evidence) CU(cudaMemcpyAsync(seed_log_evidence, ev, n_seeds * sizeof(double), out_kind, e->stream));
+    if (seed_iterations) CU(cudaMemcpyAsync(seed_iterations, iters, n_seeds * sizeof(int), out_kind, e->stream));
+    if (space == PHMM_SPACE_HOST) {
+        CU(cudaMemcpyAsync(posteriors, o_post, G * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(log_posteriors, o_lpost, G * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(weighted_posteriors, o_w, G * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(alphas, o_alpha, SK * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(max_log_evidence, o_mev, sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaMemcpyAsync(max_seed, o_ms, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+    }
+    int bad_host = 0;
+    CU(cudaMemcpyAsync(&bad_host, bad, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    if (bad_host) { e->err = "haplotype index out of range"; return PHMM_ERR_INVALID; }
     return PHMM_OK;
 }
 
