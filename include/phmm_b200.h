@@ -440,6 +440,30 @@ int phmm_variational_bayes(phmm_engine* e, const double* lnl, int32_t n_haplotyp
                            double* weighted_posteriors, double* max_log_evidence, int32_t* max_seed, double* seed_log_evidence,
                            int32_t* seed_iterations, int space);
 
+/* Consumer of the matrix: SingleCellModel::evaluate_model's mixture-of-mixtures variational Bayes inference, every seed in one
+ * call (VariationalBayesMixtureMixtureModel::evaluate, core/models/genotype/variational_bayes_mixture_mixture_model.cpp), in
+ * double. Sample s (a cell) owns the columns [sample_off[s], sample_off[s+1]) as in phmm_variational_bayes. Group t (a clone) has
+ * group_sizes[t] = K_t components (host memory in either space); its slots are j = koff_t + k, koff_t = sum_{t' < t} K_t'.
+ * combinations[c*sum K + j] = haplotype of slot j in combination c (repeats allowed); genotype_log_priors[C]; group_priors[S*T]
+ * probabilities (may be null: none), for the samples whose group_prior_mask[s] is nonzero (host memory; null: every sample);
+ * group_concentrations[T] and mixture_concentrations[S*sum K] the prior concentrations; seeds[i*C + c] seed i's initial log
+ * posteriors. Each seed iterates until its evidence improves by less than epsilon, or for max_iterations. Outputs: the
+ * max-evidence seed's posteriors, log posteriors, group concentrations [T], mixture concentrations [S*sum K] and group
+ * responsibilities [S*T]; the evidence-weighted posteriors and group responsibilities; the max log evidence and its seed;
+ * optionally (may be null) every seed's final log evidence and iteration count. 1 <= T <= 32, 1 <= K_t <= 100, sum K <= 100,
+ * C, n_seeds, S, max_iterations >= 1, H <= 50000 and every index in [0, H), else PHMM_ERR_INVALID in either space. */
+int phmm_variational_bayes_mixture_mixture(phmm_engine* e, const double* lnl, int32_t n_haplotypes, int32_t n_reads,
+                                           const int64_t* sample_off, int32_t n_samples, const int32_t* group_sizes, int32_t n_groups,
+                                           const int32_t* combinations, int32_t n_combinations, const double* genotype_log_priors,
+                                           const double* group_priors, const int32_t* group_prior_mask,
+                                           const double* group_concentrations, const double* mixture_concentrations,
+                                           const double* seeds, int32_t n_seeds, double epsilon, int32_t max_iterations,
+                                           double* posteriors, double* log_posteriors, double* group_concentrations_out,
+                                           double* mixture_concentrations_out, double* group_responsibilities,
+                                           double* weighted_posteriors, double* weighted_group_responsibilities,
+                                           double* max_log_evidence, int32_t* max_seed, double* seed_log_evidence,
+                                           int32_t* seed_iterations, int space);
+
 /* ---------------------------------------------------------------------------------------------------------------------
  * HaplotypeLikelihoodModel::reset (haplotype_likelihood_model.cpp:60-78): the per-haplotype penalty arrays of phmm_haplotypes
  * from the haplotype sequences, by the reference's error models — on host threads (phmm_reset_haplotypes, no GPU needed) or on

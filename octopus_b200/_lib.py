@@ -11,7 +11,7 @@ MUT_HMM, MUT_SELF, MUT_APPROX_LENGTH, MUT_APPROX_OFFSET, MUT_APPROX_OVERFLOW, MU
 MUT_MAX_HAPLOTYPES, MUT_MAX_LENGTH, MUT_MAX_PAIRS = 4096, 65535, 1 << 26
 
 EXPORTS = ["phmm_version", "phmm_default_config", "phmm_create", "phmm_destroy", "phmm_last_error", "phmm_launch_count",
-           "phmm_last_dp_kernel_ms", "phmm_last_dp_cells", "phmm_align_scores", "phmm_align_traceback", "phmm_align_reads", "phmm_align_pairs", "phmm_map_pairs", "phmm_realign_reads", "phmm_genotype_likelihoods", "phmm_variational_bayes", "phmm_populate", "phmm_populate_templates", "phmm_populate_regions", "phmm_assign_reads",
+           "phmm_last_dp_kernel_ms", "phmm_last_dp_cells", "phmm_align_scores", "phmm_align_traceback", "phmm_align_reads", "phmm_align_pairs", "phmm_map_pairs", "phmm_realign_reads", "phmm_genotype_likelihoods", "phmm_variational_bayes", "phmm_variational_bayes_mixture_mixture", "phmm_populate", "phmm_populate_templates", "phmm_populate_regions", "phmm_assign_reads",
            "phmm_assign_templates",
            "phmm_error_model_create", "phmm_error_model_create_custom", "phmm_error_model_destroy", "phmm_error_model_last_error",
            "phmm_reset_haplotypes", "phmm_engine_reset_haplotypes", "phmm_tandem_repeats", "phmm_mutation_model_create", "phmm_mutation_model_destroy", "phmm_mutation_context",
@@ -119,6 +119,10 @@ def load():
     lib.phmm_variational_bayes.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                            C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_double, C.c_int32] + \
                                           [C.c_void_p] * 8 + [C.c_int]
+    lib.phmm_variational_bayes_mixture_mixture.restype = C.c_int
+    lib.phmm_variational_bayes_mixture_mixture.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                                           C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p] * 6 + \
+                                                          [C.c_int32, C.c_double, C.c_int32] + [C.c_void_p] * 11 + [C.c_int]
     lib.phmm_populate.restype = C.c_int
     lib.phmm_populate.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(Haplotypes), C.POINTER(Reads),
                                   C.POINTER(Positions), C.POINTER(FlankState), C.c_void_p, C.c_void_p, C.c_int]

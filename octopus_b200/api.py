@@ -485,6 +485,64 @@ class PairHMMEngine(_Handle):
             mev, ms = float(mev), int(ms)
         return VBResult(post, lpost, alphas, mev, wpost, ms, sev, sit)
 
+    def variational_bayes_mixture_mixture(self, lnl, group_sizes, combinations, genotype_log_priors, group_concentrations,
+                                          mixture_concentrations, seeds, sample_off=None, group_priors=None, group_prior_mask=None,
+                                          epsilon=0.05, max_iterations=1000):
+        """VariationalBayesMixtureMixtureModel::evaluate (variational_bayes_mixture_mixture_model.cpp) of SingleCellModel over the
+        (H, R) matrix `lnl` (numpy on the host, or a torch CUDA tensor left where populate produced it), every seed in one call
+        (phmm_variational_bayes_mixture_mixture). group_sizes: the T groups' component counts K_t; combinations: (C, sum K_t)
+        haplotype indices, group t's components at columns [koff_t, koff_t + K_t); genotype_log_priors: (C,); seeds: (n_seeds, C)
+        initial log posteriors; sample_off: S + 1 column offsets of the samples (default: one sample over every column).
+        group_concentrations: a scalar or (T,); mixture_concentrations: a scalar, one per sample (S,), or (S, sum K_t), expanded as
+        the reference's scalar overloads expand them. group_priors: None, or (S, T) probabilities for the samples group_prior_mask
+        selects (default: all). Returns a VBMixtureMixtureResult; for a device matrix its arrays (and the two scalars, as 0-d
+        tensors) stay on the device."""
+        sp = _Space(lnl.device if _is_torch(lnl) else None)
+        sizes = np.ascontiguousarray(group_sizes, dtype=np.int32).ravel()
+        T, K = len(sizes), int(sizes.sum()) if len(sizes) else 0
+        m, gt = sp.input(lnl, np.float64), sp.input(combinations, np.int32)
+        lp, sd = sp.input(genotype_log_priors, np.float64), sp.input(seeds, np.float64)
+        if gt.ndim != 2 or sd.ndim != 2 or m.ndim != 2:
+            raise ValueError("lnl, combinations and seeds must be 2-dimensional")
+        off = np.ascontiguousarray([0, m.shape[1]] if sample_off is None else sample_off, dtype=np.int64)
+        Cn, S = gt.shape[0], len(off) - 1
+        if gt.shape[1] != K or lp.shape != (Cn,) or sd.shape[1] != Cn:
+            raise ValueError("combinations must be (C, sum of group_sizes), genotype_log_priors (C,) and seeds (n_seeds, C)")
+        ndim = lambda v: v.dim() if _is_torch(v) else np.ndim(v)
+        scalar_gc, per_sample_mc = ndim(group_concentrations) == 0, ndim(mixture_concentrations) < 2
+        gc, mc = sp.input(group_concentrations, np.float64), sp.input(mixture_concentrations, np.float64)
+        if scalar_gc:                    # one concentration for every group
+            gc = gc.reshape(1).expand(T).contiguous() if sp.on_device else np.full(T, float(gc.ravel()[0]))
+        if per_sample_mc:                # one concentration, or one per sample, for every component
+            mc = mc.reshape(-1, 1).expand(S, K).contiguous() if sp.on_device else \
+                np.repeat(np.broadcast_to(mc.ravel(), (S,))[:, None], K, axis=1)
+        sp.enqueued |= sp.on_device and (scalar_gc or per_sample_mc)     # the expansion ran on torch's current stream
+        if gc.shape != (T,) or mc.shape != (S, K):
+            raise ValueError("group_concentrations must be (T,) and mixture_concentrations (S, sum of group_sizes)")
+        gp, mask = None, None
+        if group_priors is not None:
+            gp = sp.input(group_priors, np.float64)
+            if gp.shape != (S, T):
+                raise ValueError("group_priors must be (S, T)")
+            if group_prior_mask is not None:
+                mask = np.ascontiguousarray(group_prior_mask, dtype=np.int32)
+                if mask.shape != (S,):
+                    raise ValueError("group_prior_mask must be (S,)")
+        post, lpost, wpost = sp.empty(Cn, np.float64), sp.empty(Cn, np.float64), sp.empty(Cn, np.float64)
+        gco, mco = sp.empty(T, np.float64), sp.empty((S, K), np.float64)
+        sigma, wsigma = sp.empty((S, T), np.float64), sp.empty((S, T), np.float64)
+        mev, ms = sp.empty((), np.float64), sp.empty((), np.int32)
+        sev, sit = sp.empty(sd.shape[0], np.float64), sp.empty(sd.shape[0], np.int32)
+        sp.order(self)
+        self._check(self._lib.phmm_variational_bayes_mixture_mixture(
+            self._h, sp.ptr(m), m.shape[0], m.shape[1], off.ctypes.data, S, sizes.ctypes.data, T, sp.ptr(gt), Cn, sp.ptr(lp),
+            sp.ptr(gp), None if mask is None else mask.ctypes.data, sp.ptr(gc), sp.ptr(mc), sp.ptr(sd), sd.shape[0], float(epsilon),
+            int(max_iterations), sp.ptr(post), sp.ptr(lpost), sp.ptr(gco), sp.ptr(mco), sp.ptr(sigma), sp.ptr(wpost), sp.ptr(wsigma),
+            sp.ptr(mev), sp.ptr(ms), sp.ptr(sev), sp.ptr(sit), sp.flag))
+        if not sp.on_device:
+            mev, ms = float(mev), int(ms)
+        return VBMixtureMixtureResult(post, lpost, gco, mco, sigma, mev, wpost, wsigma, ms, sev, sit)
+
     # -- batch boundary ----------------------------------------------------------------------------------------
     def populate_templates(self, config, haps: HaplotypeBlock, reads: ReadBlock, template_off, flank_state=None, error_model=None):
         """HaplotypeLikelihoodArray::populate(TemplateMap): host blocks; template t = reads [template_off[t], template_off[t+1]).
@@ -830,6 +888,21 @@ class VBResult:
             setattr(self, name, v)
 
 
+class VBMixtureMixtureResult:
+    """VariationalBayesMixtureMixtureModel::Inferences (variational_bayes_mixture_mixture_model.hpp:72-77) of one
+    variational_bayes_mixture_mixture call, without the component responsibilities: the max-evidence seed's genotype_posteriors,
+    genotype_log_posteriors, group_concentrations [T], mixture_concentrations [S, sum K_t] and group_responsibilities [S, T],
+    its approx_log_evidence (max_log_evidence); the weighted_genotype_posteriors and weighted_group_responsibilities; and which
+    seed that was (max_seed), every seed's final log evidence and its number of iterations."""
+    __slots__ = ("genotype_posteriors", "genotype_log_posteriors", "group_concentrations", "mixture_concentrations",
+                 "group_responsibilities", "max_log_evidence", "weighted_genotype_posteriors", "weighted_group_responsibilities",
+                 "max_seed", "seed_log_evidences", "seed_iterations")
+
+    def __init__(self, *values):
+        for name, v in zip(self.__slots__, values):
+            setattr(self, name, v)
+
+
 class HaplotypeLikelihoodArray:
     """likelihoods_[haplotype][sample][read or template] (haplotype_likelihood_array.hpp:34-175).
 
@@ -954,22 +1027,36 @@ class HaplotypeLikelihoodArray:
         assert all(a < b for a, b in zip(keep, keep[1:])) and 0 <= keep[0] and keep[-1] < self.likelihoods.shape[0]
         self.likelihoods = self.likelihoods[keep]
 
+    def _columns(self, samples):
+        """The matrix and column offsets of these samples in the given order: the array's own when they are its samples in its
+        order, and gathered back to back otherwise."""
+        idx = [self._sample_index(s) for s in samples]
+        if idx == list(range(len(self._samples))):
+            return self.likelihoods, self._off
+        parts = [self.likelihoods[:, self._off[s]:self._off[s + 1]] for s in idx]
+        if isinstance(self.likelihoods, np.ndarray):
+            lnl = np.concatenate(parts, axis=1)
+        else:
+            import torch
+            lnl = torch.cat(parts, dim=1)
+        return lnl, np.concatenate([[0], np.cumsum([self._off[s + 1] - self._off[s] for s in idx])])
+
     def variational_bayes(self, samples, genotypes, prior_alphas, genotype_log_priors, seeds, epsilon=0.05, max_iterations=1000):
         """SubcloneModel::evaluate's inference (PairHMMEngine.variational_bayes) over these samples' columns, in the given order;
         prior_alphas[i] belongs to samples[i]. The samples' column ranges are passed as they are when they are the array's samples
         in its order, and gathered back to back otherwise."""
-        idx = [self._sample_index(s) for s in samples]
-        if idx == list(range(len(self._samples))):
-            lnl, off = self.likelihoods, self._off
-        else:
-            parts = [self.likelihoods[:, self._off[s]:self._off[s + 1]] for s in idx]
-            if isinstance(self.likelihoods, np.ndarray):
-                lnl = np.concatenate(parts, axis=1)
-            else:
-                import torch
-                lnl = torch.cat(parts, dim=1)
-            off = np.concatenate([[0], np.cumsum([self._off[s + 1] - self._off[s] for s in idx])])
+        lnl, off = self._columns(samples)
         return self.engine.variational_bayes(lnl, genotypes, prior_alphas, genotype_log_priors, seeds, off, epsilon, max_iterations)
+
+    def variational_bayes_mixture_mixture(self, samples, group_sizes, combinations, genotype_log_priors, group_concentrations,
+                                          mixture_concentrations, seeds, group_priors=None, group_prior_mask=None, epsilon=0.05,
+                                          max_iterations=1000):
+        """SingleCellModel's inference (PairHMMEngine.variational_bayes_mixture_mixture) over these samples' columns, in the given
+        order; row i of the per-sample inputs belongs to samples[i]."""
+        lnl, off = self._columns(samples)
+        return self.engine.variational_bayes_mixture_mixture(lnl, group_sizes, combinations, genotype_log_priors, group_concentrations,
+                                                             mixture_concentrations, seeds, off, group_priors, group_prior_mask,
+                                                             epsilon, max_iterations)
 
     def merge_samples(self, samples=None, new_sample=None):
         """merge_samples (:362-409): a one-sample array holding the chosen samples' likelihoods back to back; primed."""

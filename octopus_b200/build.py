@@ -8,7 +8,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB = os.path.join(_HERE, "libphmm_b200.so")
 SOURCES = ["phmm_engine.cu", "phmm_error_model.cpp", "phmm_batcher.cpp", "phmm_batcher_reset.cpp", "phmm_batcher_align.cpp",
            "phmm_batcher_templates.cpp"]
-DEPS = ["phmm_engine.cu", "phmm_kernels.cuh", "phmm_device.cuh", "phmm_checks.h", "phmm_mutation.h", "phmm_reset.cuh", "phmm_vb.cuh", "phmm_error_model.cpp", "phmm_error_model_tables.inc",
+DEPS = ["phmm_engine.cu", "phmm_kernels.cuh", "phmm_device.cuh", "phmm_checks.h", "phmm_mutation.h", "phmm_reset.cuh", "phmm_vb.cuh", "phmm_vb_mm.cuh", "phmm_error_model.cpp", "phmm_error_model_tables.inc",
         "phmm_batcher.cpp", "phmm_batcher_reset.cpp", "phmm_batcher_align.cpp", "phmm_batcher_templates.cpp", "phmm_batcher_seam.h", os.path.join("..", "..", "include", "phmm_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]
@@ -59,6 +59,18 @@ def build_vb_emulation(force=False):
     src = os.path.join(root, "tests", "cpu_emul", "vb_emul.cu")
     out = os.path.join(root, "tests", "cpu_emul", "libvb_emul.so")
     if not force and not _stale(out, [src, os.path.join(CSRC, "phmm_vb.cuh"), __file__]):
+        return out
+    subprocess.run([_nvcc(), "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
+                    "-shared", "-o", out, src], check=True)
+    return out
+
+
+def build_vbmm_emulation(force=False):
+    """tests/cpu_emul/libvbmm_emul.so: the mixture-of-mixtures VB loop over the engine's __host__ __device__ arithmetic (test helper)."""
+    root = os.path.dirname(_HERE)
+    src = os.path.join(root, "tests", "cpu_emul", "vbmm_emul.cu")
+    out = os.path.join(root, "tests", "cpu_emul", "libvbmm_emul.so")
+    if not force and not _stale(out, [src, os.path.join(CSRC, "phmm_vb_mm.cuh"), os.path.join(CSRC, "phmm_vb.cuh"), __file__]):
         return out
     subprocess.run([_nvcc(), "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
                     "-shared", "-o", out, src], check=True)

@@ -1163,6 +1163,27 @@ struct InferredLatents
     double approx_log_evidence = 0.0;
 };
 
+namespace detail {
+
+// The samples' columns of the matrix back to back, in the given sample order ([H][R]); off receives the S + 1 column offsets.
+inline std::vector<double> sample_columns(const HaplotypeLikelihoodArray& likelihoods, const std::vector<SampleName>& samples,
+                                          std::vector<std::int64_t>& off)
+{
+    const std::size_t H = likelihoods.num_haplotypes(), S = samples.size();
+    off.assign(1, 0);
+    for (const auto& s : samples) off.push_back(off.back() + static_cast<std::int64_t>(likelihoods.num_likelihoods(s)));
+    const auto R = static_cast<std::size_t>(off.back());
+    std::vector<double> lnl(H * R);
+    for (std::size_t h = 0; h < H; ++h)
+        for (std::size_t s = 0; s < S; ++s) {
+            const auto span = likelihoods(samples[s], h);
+            std::copy(span.begin(), span.end(), lnl.begin() + static_cast<std::ptrdiff_t>(h * R + static_cast<std::size_t>(off[s])));
+        }
+    return lnl;
+}
+
+} // namespace detail
+
 inline InferredLatents run_variational_bayes(Engine& engine, const HaplotypeLikelihoodArray& likelihoods, const std::vector<SampleName>& samples,
                                              const std::vector<std::vector<std::int32_t>>& genotypes,
                                              const std::unordered_map<SampleName, std::vector<double>>& prior_alphas,
@@ -1171,15 +1192,9 @@ inline InferredLatents run_variational_bayes(Engine& engine, const HaplotypeLike
 {
     const std::size_t G = genotypes.size(), H = likelihoods.num_haplotypes(), S = samples.size();
     const std::size_t K = G ? genotypes.front().size() : 0;
-    std::vector<std::int64_t> off {0};
-    for (const auto& s : samples) off.push_back(off.back() + static_cast<std::int64_t>(likelihoods.num_likelihoods(s)));
+    std::vector<std::int64_t> off;
+    const auto lnl = detail::sample_columns(likelihoods, samples, off);
     const auto R = static_cast<std::size_t>(off.back());
-    std::vector<double> lnl(H * R);       // the samples' columns back to back, in the given sample order
-    for (std::size_t h = 0; h < H; ++h)
-        for (std::size_t s = 0; s < S; ++s) {
-            const auto span = likelihoods(samples[s], h);
-            std::copy(span.begin(), span.end(), lnl.begin() + static_cast<std::ptrdiff_t>(h * R + static_cast<std::size_t>(off[s])));
-        }
     std::vector<std::int32_t> gt;
     gt.reserve(G * K);
     for (const auto& g : genotypes) {
@@ -1219,6 +1234,199 @@ inline InferredLatents run_variational_bayes(Engine& engine, const HaplotypeLike
     r.genotype_log_priors = std::move(genotype_log_priors);
     return r;
 }
+
+// SingleCellModel::evaluate_model's inference (VariationalBayesMixtureMixtureModel::evaluate,
+// variational_bayes_mixture_mixture_model.hpp:89-132) on the GPU, every seed in one phmm_variational_bayes_mixture_mixture call, in
+// double. Where the reference takes a HaplotypeLikelihoodMatrix, the overloads take what make_likelihood_matrix
+// (single_cell_model.cpp:824-851) reads: the likelihood array and its samples (the cells, in order), the genotypes as
+// haplotype-index vectors, and the combinations as one genotype index per group. Every combination's genotype of group t has
+// the same ploidy K_t (1 to 100, sum at most 100, at most 32 groups). The scalar overloads expand their concentrations as the
+// reference's do (:61-126). A sample's group priors are its entry of GroupOptionalPriorArray; an empty vector means none (the
+// reference's boost::none). The result is shaped like the reference's Inferences, without the component responsibilities, which
+// no caller reads. Throws Error for input phmm_variational_bayes_mixture_mixture refuses.
+class VariationalBayesMixtureMixtureModel
+{
+public:
+    struct Options { double epsilon = 0.05; unsigned max_iterations = 1000; };
+
+    using ProbabilityVector = std::vector<double>;
+    using LogProbabilityVector = std::vector<double>;
+    using GroupConcentrationVector = std::vector<double>;                      // one per group
+    using ComponentConcentrationVector = std::vector<double>;                  // one per component of the group
+    using MixtureConcentrationVector = std::vector<ComponentConcentrationVector>;   // one per group
+    using MixtureConcentrationArray = std::vector<MixtureConcentrationVector>;      // one per sample
+    using Sigma = std::vector<double>;                                         // one per group
+    using GroupResponsibilityVector = std::vector<Sigma>;                      // one per sample
+    using GroupOptionalPriorArray = std::vector<ProbabilityVector>;            // one per sample; empty: no priors
+    using GenotypeVector = std::vector<std::vector<std::int32_t>>;              // haplotype indices of each genotype
+    using GenotypeCombinationVector = std::vector<std::vector<std::size_t>>;    // a genotype index per group
+
+    struct Latents
+    {
+        ProbabilityVector genotype_posteriors;
+        LogProbabilityVector genotype_log_posteriors;
+        GroupConcentrationVector group_concentrations;
+        MixtureConcentrationArray mixture_concentrations;
+        GroupResponsibilityVector group_responsibilities;
+    };
+    struct PointInferences { Latents latents; double approx_log_evidence = 0.0; };
+    struct Inferences
+    {
+        PointInferences map;
+        ProbabilityVector weighted_genotype_posteriors;
+        GroupResponsibilityVector weighted_group_responsibilities;
+    };
+
+    VariationalBayesMixtureMixtureModel(Options options, Engine& engine) : options_ {options}, engine_ {&engine} {}
+
+    Inferences evaluate(const LogProbabilityVector& genotype_log_priors, const HaplotypeLikelihoodArray& likelihoods,
+                        const std::vector<SampleName>& samples, const GenotypeVector& genotypes,
+                        const GenotypeCombinationVector& genotype_combinations, const GroupOptionalPriorArray& group_priors,
+                        const GroupConcentrationVector& group_concentrations, const MixtureConcentrationArray& mixture_concentrations,
+                        const std::vector<LogProbabilityVector>& seeds) const
+    {
+        return run(genotype_log_priors, likelihoods, samples, genotypes, genotype_combinations, group_priors, group_concentrations,
+                   mixture_concentrations, seeds);
+    }
+    Inferences evaluate(const LogProbabilityVector& genotype_log_priors, const HaplotypeLikelihoodArray& likelihoods,
+                        const std::vector<SampleName>& samples, const GenotypeVector& genotypes,
+                        const GenotypeCombinationVector& genotype_combinations, const GroupConcentrationVector& group_concentrations,
+                        const MixtureConcentrationArray& mixture_concentrations, const std::vector<LogProbabilityVector>& seeds) const
+    {
+        return run(genotype_log_priors, likelihoods, samples, genotypes, genotype_combinations, GroupOptionalPriorArray(samples.size()),
+                   group_concentrations, mixture_concentrations, seeds);
+    }
+    Inferences evaluate(const LogProbabilityVector& genotype_log_priors, const HaplotypeLikelihoodArray& likelihoods,
+                        const std::vector<SampleName>& samples, const GenotypeVector& genotypes,
+                        const GenotypeCombinationVector& genotype_combinations, const GroupOptionalPriorArray& group_priors,
+                        double group_concentration, const std::vector<double>& mixture_concentrations,
+                        const std::vector<LogProbabilityVector>& seeds) const
+    {
+        const auto sizes = group_sizes(genotypes, genotype_combinations);
+        if (mixture_concentrations.size() != samples.size()) throw Error {PHMM_ERR_INVALID, "one mixture concentration per sample"};
+        MixtureConcentrationArray m;
+        for (double c : mixture_concentrations) m.push_back(expand(sizes, c));
+        return run(genotype_log_priors, likelihoods, samples, genotypes, genotype_combinations, group_priors,
+                   GroupConcentrationVector(sizes.size(), group_concentration), m, seeds);
+    }
+    Inferences evaluate(const LogProbabilityVector& genotype_log_priors, const HaplotypeLikelihoodArray& likelihoods,
+                        const std::vector<SampleName>& samples, const GenotypeVector& genotypes,
+                        const GenotypeCombinationVector& genotype_combinations, double group_concentration,
+                        const std::vector<double>& mixture_concentrations, const std::vector<LogProbabilityVector>& seeds) const
+    {
+        return evaluate(genotype_log_priors, likelihoods, samples, genotypes, genotype_combinations, GroupOptionalPriorArray(samples.size()),
+                        group_concentration, mixture_concentrations, seeds);
+    }
+    Inferences evaluate(const LogProbabilityVector& genotype_log_priors, const HaplotypeLikelihoodArray& likelihoods,
+                        const std::vector<SampleName>& samples, const GenotypeVector& genotypes,
+                        const GenotypeCombinationVector& genotype_combinations, const GroupOptionalPriorArray& group_priors,
+                        double group_concentration, double mixture_concentration, const std::vector<LogProbabilityVector>& seeds) const
+    {
+        const auto sizes = group_sizes(genotypes, genotype_combinations);
+        return run(genotype_log_priors, likelihoods, samples, genotypes, genotype_combinations, group_priors,
+                   GroupConcentrationVector(sizes.size(), group_concentration),
+                   MixtureConcentrationArray(samples.size(), expand(sizes, mixture_concentration)), seeds);
+    }
+    Inferences evaluate(const LogProbabilityVector& genotype_log_priors, const HaplotypeLikelihoodArray& likelihoods,
+                        const std::vector<SampleName>& samples, const GenotypeVector& genotypes,
+                        const GenotypeCombinationVector& genotype_combinations, double group_concentration, double mixture_concentration,
+                        const std::vector<LogProbabilityVector>& seeds) const
+    {
+        return evaluate(genotype_log_priors, likelihoods, samples, genotypes, genotype_combinations, GroupOptionalPriorArray(samples.size()),
+                        group_concentration, mixture_concentration, seeds);
+    }
+
+private:
+    Options options_;
+    Engine* engine_;
+
+    // K_t: the ploidy of group t's genotype, the same in every combination.
+    static std::vector<std::int32_t> group_sizes(const GenotypeVector& genotypes, const GenotypeCombinationVector& combinations)
+    {
+        if (combinations.empty()) throw Error {PHMM_ERR_INVALID, "no genotype combinations"};
+        std::vector<std::int32_t> sizes;
+        for (const auto g : combinations.front()) sizes.push_back(static_cast<std::int32_t>(genotypes.at(g).size()));
+        for (const auto& c : combinations) {
+            if (c.size() != sizes.size()) throw Error {PHMM_ERR_INVALID, "combinations of different group counts"};
+            for (std::size_t t = 0; t < c.size(); ++t)
+                if (genotypes.at(c[t]).size() != static_cast<std::size_t>(sizes[t])) throw Error {PHMM_ERR_INVALID, "a group's genotypes differ in ploidy"};
+        }
+        return sizes;
+    }
+    static MixtureConcentrationVector expand(const std::vector<std::int32_t>& sizes, double c)
+    {
+        MixtureConcentrationVector r;
+        for (const auto k : sizes) r.emplace_back(static_cast<std::size_t>(k), c);
+        return r;
+    }
+
+    Inferences run(const LogProbabilityVector& genotype_log_priors, const HaplotypeLikelihoodArray& likelihoods,
+                   const std::vector<SampleName>& samples, const GenotypeVector& genotypes,
+                   const GenotypeCombinationVector& genotype_combinations, const GroupOptionalPriorArray& group_priors,
+                   const GroupConcentrationVector& group_concentrations, const MixtureConcentrationArray& mixture_concentrations,
+                   const std::vector<LogProbabilityVector>& seeds) const
+    {
+        const auto sizes = group_sizes(genotypes, genotype_combinations);
+        const std::size_t C = genotype_combinations.size(), S = samples.size(), T = sizes.size(), H = likelihoods.num_haplotypes();
+        std::size_t K = 0;
+        for (const auto k : sizes) K += static_cast<std::size_t>(k);
+        std::vector<std::int64_t> off;
+        const auto lnl = detail::sample_columns(likelihoods, samples, off);
+        std::vector<std::int32_t> gt;
+        gt.reserve(C * K);
+        for (const auto& c : genotype_combinations)
+            for (const auto g : c) gt.insert(gt.end(), genotypes[g].begin(), genotypes[g].end());
+        if (genotype_log_priors.size() != C) throw Error {PHMM_ERR_INVALID, "genotype_log_priors of the wrong size"};
+        if (group_concentrations.size() != T) throw Error {PHMM_ERR_INVALID, "group concentrations of the wrong size"};
+        if (group_priors.size() != S || mixture_concentrations.size() != S) throw Error {PHMM_ERR_INVALID, "one entry per sample expected"};
+        std::vector<double> mc, gp(S * T, 0.0);
+        std::vector<std::int32_t> mask(S, 0);
+        bool any_prior = false;
+        for (std::size_t s = 0; s < S; ++s) {
+            if (mixture_concentrations[s].size() != T) throw Error {PHMM_ERR_INVALID, "mixture concentrations of the wrong shape"};
+            for (std::size_t t = 0; t < T; ++t) {
+                if (mixture_concentrations[s][t].size() != static_cast<std::size_t>(sizes[t])) throw Error {PHMM_ERR_INVALID, "mixture concentrations of the wrong shape"};
+                mc.insert(mc.end(), mixture_concentrations[s][t].begin(), mixture_concentrations[s][t].end());
+            }
+            if (!group_priors[s].empty()) {
+                if (group_priors[s].size() != T) throw Error {PHMM_ERR_INVALID, "group priors of the wrong size"};
+                std::copy(group_priors[s].begin(), group_priors[s].end(), gp.begin() + static_cast<std::ptrdiff_t>(s * T));
+                mask[s] = 1;
+                any_prior = true;
+            }
+        }
+        std::vector<double> sd;
+        sd.reserve(seeds.size() * C);
+        for (const auto& v : seeds) {
+            if (v.size() != C) throw Error {PHMM_ERR_INVALID, "seed of the wrong size"};
+            sd.insert(sd.end(), v.begin(), v.end());
+        }
+        Inferences r;
+        auto& L = r.map.latents;
+        L.genotype_posteriors.resize(C);
+        L.genotype_log_posteriors.resize(C);
+        L.group_concentrations.resize(T);
+        r.weighted_genotype_posteriors.resize(C);
+        std::vector<double> mco(S * K), sigma(S * T), wsigma(S * T);
+        std::int32_t max_seed = 0;
+        engine_->check(phmm_variational_bayes_mixture_mixture(
+            engine_->get(), lnl.data(), static_cast<std::int32_t>(H), static_cast<std::int32_t>(off.back()), off.data(),
+            static_cast<std::int32_t>(S), sizes.data(), static_cast<std::int32_t>(T), gt.data(), static_cast<std::int32_t>(C),
+            genotype_log_priors.data(), any_prior ? gp.data() : nullptr, mask.data(), group_concentrations.data(), mc.data(), sd.data(),
+            static_cast<std::int32_t>(seeds.size()), options_.epsilon, static_cast<std::int32_t>(std::min<unsigned>(options_.max_iterations, 0x7fffffffu)),
+            L.genotype_posteriors.data(), L.genotype_log_posteriors.data(), L.group_concentrations.data(), mco.data(), sigma.data(),
+            r.weighted_genotype_posteriors.data(), wsigma.data(), &r.map.approx_log_evidence, &max_seed, nullptr, nullptr, PHMM_SPACE_HOST));
+        for (std::size_t s = 0; s < S; ++s) {
+            L.mixture_concentrations.emplace_back();
+            for (std::size_t t = 0, o = s * K; t < T; o += static_cast<std::size_t>(sizes[t]), ++t)
+                L.mixture_concentrations.back().emplace_back(mco.begin() + static_cast<std::ptrdiff_t>(o),
+                                                             mco.begin() + static_cast<std::ptrdiff_t>(o + static_cast<std::size_t>(sizes[t])));
+            L.group_responsibilities.emplace_back(sigma.begin() + static_cast<std::ptrdiff_t>(s * T), sigma.begin() + static_cast<std::ptrdiff_t>((s + 1) * T));
+            r.weighted_group_responsibilities.emplace_back(wsigma.begin() + static_cast<std::ptrdiff_t>(s * T), wsigma.begin() + static_cast<std::ptrdiff_t>((s + 1) * T));
+        }
+        return r;
+    }
+};
 
 #ifdef pair_hmm_hpp   // the include guard of the reference's src/core/models/pairhmm/pair_hmm.hpp
 template <typename Parameters, int BandSize = 0>

@@ -6,6 +6,7 @@
 #include "phmm_mutation.h"
 #include "phmm_kernels.cuh"
 #include "phmm_vb.cuh"
+#include "phmm_vb_mm.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -79,6 +80,7 @@ struct phmm_engine {
     DBuf mu_in, mu_list, mu_res, mu_cig, mu_out;      // phmm_mutation_prime: staged set, DP pair list, per-tile results, CIGARs, matrix
     DBuf rs_sub, rs_model, rs_words, rs_runs, rs_flags;   // phmm_engine_reset_haplotypes: flags, model tables, scratch slots, overflow
     DBuf vb_lnl, vb_gt, vb_in, vb_idx, vb_ws, vb_seed, vb_out;   // phmm_variational_bayes: staged inputs, genotype index, workspace, results
+    DBuf mm_lnl, mm_gt, mm_in, mm_idx, mm_pairs, mm_ws, mm_seed, mm_out;   // phmm_variational_bayes_mixture_mixture: the same, and the slot pairs
     std::vector<cudaEvent_t> tile_events;
     std::vector<int2> info_host;
     // per-kernel launch configuration already applied / queried (the runtime calls are not free and need not be repeated)
@@ -849,6 +851,174 @@ int phmm_variational_bayes(phmm_engine* e, const double* lnl, int32_t H, int32_t
     CU(cudaMemcpyAsync(&bad_host, bad, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
     if (bad_host) { e->err = "haplotype index out of range"; return PHMM_ERR_INVALID; }
+    return PHMM_OK;
+}
+
+// -------------------------------------------------------------------------------------------------------------
+// phmm_variational_bayes_mixture_mixture
+// -------------------------------------------------------------------------------------------------------------
+int phmm_variational_bayes_mixture_mixture(phmm_engine* e, const double* lnl, int32_t H, int32_t R, const int64_t* sample_off, int32_t S,
+                                           const int32_t* group_sizes, int32_t T, const int32_t* combinations, int32_t C,
+                                           const double* genotype_log_priors, const double* group_priors, const int32_t* group_prior_mask,
+                                           const double* group_concentrations, const double* mixture_concentrations, const double* seeds,
+                                           int32_t n_seeds, double epsilon, int32_t max_iterations, double* posteriors,
+                                           double* log_posteriors, double* group_concentrations_out, double* mixture_concentrations_out,
+                                           double* group_responsibilities, double* weighted_posteriors,
+                                           double* weighted_group_responsibilities, double* max_log_evidence, int32_t* max_seed,
+                                           double* seed_log_evidence, int32_t* seed_iterations, int space)
+{
+    using namespace phmm::vbmm;
+    if (int rc0 = begin_call(e)) return rc0;
+    if (T < 1 || T > kMaxGroups || !group_sizes) { e->err = "the number of groups must be in [1, 32]"; return PHMM_ERR_INVALID; }
+    int K = 0, maxK = 0;
+    std::vector<int> koff_host(T + 1, 0), slot_host;
+    for (int t = 0; t < T; ++t) {
+        if (group_sizes[t] < 1 || group_sizes[t] > kMaxSlots) { e->err = "group sizes must be in [1, 100]"; return PHMM_ERR_INVALID; }
+        koff_host[t] = K;
+        K += group_sizes[t];
+        maxK = std::max(maxK, (int)group_sizes[t]);
+        if (K > kMaxSlots) { e->err = "the group sizes must sum to at most 100"; return PHMM_ERR_INVALID; }
+        slot_host.insert(slot_host.end(), group_sizes[t], t);
+    }
+    koff_host[T] = K;
+    if (C < 1 || n_seeds < 1 || S < 1) { e->err = "no combinations, seeds or samples"; return PHMM_ERR_INVALID; }
+    if (max_iterations < 1) { e->err = "max_iterations must be at least 1"; return PHMM_ERR_INVALID; }
+    if (H < 1 || H > kVbMaxHaplotypes || R < 0) { e->err = "bad matrix shape (1 <= H <= 50000, R >= 0)"; return PHMM_ERR_INVALID; }
+    if ((!lnl && R > 0) || !sample_off || !combinations || !genotype_log_priors || !group_concentrations || !mixture_concentrations ||
+        !seeds || !posteriors || !log_posteriors || !group_concentrations_out || !mixture_concentrations_out || !group_responsibilities ||
+        !weighted_posteriors || !weighted_group_responsibilities || !max_log_evidence || !max_seed) { e->err = "bad argument"; return PHMM_ERR_INVALID; }
+    if (sample_off[0] != 0 || sample_off[S] != R) { e->err = "sample_off must run from 0 to R"; return PHMM_ERR_INVALID; }
+    for (int s = 0; s < S; ++s) if (sample_off[s + 1] < sample_off[s]) { e->err = "sample_off decreases"; return PHMM_ERR_INVALID; }
+    if (space == PHMM_SPACE_HOST)   // the kernel checks device-space indices
+        for (long long i = 0; i < (long long)C * K; ++i) if (combinations[i] < 0 || combinations[i] >= H) { e->err = "haplotype index out of range"; return PHMM_ERR_INVALID; }
+
+    // the reads' samples and the per-sample chunks of at most kChunk reads
+    std::vector<int> rsamp_host(R), chunk_s, chunk_n0, schunk_host(S + 1), has_prior_host(S, group_priors ? 1 : 0);
+    for (int s = 0; s < S; ++s) {
+        schunk_host[s] = (int)chunk_s.size();
+        for (int64_t n = sample_off[s]; n < sample_off[s + 1]; ++n) rsamp_host[n] = s;
+        for (int64_t n = sample_off[s]; n < sample_off[s + 1]; n += kChunk) { chunk_s.push_back(s); chunk_n0.push_back((int)n); }
+        if (group_priors && group_prior_mask) has_prior_host[s] = group_prior_mask[s] != 0;
+    }
+    schunk_host[S] = (int)chunk_s.size();
+    const int NC = (int)chunk_s.size();
+
+    const long long KH = (long long)K * H, KC = (long long)K * C, SK = (long long)S * K, ST = (long long)S * T;
+    const double *d_lnl, *d_lp, *d_seeds, *d_gprior = nullptr, *d_gc0, *d_mc0; const int32_t* d_gt;
+    int rc;
+    if ((rc = stage(e, e->mm_lnl, lnl, (size_t)H * R, space, &d_lnl))) return rc;
+    if ((rc = stage(e, e->mm_gt, combinations, (size_t)KC, space, &d_gt))) return rc;
+    if (space == PHMM_SPACE_HOST) {
+        const size_t n_in = C + (size_t)n_seeds * C + (group_priors ? ST : 0) + T + SK;
+        CU(e->mm_in.ensure(n_in * sizeof(double)));
+        double* p = e->mm_in.as<double>();
+        auto put = [&](const double* src, size_t n, const double** dst) -> cudaError_t {
+            *dst = p;
+            cudaError_t r = cudaMemcpyAsync(p, src, n * sizeof(double), cudaMemcpyHostToDevice, e->stream);
+            p += n;
+            return r;
+        };
+        CU(put(genotype_log_priors, C, &d_lp));
+        CU(put(seeds, (size_t)n_seeds * C, &d_seeds));
+        if (group_priors) CU(put(group_priors, ST, &d_gprior));
+        CU(put(group_concentrations, T, &d_gc0));
+        CU(put(mixture_concentrations, SK, &d_mc0));
+    } else {
+        d_lp = genotype_log_priors; d_seeds = seeds; d_gprior = group_priors; d_gc0 = group_concentrations; d_mc0 = mixture_concentrations;
+    }
+
+    // ints: cnt, start, kh [K*H]; nk [K]; L, sid [K*C]; bad; soff [S+1]; rsamp [R]; gsz [T]; koff [T+1]; slot_t [K]; has_prior [S];
+    // chunk_s, chunk_n0 [NC]; schunk [S+1]; pofs [K+1]; first, modes [C]; n_modes, max_seed; map, iters [n_seeds]
+    const long long n_int = 3 * KH + K + 2 * KC + 1 + (S + 1) + R + T + (T + 1) + K + S + 2LL * NC + (S + 1) + (K + 1) + 2LL * C + 2 + 2LL * n_seeds;
+    CU(e->mm_idx.ensure((size_t)n_int * sizeof(int)));
+    int* ip = e->mm_idx.as<int>();
+    int *cnt = ip, *start = cnt + KH, *kh = start + KH, *nk = kh + KH, *L = nk + K, *sid = L + KC, *bad = sid + KC, *soff = bad + 1,
+        *rsamp = soff + S + 1, *gsz = rsamp + R, *koff = gsz + T, *slot_t = koff + T + 1, *has_prior = slot_t + K, *d_chunk_s = has_prior + S,
+        *d_chunk_n0 = d_chunk_s + NC, *schunk = d_chunk_n0 + NC, *pofs = schunk + S + 1, *first = pofs + K + 1, *modes = first + C,
+        *n_modes = modes + C, *d_max_seed = n_modes + 1, *map = d_max_seed + 1, *iters = map + n_seeds;
+    {   // one staging copy of the host-built int arrays (soff .. schunk are contiguous)
+        std::vector<int> h;
+        h.reserve((size_t)(schunk + S + 1 - soff));
+        h.insert(h.end(), sample_off, sample_off + S + 1);
+        h.insert(h.end(), rsamp_host.begin(), rsamp_host.end());
+        h.insert(h.end(), group_sizes, group_sizes + T);
+        h.insert(h.end(), koff_host.begin(), koff_host.end());
+        h.insert(h.end(), slot_host.begin(), slot_host.end());
+        h.insert(h.end(), has_prior_host.begin(), has_prior_host.end());
+        h.insert(h.end(), chunk_s.begin(), chunk_s.end());
+        h.insert(h.end(), chunk_n0.begin(), chunk_n0.end());
+        h.insert(h.end(), schunk_host.begin(), schunk_host.end());
+        CU(cudaMemcpyAsync(soff, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, e->stream));
+        CU(cudaMemsetAsync(bad, 0, sizeof(int), e->stream));
+        CU(cudaMemsetAsync(first, 0x7f, C * sizeof(int), e->stream));   // 0x7f7f7f7f: above every seed index
+        const size_t smem = (size_t)H * sizeof(int);
+        if (smem > 48 * 1024) CU(cudaFuncSetAttribute(phmm::vb::k_vb_index, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        phmm::vb::k_vb_index<<<K, 256, smem, e->stream>>>(d_gt, C, K, H, cnt, start, kh, nk, L, sid, bad);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        // the occurring (slot, haplotype) pairs; their count, at most K min(H, C), stays on the device (pofs[K])
+        const long long Pmax = (long long)K * std::min(H, C);
+        CU(e->mm_pairs.ensure((size_t)(2 * Pmax) * sizeof(int)));
+        int *pj = e->mm_pairs.as<int>(), *ph = pj + Pmax;
+        k_vbmm_pairs<<<1, 256, 0, e->stream>>>(bad, nk, kh, K, H, pofs, pj, ph);
+        LAUNCHED();
+
+        // doubles: lpost [n_seeds][C]; ev [n_seeds]; gconc [n_seeds][T]; mconc [n_seeds][S][K]; sigma [n_seeds][S][T]; weights [C]; keys [C] (u64)
+        const long long n_dbl = (long long)n_seeds * C + n_seeds + (long long)n_seeds * (T + SK + ST) + 2LL * C;
+        CU(e->mm_seed.ensure((size_t)n_dbl * sizeof(double)));
+        double* dp = e->mm_seed.as<double>();
+        double *lpost = dp, *ev = lpost + (long long)n_seeds * C, *seed_gconc = ev + n_seeds, *seed_mconc = seed_gconc + (long long)n_seeds * T,
+               *seed_sigma = seed_mconc + n_seeds * SK, *weights = seed_sigma + n_seeds * ST, *keys = weights + C;
+        CU(cudaMemsetAsync(keys, 0, C * sizeof(double), e->stream));
+
+        const long long ws = Workspace::doubles(H, R, S, C, K, T, (int)Pmax, NC);
+        const long long by_budget = std::max<long long>(1, (long long)(kVbWorkspaceBudget / sizeof(double)) / ws);
+        const int blocks = (int)std::min<long long>({(long long)n_seeds, 2LL * std::max(1, e->sm_count), by_budget});
+        CU(e->mm_ws.ensure((size_t)blocks * ws * sizeof(double)));
+        Args a{d_lnl, H, R, S, C, K, T, maxK, n_seeds, soff, rsamp, gsz, koff, slot_t, d_gt, d_lp, d_seeds, d_gprior, has_prior, d_gc0, d_mc0,
+               epsilon, max_iterations, cnt, start, kh, nk, L, sid, bad, pofs, pj, ph, 0, (int)Pmax, d_chunk_s, d_chunk_n0, schunk, NC,
+               e->mm_ws.as<double>(), ws, lpost, ev, iters, map, seed_gconc, seed_mconc, seed_sigma};
+        k_vbmm_seeds<<<blocks, kThreads, 0, e->stream>>>(a);
+        LAUNCHED();
+        const unsigned seed_grid = (unsigned)((n_seeds + 255) / 256), c_grid = (unsigned)((C + 255) / 256);
+        unsigned long long* ukeys = reinterpret_cast<unsigned long long*>(keys);
+        phmm::vb::k_vb_mode_max<<<seed_grid, 256, 0, e->stream>>>(bad, ev, map, n_seeds, ukeys);
+        phmm::vb::k_vb_mode_first<<<seed_grid, 256, 0, e->stream>>>(bad, ev, map, n_seeds, ukeys, first);
+        phmm::vb::k_vb_modes_compact<<<1, kFinishThreads, 0, e->stream>>>(bad, ev, n_seeds, first, C, modes, weights, n_modes, d_max_seed);
+        LAUNCHED(); LAUNCHED(); LAUNCHED();
+
+        double *o_post = posteriors, *o_lpost = log_posteriors, *o_w = weighted_posteriors, *o_gc = group_concentrations_out,
+               *o_mc = mixture_concentrations_out, *o_sg = group_responsibilities, *o_wsg = weighted_group_responsibilities, *o_mev = max_log_evidence;
+        int* o_ms = max_seed;
+        if (space == PHMM_SPACE_HOST) {
+            CU(e->mm_out.ensure((3 * (size_t)C + T + SK + 2 * ST + 2) * sizeof(double)));
+            o_post = e->mm_out.as<double>(); o_lpost = o_post + C; o_w = o_lpost + C; o_gc = o_w + C; o_mc = o_gc + T; o_sg = o_mc + SK;
+            o_wsg = o_sg + ST; o_mev = o_wsg + ST; o_ms = reinterpret_cast<int*>(o_mev + 1);
+        }
+        phmm::vb::k_vb_weighted<<<c_grid, 256, 0, e->stream>>>(bad, lpost, C, modes, weights, n_modes, d_max_seed, o_w, o_post, o_lpost);
+        k_vbmm_finish<<<1, kFinishThreads, 0, e->stream>>>(bad, C, S, T, K, o_w, modes, weights, n_modes, d_max_seed, ev, seed_gconc, seed_mconc,
+                                                           seed_sigma, o_gc, o_mc, o_sg, o_wsg, o_mev, o_ms);
+        LAUNCHED(); LAUNCHED();
+        CU(cudaGetLastError());
+        const cudaMemcpyKind out_kind = space == PHMM_SPACE_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+        if (seed_log_evidence) CU(cudaMemcpyAsync(seed_log_evidence, ev, n_seeds * sizeof(double), out_kind, e->stream));
+        if (seed_iterations) CU(cudaMemcpyAsync(seed_iterations, iters, n_seeds * sizeof(int), out_kind, e->stream));
+        if (space == PHMM_SPACE_HOST) {
+            CU(cudaMemcpyAsync(posteriors, o_post, C * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaMemcpyAsync(log_posteriors, o_lpost, C * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaMemcpyAsync(weighted_posteriors, o_w, C * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaMemcpyAsync(group_concentrations_out, o_gc, T * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaMemcpyAsync(mixture_concentrations_out, o_mc, SK * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaMemcpyAsync(group_responsibilities, o_sg, ST * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaMemcpyAsync(weighted_group_responsibilities, o_wsg, ST * sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaMemcpyAsync(max_log_evidence, o_mev, sizeof(double), cudaMemcpyDeviceToHost, e->stream));
+            CU(cudaMemcpyAsync(max_seed, o_ms, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+        }
+        int bad_host = 0;
+        CU(cudaMemcpyAsync(&bad_host, bad, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaStreamSynchronize(e->stream));
+        if (bad_host) { e->err = "haplotype index out of range"; return PHMM_ERR_INVALID; }
+    }
     return PHMM_OK;
 }
 

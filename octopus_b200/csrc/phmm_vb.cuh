@@ -285,8 +285,10 @@ struct Shared {
 };
 
 // W[k][h] = sum of post over slot k's genotypes with haplotype h, in L's order: each thread sums a contiguous chunk of L; a
-// segment that crosses chunks is finished by the thread where it starts, adding the later chunks' heads in order.
-__device__ void rebuild_w(const Args& a, const Workspace& w, Shared& sh)
+// segment that crosses chunks is finished by the thread where it starts, adding the later chunks' heads in order. Also used by
+// phmm_vb_mm.cuh, whose arguments carry the same index fields (K slots, G genotypes) and whose workspace the same W and post.
+template <typename A, typename WS>
+__device__ void rebuild_w(const A& a, const WS& w, Shared& sh)
 {
     const long long NL = (long long)a.K * a.G;
     const long long chunk = (NL + blockDim.x - 1) / blockDim.x;
