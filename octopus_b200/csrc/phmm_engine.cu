@@ -810,8 +810,10 @@ int phmm_variational_bayes(phmm_engine* e, const double* lnl, int32_t H, int32_t
     const int blocks = (int)std::min<long long>({(long long)n_seeds, 2LL * std::max(1, e->sm_count), by_budget});
     CU(e->vb_ws.ensure((size_t)blocks * ws * sizeof(double)));
 
+    // The limit covers the kernel's static shared memory too, so the 48 KB default fails already at H = 12 288: it is set for every
+    // H, through the per-process high-water mark (only ever raised; another engine may be about to launch with more).
     const size_t smem = (size_t)H * sizeof(int);
-    if (smem > 48 * 1024) CU(cudaFuncSetAttribute(k_vb_index, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (int arc = fast_smem_attr(e, k_vb_index, smem)) return arc;
     k_vb_index<<<K, 256, smem, e->stream>>>(d_gt, G, K, H, cnt, start, kh, nk, L, sid, bad);
     LAUNCHED();
     Args a{d_lnl, H, R, S, G, K, n_seeds, soff, d_gt, d_prior, d_lp, d_seeds, epsilon, max_iterations,
@@ -952,7 +954,7 @@ int phmm_variational_bayes_mixture_mixture(phmm_engine* e, const double* lnl, in
         CU(cudaMemsetAsync(bad, 0, sizeof(int), e->stream));
         CU(cudaMemsetAsync(first, 0x7f, C * sizeof(int), e->stream));   // 0x7f7f7f7f: above every seed index
         const size_t smem = (size_t)H * sizeof(int);
-        if (smem > 48 * 1024) CU(cudaFuncSetAttribute(phmm::vb::k_vb_index, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if (int arc = fast_smem_attr(e, phmm::vb::k_vb_index, smem)) return arc;   // as in phmm_variational_bayes
         phmm::vb::k_vb_index<<<K, 256, smem, e->stream>>>(d_gt, C, K, H, cnt, start, kh, nk, L, sid, bad);
         LAUNCHED();
         CU(cudaGetLastError());

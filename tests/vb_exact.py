@@ -64,6 +64,8 @@ class _Problem:
         self.S = len(self.off) - 1
         self.H = self.L.shape[0]
         self.direct = direct
+        # per slot: the haplotypes that occur there, and each genotype's position among them (sums over the others are never read)
+        self.used = [np.unique(self.gt[:, k], return_inverse=True) for k in range(self.K)]
 
     def cols(self, s):
         return self.L[:, self.off[s]:self.off[s + 1]]
@@ -93,8 +95,8 @@ class _Problem:
             if self.direct:
                 r += np.array([np.sum(tau[k] * Ls[self.gt[g, k]]) for g in range(self.G)], dtype=LD)
             else:
-                M = Ls @ tau[k]
-                r += M[self.gt[:, k]]
+                used, at = self.used[k]
+                r += (Ls[used] @ tau[k])[at]
         return r
 
     def responsibilities(self, alphas, post):
@@ -197,12 +199,21 @@ def combine(seed_results):
                 weighted=weighted, max_log_evidence=ev[ms], max_seed=ms, modes=modes)
 
 
+def _reuse(free, forced, i):
+    """A seed's run without `forced` when it ran for exactly forced[i] iterations: forcing that count then changes no decision."""
+    if free is None or forced is None or free["seeds"][i]["iterations"] != int(forced[i]):
+        return None
+    return free["seeds"][i]
+
+
 def run(lnl, sample_off, genotypes, prior_alphas, genotype_log_priors, seeds, epsilon=0.05, max_iterations=1000, forced=None,
-        direct=False):
-    """The whole call. forced: None, or one iteration count per seed (e.g. the device's) to run each seed for exactly that long."""
+        direct=False, free=None):
+    """The whole call. forced: None, or one iteration count per seed (e.g. the device's) to run each seed for exactly that long.
+    free: this call's result without `forced`, whose seeds are reused where they ran for their forced count."""
     P = _Problem(lnl, sample_off, genotypes, prior_alphas, genotype_log_priors, direct)
     seeds = np.asarray(seeds, dtype=np.float64)
-    res = [run_seed(P, seeds[i], epsilon, max_iterations, None if forced is None else int(forced[i])) for i in range(len(seeds))]
+    res = [_reuse(free, forced, i) or run_seed(P, seeds[i], epsilon, max_iterations, None if forced is None else int(forced[i]))
+           for i in range(len(seeds))]
     out = combine(res)
     out["seeds"] = res
     return out

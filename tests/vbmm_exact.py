@@ -31,7 +31,7 @@ import functools
 import mpmath
 import numpy as np
 
-from vb_exact import LD, LOWEST, _lse, _xlogx, near_threshold  # noqa: F401  (near_threshold: re-exported for the tests)
+from vb_exact import LD, LOWEST, _lse, _reuse, _xlogx, near_threshold  # noqa: F401  (near_threshold: re-exported for the tests)
 
 NULL = LD(-10000)
 MIN_LOG_PRIOR = LD(np.log(np.finfo(np.float64).tiny))
@@ -83,6 +83,8 @@ class _Problem:
                     with np.errstate(divide="ignore"):
                         self.lprior[s] = np.where(gp[s] > 0, np.log(np.where(gp[s] > 0, gp[s], 1)).astype(LD), MIN_LOG_PRIOR).astype(LD)
         self.direct, self.quirk = direct, quirk
+        # per slot: the haplotypes that occur there, and each combination's position among them (as vb_exact._Problem.used)
+        self.used = [np.unique(self.gt[:, j], return_inverse=True) for j in range(self.K)]
 
     def cols(self, s):
         return self.L[:, self.off[s]:self.off[s + 1]]
@@ -126,7 +128,8 @@ class _Problem:
                     if self.direct:
                         acc += np.array([np.sum(taus[s][t][k] * Ls[self.gt[c, j]]) for c in range(self.C)], dtype=LD)
                     else:
-                        acc += (Ls @ taus[s][t][k])[self.gt[:, j]]
+                        used, at = self.used[j]
+                        acc += (Ls[used] @ taus[s][t][k])[at]
                 r += sigma[s][t] * acc
         return r
 
@@ -260,13 +263,15 @@ def combine(res):
 
 
 def run(lnl, sample_off, group_sizes, combinations, genotype_log_priors, group_concentrations, mixture_concentrations, seeds,
-        group_priors=None, group_prior_mask=None, epsilon=0.05, max_iterations=1000, forced=None, direct=False, quirk=True):
+        group_priors=None, group_prior_mask=None, epsilon=0.05, max_iterations=1000, forced=None, direct=False, quirk=True, free=None):
     """The whole call (concentrations already expanded: (T,) and (S, sum K)). forced: None, or one iteration count per seed (e.g.
-    the device's) to run each seed for exactly that long."""
+    the device's) to run each seed for exactly that long. free: this call's result without `forced`, whose seeds are reused where
+    they ran for their forced count (vb_exact._reuse)."""
     P = _Problem(lnl, sample_off, group_sizes, combinations, genotype_log_priors, group_concentrations, mixture_concentrations,
                  group_priors, group_prior_mask, direct, quirk)
     seeds = np.asarray(seeds, dtype=np.float64)
-    res = [run_seed(P, seeds[i], epsilon, max_iterations, None if forced is None else int(forced[i])) for i in range(len(seeds))]
+    res = [_reuse(free, forced, i) or run_seed(P, seeds[i], epsilon, max_iterations, None if forced is None else int(forced[i]))
+           for i in range(len(seeds))]
     out = combine(res)
     out["seeds"] = res
     return out
